@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- ICAFusion hot path on B200: 640x512 RGB+IR pairs/s end to end (+ roofline of the dominant kernel).
+"""bench.py -- ICAFusion hot path on H100: 640x512 RGB+IR pairs/s end to end (+ roofline of the dominant kernel).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload NAME]
 
@@ -15,10 +15,10 @@ every rank runs its own pairs, there is no collective on the inference path ("we
            between steps, max over ranks.
 `e2e`    : pairs/s through the reference-facing call with HOST (pinned, uint8) frames: H2D + forward + D2H of the
            decoded predictions inside the timed region.
-`roofline`: the tcgen05 implicit-GEMM conv kernels (every Conv / Linear / Detect GEMM of a step): algorithmic FLOPs of those
+`roofline`: the wgmma implicit-GEMM conv kernel (every Conv / Linear / Detect GEMM of a step): algorithmic FLOPs of those
            launches / the time they take INSIDE the timed step = ms_per_step x their share of the step's kernel time (the
-           share from a CUDA-event pass over one step on the launching stream; profiles/ holds the ncu launch list of the
-           same step for comparison), against the SUSTAINED tensor peak of MEASURED_PEAKS.json.
+           share from a CUDA-event pass over one step on the launching stream), against the sustained tensor peak of
+           MEASURED_PEAKS.json when that file exists, else the H100 SXM data-sheet figure.
 `cpu_baseline` / `--impl reference`: the oracle (fp32 PyTorch-CPU restatement of the reference forward; the reference
            itself is Python and cannot travel to the GPU box) timed on this host's cores at a FIXED intra-op thread count
            (32, or fewer if the host has fewer usable cores) so the two arms share one denominator.
@@ -55,7 +55,8 @@ def _peaks():
         return {"tensor": p.get("bf16_tflops_sustained", p["bf16_tflops"]), "tensor_burst": p["bf16_tflops"], "hbm": p["hbm_gbs"],
                 "src": "measured (MEASURED_PEAKS.json: bf16_tflops_sustained -- the kernels run inside a multi-ms step; hbm_gbs)"}
     except Exception:  # noqa: BLE001
-        return {"tensor": 1590.0, "tensor_burst": 1590.0, "hbm": 6650.0, "src": "fallback (B200_PROFILING.md)"}
+        # NVIDIA H100 SXM data sheet: dense FP16 tensor rate and HBM3 bandwidth at up to 700 W (a lower power limit lowers them)
+        return {"tensor": 989.0, "tensor_burst": 989.0, "hbm": 3350.0, "src": "H100 SXM data sheet (dense FP16, 700 W)"}
 
 
 class ClockSampler(threading.Thread):
@@ -116,9 +117,10 @@ CPU_THREADS = 32        # fixed intra-op thread count of the CPU arm: the fastes
                         # pool stops scaling on these convolutions beyond it: 47 s/pair at 128 threads); both arms use it -> one denominator
 
 
-def cpu_reference_throughput(wl, budget_s=20.0, max_pairs=64, warm=1):
+def cpu_reference_throughput(wl, budget_s=20.0, max_pairs=64, warm=1, dump_dir=None):
     """The reference's CPU path (oracle port: same torch CPU ops, fp32, fused BN) on the host cores; bounded sample:
-    batch-1 forwards of the workload's model until `max_pairs` pairs or `budget_s` seconds, median forward time."""
+    batch-1 forwards of the workload's model until `max_pairs` pairs or `budget_s` seconds (None: no time cap), median
+    forward time.  `dump_dir`: write the last timed forward's outputs there (dump_outputs)."""
     import torch
     from oracle import icaf_oracle as O
     from oracle import synth
@@ -131,14 +133,16 @@ def cpu_reference_throughput(wl, budget_s=20.0, max_pairs=64, warm=1):
     with torch.no_grad():
         for _ in range(max(1, warm)):
             O.model_forward(sd, cfg, rgb, ir)
-        t0, n, times = time.perf_counter(), 0, []
-        while n < max_pairs and (time.perf_counter() - t0) < budget_s:
+        t0, n, times, out = time.perf_counter(), 0, [], None
+        while n < max_pairs and (budget_s is None or (time.perf_counter() - t0) < budget_s):
             t = time.perf_counter()
-            O.model_forward(sd, cfg, rgb, ir)
+            out = O.model_forward(sd, cfg, rgb, ir)
             times.append(time.perf_counter() - t)
             n += B
+    if dump_dir:
+        dump_outputs(dump_dir, *out)
     per = sorted(times)[len(times) // 2]
-    return {"value": round(B / per, 3), "unit": "pairs/s", "cores": nt, "kind": "port",
+    return {"value": round(B / per, 3), "unit": "pairs/s", "cores": nt, "kind": "port", "pairs_timed": n,
             "sample": f"{n} pairs of {wl['desc'].split(',')[0]} at batch 1, fp32, median of {len(times)} forwards "
                       f"({sum(times):.1f} s of CPU work) on {nt} intra-op threads (fixed; {usable} usable cores); "
                       "oracle/icaf_oracle.py (PyTorch-CPU restatement of the reference forward)",
@@ -161,16 +165,45 @@ def run_reference(args, wl):
     if rank != 0:
         return
     steps = max(1, args.steps)
-    # one "step" of this arm = one pair of the workload (a bounded sample of its batch); W warm-up pairs, K timed pairs, capped at 90 s
-    cb = cpu_reference_throughput(wl, budget_s=90.0, max_pairs=steps, warm=max(1, min(args.warmup, 3)))
+    # one "step" of this arm = one pair of the workload (a bounded sample of its batch); W warm-up pairs, then exactly K timed pairs
+    cb = cpu_reference_throughput(wl, budget_s=None, max_pairs=steps, warm=args.warmup, dump_dir=args.dump_outputs)
     line = {"impl": "reference", "metric": METRIC, "value": cb["value"], "unit": "pairs/s", "n_gpus": args.gpus, "steps": steps,
             "warmup": args.warmup, "ms_per_step": round(1000.0 / cb["value"], 3), "higher_is_better": True, "scaling": "weak",
             "vs_baseline": None, "dtype": "f32", "data": "synthetic",
-            "config": {"workload": wl["desc"], "note": "reference forward restated with the same PyTorch CPU ops (oracle port); "
-                                                       "the Python reference cannot travel to the GPU box"},
+            "config": {"workload": wl["desc"], "note": "reference forward restated with the same PyTorch CPU ops (oracle port), "
+                                                       "batch 1"},
             "cpu_baseline": cb,
             "e2e": {"value": cb["value"], "unit": "pairs/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0}}
     print(json.dumps(line))
+
+
+DUMP_BUDGET = 64 << 20      # bytes of .npy data --dump-outputs may write in all
+
+
+def dump_outputs(out_dir, z, logits, xs):
+    """What a timed forward computed, as its caller receives it (`z, logits, xs = model(rgb, ir)`): the decoded predictions
+    `pred` (B, anchors, 6), the class logits `logits` (B, anchors, nc) and the raw head maps `head_<i>` (B, 3, H, W, 6), as
+    float32 .npy files.  An array that would overrun the 64 MiB budget is replaced by a fixed, seeded sample of its
+    flattened values (`<name>_sample_idx.npy` holds the indices), so two builds given the same arguments can be compared
+    output for output."""
+    import numpy as np
+    import torch
+    if torch.cuda.is_available():
+        torch.cuda.synchronize()
+    os.makedirs(out_dir, exist_ok=True)
+    xs = [xs] if torch.is_tensor(xs) else list(xs)
+    arrays = [("pred", z), ("logits", logits)] + [(f"head_{i}", x) for i, x in enumerate(xs)]
+    left = DUMP_BUDGET
+    for name, t in arrays:
+        a = t.detach().float().cpu().numpy()
+        if a.nbytes > left // 2:
+            n = max(1, (left // 2) // 12)                 # 4 bytes of value + 8 bytes of index per sampled element
+            idx = np.sort(np.random.default_rng(0).choice(a.size, size=min(n, a.size), replace=False))
+            np.save(os.path.join(out_dir, f"{name}_sample_idx.npy"), idx)
+            a = a.reshape(-1)[idx]
+            left -= idx.nbytes
+        np.save(os.path.join(out_dir, f"{name}.npy"), a)
+        left -= a.nbytes
 
 
 def _measure(args, wl, K, Wm, dev, world, rank, local, primary=True):
@@ -191,7 +224,7 @@ def _measure(args, wl, K, Wm, dev, world, rank, local, primary=True):
     rgb_pin, ir_pin = rgb_u8.pin_memory(), ir_u8.pin_memory()
     eng.rgb.copy_(rgb_u8)
     eng.ir.copy_(ir_u8)
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)      # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)      # > 50 MB L2
 
     def barrier():
         if world > 1:
@@ -214,6 +247,8 @@ def _measure(args, wl, K, Wm, dev, world, rank, local, primary=True):
     barrier()
     t_wall = time.perf_counter() - t_wall
     dev_ms = sum(s.elapsed_time(e) for s, e in ev)
+    if primary and rank == 0 and args.dump_outputs:
+        dump_outputs(args.dump_outputs, eng.z, eng.logits, eng.xs)
     # ---------------- end-to-end timing through the public streaming call with host frames ----------------------
     # PipelinedDetector.infer_stream: per frame H2D (pinned uint8) -> forward -> D2H of the decoded predictions; the copy
     # of frame i+1 overlaps the forward of frame i (depth-2), the host blocks on the oldest frame in flight.
@@ -329,7 +364,7 @@ def _measure(args, wl, K, Wm, dev, world, rank, local, primary=True):
     conv_ms_in_step = step_ms * share
     conv_flops_step = conv["flops"] / reps
     ach = conv_flops_step / (conv_ms_in_step * 1e-3) / 1e12 if conv_ms_in_step > 0 else 0.0
-    roofline = {"kernel": "icaf_conv2d_fwd = conv_gemm_{tc,persist,pair}_kernel (every Conv/Linear/Detect GEMM of a step)", "bound": "tensor",
+    roofline = {"kernel": "icaf_conv2d_fwd = conv_gemm_tc_kernel (every Conv/Linear/Detect GEMM of a step)", "bound": "tensor",
                 "achieved": round(ach, 3), "peak": pk["tensor"], "unit": "TFLOP/s", "frac": round(ach / pk["tensor"], 5),
                 "traffic": traffic, "traffic_source": traffic_src,
                 "algorithmic_flops_per_launch": round(conv_flops_step / max(1, conv_launches)),
@@ -642,9 +677,14 @@ def main():
     ap.add_argument("--train", default="on", choices=["on", "off"], help="also time the training step of the workload's model (reported "
                     "under 'train'; with N > 1 it runs under DDP and names the gradient all-reduce's share)")
     ap.add_argument("--train-steps", type=int, default=10)
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR", help="after the timed steps, write what the last timed step "
+                    "computed (predictions, class logits and head maps of the primary workload's forward; with --impl reference "
+                    "those of the last timed CPU forward) to DIR/<name>.npy as float32, 64 MiB at most; inference only")
     ap.add_argument("--mode", default="infer", choices=["infer", "train"], help="train: the JSON line's top-level metric is the training "
                     "step (BASELINE configs[3]; under torchrun it is the DDP step with its gradient all-reduce) instead of inference")
     args = ap.parse_args()
+    if args.dump_outputs and args.mode == "train":
+        ap.error("--dump-outputs writes the outputs of the inference forward; it cannot be combined with --mode train")
     wl = WORKLOADS[args.workload]
     if args.impl == "reference":
         run_reference(args, wl)

@@ -1,4 +1,4 @@
-"""icafusion_b200 -- B200 (sm_100a) native implementation of the ICAFusion hot path:
+"""icafusion_b200 -- H100 (sm_90a) native implementation of the ICAFusion hot path:
 two-stream CSPDarknet Conv+BN+SiLU backbone + DMFF cross-attention fusion + Detect head.
 
     from icafusion_b200 import Model

@@ -40,7 +40,7 @@ class LossHyp(C.Structure):
                [("balance", C.c_float * 5)]
 
 
-KERNEL_TC, KERNEL_PERSIST, KERNEL_PAIR, KERNEL_STEM = 0, 1, 2, 3
+KERNEL_TC = 0
 
 _vp, _i, _i64, _f = C.c_void_p, C.c_int, C.c_int64, C.c_float
 # name -> argtypes; every symbol include/icaf_b200.h declares (tests check the .so exports them all)

@@ -1,4 +1,4 @@
-"""Build libicaf_b200.so in-tree with nvcc for sm_100a (cross-compiles without a GPU).
+"""Build libicaf_b200.so in-tree with nvcc for sm_90a (cross-compiles without a GPU).
 
     python -m icafusion_b200.build [--force]
 """
@@ -12,9 +12,9 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libicaf_b200.so")
-SOURCES = ["api.cu", "conv_gemm.cu", "conv_persist.cu", "conv_pair.cu", "attn.cu", "aux.cu", "loss.cu", "conv_stem.cu", "wgrad.cu", "train.cu", "attn_bwd.cu", "dmff_bwd.cu"]
+SOURCES = ["api.cu", "conv_gemm.cu", "attn.cu", "aux.cu", "loss.cu", "wgrad.cu", "train.cu", "attn_bwd.cu", "dmff_bwd.cu"]
 HEADERS = ["ptx.cuh", "icaf_internal.cuh", "conv_common.cuh", os.path.join("..", "..", "include", "icaf_b200.h")]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "--use_fast_math=false"]
 
 
@@ -39,8 +39,6 @@ def build(force: bool = False, verbose: bool = False) -> str:
     nvcc = _nvcc()
     objs = []
     flags = [f for f in NVCC_FLAGS if not f.startswith("--use_fast_math")]
-    if os.environ.get("ICAF_PROBE") == "1":      # diagnostic build for tools/conv_probe.py (stage switches in the conv kernels)
-        flags.append("-DICAF_PROBE")
     procs = []
     for s in SOURCES:
         obj = os.path.join(CSRC, s[:-3] + ".o")
@@ -55,7 +53,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
             print(out)
         if p.returncode:
             raise RuntimeError(f"nvcc failed on {s}")
-    cmd = [nvcc, "-shared", "-o", LIB, *objs, "-lcudart"]
+    cmd = [nvcc, *NVCC_FLAGS[:2], "-shared", "-o", LIB, *objs, "-lcudart"]
     subprocess.check_call(cmd)
     return LIB
 

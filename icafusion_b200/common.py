@@ -3,7 +3,7 @@
 Same class names, constructor signatures, sub-module / parameter names and ``state_dict`` keys as the
 reference, so reference checkpoints load with ``strict=True`` and ``models/yolo_test.py``-style graph
 builders can ``eval()`` these names.  The ``forward`` bodies do not call PyTorch operators: they
-marshal tensors into libicaf_b200.so (hand-written sm_100a kernels, see include/icaf_b200.h).
+marshal tensors into libicaf_b200.so (hand-written sm_90a kernels, see include/icaf_b200.h).
 
 Data layout: modules accept logical (B,C,H,W) tensors like the reference; internally everything is
 fp16 NHWC, which is exactly torch's ``channels_last`` memory format, so consecutive modules exchange

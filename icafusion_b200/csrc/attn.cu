@@ -1,12 +1,13 @@
-// Bidirectional DMFF cross-attention core (models/common.py:670-684) as a flash-style tcgen05 kernel:
+// Bidirectional DMFF cross-attention core (models/common.py:670-684) as a flash-style wgmma kernel:
 //   out_vis = softmax(q_ir k_vis^T / sqrt(d)) v_vis        out_ir = softmax(q_vis k_ir^T / sqrt(d)) v_ir
-// The N x N score matrix never leaves the SM: S = Q K^T is produced by the tensor core into TMEM, the 128
-// softmax threads (one per query row == TMEM lane) run the online softmax straight out of TMEM, write P (fp16)
-// into 128B-swizzled shared memory, and a second UMMA computes P V into TMEM; running (max, sum, acc) live in
-// registers.  Q / K / V^T tiles are staged by TMA (cp.async.bulk.tensor) from a producer warp, K / V^T double-buffered.
+// The N x N score matrix never leaves the SM: each of two consumer warpgroups owns 64 query rows, computes S = Q K^T
+// into registers (wgmma, both operands in shared memory), runs the online softmax on the accumulator fragments, packs P
+// to fp16 in registers and feeds it straight back as the A operand of O += P V (wgmma with a register A operand); running
+// (max, sum, O) live in registers.  Q / K / V tiles are staged by TMA (cp.async.bulk.tensor) from a producer warp, K / V
+// double-buffered.
 //
 // Layouts (see include/icaf_b200.h): either qkv (B, Npad, 3C) = [q | k | v] rows as ONE fused projection emits them (V is
-// then consumed as an MN-major UMMA operand straight from its token-major tile), or qk (B, Npad, 2C) + vt (C, B*Npad) = V^T
+// then consumed as an MN-major operand straight from its token-major tile), or qk (B, Npad, 2C) + vt (C, B*Npad) = V^T
 // (K-major); out (B, Npad, C).
 // CTA = (128-query tile, batch*head, direction).
 #include <cmath>
@@ -17,7 +18,7 @@
 
 namespace icaf {
 
-constexpr int kQT = 128;    // queries per CTA (UMMA M)
+constexpr int kQT = 128;    // queries per CTA (two warpgroups x 64 rows)
 
 struct AttnParams {
   const __half* qk[2];   // [0]=vis, [1]=ir
@@ -32,11 +33,7 @@ struct AttnParams {
 };
 
 // ---------------------------------------------------------------------------------------------------
-// The kernel: Q / K / V^T tiles arrive by cp.async.bulk.tensor issued from a dedicated producer warp,
-// so the 128 softmax threads do nothing but softmax; two CTAs share an SM for head dims <= 64 (one CTA's softmax overlaps
-// the other's MMAs and loads -- with a single CTA every SM sub-partition holds exactly one softmax warp and every TMEM /
-// MUFU latency is exposed).  192 threads: warps 0-3 softmax (thread = query row = TMEM lane), warp 4 TMEM + MMA issue,
-// warp 5 TMA producer.
+// 288 threads: warps 0-7 two consumer warpgroups (queries 0-63 / 64-127 of the tile), warp 8 TMA producer.
 //   Q / K tiles: 2-D boxes (min(D,64) columns x 128 token rows) of the (B*Npad, 2C) projection matrix -> K-major rows of
 //                32 / 64 / 128 bytes with the matching swizzle (D = 128: two 64-column blocks)
 //   V^T tiles  : two boxes (64 keys x D feature rows) of the (C, B*Npad) matrix -> K-major SW128 (keys are the K dim of PV)
@@ -48,13 +45,10 @@ struct AttnMaps {
   CUtensorMap vt[2];   // split form: (C rows, B*Npad cols), box (64, D)
 };
 
-// KV = keys per tile (UMMA N of S, K of PV).  Head dims 16 / 32 run 64-key tiles: S + O then fit 128 TMEM columns and the
-// small tiles let 4 / 3 CTAs share an SM -- these head dims are exp-bound, and with one or two CTAs per SM every TMEM load,
-// MUFU and barrier latency of the single softmax warp per sub-partition is exposed (probe: profiles/r02_attn_probe_*).
+// KV = keys per tile (N of S, K of PV).  Head dims 16 / 32 run 64-key tiles (less masked work at the DMFF token counts).
 template <int D>
 struct AttnCfg {
   static constexpr int kKV = D <= 32 ? 64 : 128;
-  static constexpr int kCtas = D == 16 ? 4 : (D == 32 ? 3 : (D == 64 ? 2 : 1));
 };
 
 template <int D, int KV>
@@ -64,17 +58,11 @@ struct AttnSmemT {
   static constexpr int kQBytes = kKB * kQT * kRowB;
   static constexpr int kKBytes = kKB * KV * kRowB;          // per buffer
   static constexpr int kVBytes = (KV / 64) * D * 128;       // per buffer: 64-key blocks of D rows (= KV rows of D halfs)
-  static constexpr int kPBytes = (KV / 64) * kQT * 128;
   static constexpr int kQOff = 0;
   static constexpr int kKOff = kQOff + kQBytes;
   static constexpr int kVOff = kKOff + 2 * kKBytes;
-  static constexpr int kPOff = kVOff + 2 * kVBytes;
-  static constexpr int kBarOff = kPOff + kPBytes;
-  static constexpr int kCtas = AttnCfg<D>::kCtas;           // CTAs per SM
-  // two CTAs of the D = 64 variant fill the SM to the byte: no alignment slack (the kernel checks its base is 1024-aligned)
-  static constexpr bool kSlack = (kBarOff + 128 + 1024) * kCtas + kCtas * 1024 <= 228 * 1024;
-  static constexpr int kTotal = kBarOff + 128 + (kSlack ? 1024 : 0);
-  static constexpr int kTmemCols = KV + D <= 128 ? 128 : 256;   // S (KV) + O (D)
+  static constexpr int kBarOff = kVOff + 2 * kVBytes;
+  static constexpr int kTotal = kBarOff + 128 + 1024;       // + alignment slack
   static_assert(kQBytes % 1024 == 0 && kKBytes % 1024 == 0 && kVBytes % 1024 == 0, "tiles must keep 1024-byte alignment");
 };
 
@@ -87,17 +75,15 @@ __device__ __forceinline__ float fast_exp2_t(float x) {
 // TRAIN: dropout on the attention probabilities (the row sum still runs over the un-dropped values, like
 // `att = softmax(..); att = attn_drop(att)`); its own instantiation, so the inference kernels keep their size.
 template <int D, bool VF, bool TRAIN = false>
-__global__ void __launch_bounds__(192, AttnCfg<D>::kCtas) cross_attn_tma_kernel(const AttnParams P, const __grid_constant__ AttnMaps M) {
+__global__ void __launch_bounds__(288, 1) cross_attn_tma_kernel(const AttnParams P, const __grid_constant__ AttnMaps M) {
   constexpr int kKV = AttnCfg<D>::kKV;
   using L = AttnSmemT<D, kKV>;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  const uint32_t sbase = L::kSlack ? ((smem_u32(smem_raw) + 1023u) & ~1023u) : smem_u32(smem_raw);
-  uint8_t* sgen = smem_raw + (sbase - smem_u32(smem_raw));
+  const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t bar = sbase + L::kBarOff;
-  const uint32_t q_full = bar, s_full = bar + 8, p_full = bar + 16, o_full = bar + 24;
+  const uint32_t q_full = bar;
   auto kv_full = [&](int i) { return bar + 32u + 8u * i; };
   auto kv_empty = [&](int i) { return bar + 48u + 8u * i; };
-  const uint32_t tmem_slot = bar + 64;
 
   pdl_launch_dependents();
   const int tid = threadIdx.x, warp = tid >> 5;
@@ -108,187 +94,117 @@ __global__ void __launch_bounds__(192, AttnCfg<D>::kCtas) cross_attn_tma_kernel(
   const int nkv = (N + kKV - 1) / kKV;
 
   if (tid == 0) {
-    if (!L::kSlack && (sbase & 1023u)) {
-      printf("icaf: cross_attn_tma_kernel<%d>: dynamic shared memory base 0x%x is not 1024-byte aligned\n", D, sbase);
-      __trap();
-    }
-    mbar_init(q_full, 1); mbar_init(s_full, 1); mbar_init(p_full, 128); mbar_init(o_full, 1);
+    mbar_init(q_full, 1);
     mbar_init(kv_full(0), 1); mbar_init(kv_full(1), 1);
-    mbar_init(kv_empty(0), 1); mbar_init(kv_empty(1), 1);
+    mbar_init(kv_empty(0), 8); mbar_init(kv_empty(1), 8);      // one arrival per consumer warp
     fence_mbar_init();
   }
-  if (warp == 4) tmem_alloc<L::kTmemCols>(tmem_slot);
-  if (warp == 5 && lane_id() == 0) {
+  if (warp == 8 && lane_id() == 0) {
     tma_prefetch_desc(dir == 0 ? &M.qk[1] : &M.qk[0]);
     tma_prefetch_desc(dir == 0 ? &M.kv[0] : &M.kv[1]);
     if (!VF) tma_prefetch_desc(dir == 0 ? &M.vt[0] : &M.vt[1]);
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
   pdl_wait();           // everything above overlapped the previous kernel's tail; q/k/v are its outputs
-  const uint32_t tmem = *reinterpret_cast<volatile uint32_t*>(sgen + L::kBarOff + 64);
-  const uint32_t tmem_S = tmem, tmem_O = tmem + kKV;
 
-  if (warp < 4) {
-    // ------------------------------------------------------------------ online softmax (TMEM lanes = query rows)
-    const int row = tid;
-    const int qn = q0 + row;
-    const uint32_t lane_off = uint32_t(warp * 32) << 16;
+  if (warp < 8) {
+    // ------------------------------------------------------------------ consumer warpgroup g: query rows 64g .. 64g+63
+    const int g = warp >> 2, w = warp & 3, l = tid & 31;
+    const int r_lo = 64 * g + 16 * w + (l >> 2);              // this thread's two rows: r_lo, r_lo + 8
+    const int qn0 = q0 + r_lo, qn1 = qn0 + 8;
     const float sl2 = P.scale_log2;
-    float m_run = -INFINITY, l_run = 0.f;
-    float acc[D];
+    const uint32_t seed = TRAIN ? P.seed + (P.seed_off ? __ldg(P.seed_off) : 0u) : 0u;
+    float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+    float o[D / 2];
 #pragma unroll
-    for (int i = 0; i < D; ++i) acc[i] = 0.f;
-    uint8_t* prow0 = sgen + L::kPOff + row * 128;
-    const int rsw = row & 7;
-
-    for (int j = 0; j < nkv; ++j) {
-      const int kv0 = j * kKV;
-      const bool full = kv0 + kKV <= N;       // every key of the tile is valid: no masking
-      mbar_wait(s_full, j & 1);
-      tc_fence_after();
-      float mx = -INFINITY;
-#pragma unroll 1
-      for (int cb = 0; cb < kKV; cb += 32) {
-        uint32_t r[32];
-        __syncwarp();
-        tmem_ld32(tmem_S + lane_off + cb, r);
-        tmem_ld_wait();
-        if (full) {
-#pragma unroll
-          for (int i = 0; i < 32; ++i) mx = fmaxf(mx, __uint_as_float(r[i]));
-        } else {
-#pragma unroll
-          for (int i = 0; i < 32; ++i)
-            if (kv0 + cb + i < N) mx = fmaxf(mx, __uint_as_float(r[i]));
-        }
-      }
-      const float m_new = fmaxf(m_run, mx);               // finite: every tile has >= 1 valid key
-      const float corr = fast_exp2_t((m_run - m_new) * sl2);
-      const float moff = m_new * sl2;
-      float rs = 0.f;
-#pragma unroll 1
-      for (int cb = 0; cb < kKV; cb += 32) {
-        uint32_t r[32];
-        __syncwarp();
-        tmem_ld32(tmem_S + lane_off + cb, r);
-        tmem_ld_wait();
-        uint32_t pk[16];
-        if (full) {
-#pragma unroll
-          for (int i = 0; i < 32; i += 2) {
-            const float p0 = fast_exp2_t(fmaf(__uint_as_float(r[i]), sl2, -moff));
-            const float p1 = fast_exp2_t(fmaf(__uint_as_float(r[i + 1]), sl2, -moff));
-            __half2 h = __floats2half2_rn(p0, p1);
-            const float2 hf = __half22float2(h);            // sum what the PV MMA will actually see
-            rs += hf.x + hf.y;
-            if (TRAIN) {
-              const float ks = 1.f / (1.f - P.p_drop);
-              const bool k0 = attn_keep(P.seed + (P.seed_off ? __ldg(P.seed_off) : 0u), dir, blockIdx.y, qn, kv0 + cb + i, P.p_drop), k1 = attn_keep(P.seed + (P.seed_off ? __ldg(P.seed_off) : 0u), dir, blockIdx.y, qn, kv0 + cb + i + 1, P.p_drop);
-              h = __floats2half2_rn(k0 ? hf.x * ks : 0.f, k1 ? hf.y * ks : 0.f);
-            }
-            pk[i >> 1] = *reinterpret_cast<const uint32_t*>(&h);
-          }
-        } else {
-#pragma unroll
-          for (int i = 0; i < 32; i += 2) {
-            const float p0 = (kv0 + cb + i < N) ? fast_exp2_t(fmaf(__uint_as_float(r[i]), sl2, -moff)) : 0.f;
-            const float p1 = (kv0 + cb + i + 1 < N) ? fast_exp2_t(fmaf(__uint_as_float(r[i + 1]), sl2, -moff)) : 0.f;
-            __half2 h = __floats2half2_rn(p0, p1);
-            const float2 hf = __half22float2(h);
-            rs += hf.x + hf.y;
-            if (TRAIN) {
-              const float ks = 1.f / (1.f - P.p_drop);
-              const bool k0 = attn_keep(P.seed + (P.seed_off ? __ldg(P.seed_off) : 0u), dir, blockIdx.y, qn, kv0 + cb + i, P.p_drop), k1 = attn_keep(P.seed + (P.seed_off ? __ldg(P.seed_off) : 0u), dir, blockIdx.y, qn, kv0 + cb + i + 1, P.p_drop);
-              h = __floats2half2_rn(k0 ? hf.x * ks : 0.f, k1 ? hf.y * ks : 0.f);
-            }
-            pk[i >> 1] = *reinterpret_cast<const uint32_t*>(&h);
-          }
-        }
-        // P row -> K-major SW128 smem (block = cb/64, 16-byte chunks (cb%64)/8 ..)
-        uint8_t* prow = prow0 + (cb >> 6) * (kQT * 128);
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          const int c = ((cb & 63) >> 3) + q;
-          *reinterpret_cast<uint4*>(prow + ((c ^ rsw) << 4)) = make_uint4(pk[4 * q], pk[4 * q + 1], pk[4 * q + 2], pk[4 * q + 3]);
-        }
-      }
-      l_run = l_run * corr + rs;
-      m_run = m_new;
-      fence_proxy_async_smem();
-      tc_fence_before();
-      mbar_arrive(p_full);
-      // ---- O_tile = P V ; fold into the running accumulator ----
-      mbar_wait(o_full, j & 1);
-      tc_fence_after();
-#pragma unroll
-      for (int cb = 0; cb < D; cb += 32) {
-        if (D - cb >= 32) {
-          uint32_t r[32];
-          __syncwarp();
-          tmem_ld32(tmem_O + lane_off + cb, r);
-          tmem_ld_wait();
-#pragma unroll
-          for (int i = 0; i < 32; ++i) acc[cb + i] = fmaf(acc[cb + i], corr, __uint_as_float(r[i]));
-        } else {
-          uint32_t r[16];
-          __syncwarp();
-          tmem_ld16(tmem_O + lane_off + cb, r);
-          tmem_ld_wait();
-#pragma unroll
-          for (int i = 0; i < 16; ++i) acc[cb + i] = fmaf(acc[cb + i], corr, __uint_as_float(r[i]));
-        }
-      }
-      tc_fence_before();
-    }
-    // ---- normalise and store (heads merged: column head*D) ; zero the pad rows ----
-    if (qn < n_pad) {
-      const float inv = qn < N ? 1.f / l_run : 0.f;
-      __half* o = (dir == 0 ? P.out[0] : P.out[1]) + (size_t(b) * n_pad + qn) * C + head * D;
-#pragma unroll
-      for (int i = 0; i < D; i += 8) {
-        uint4 v;
-        v.x = pack_half2(acc[i] * inv, acc[i + 1] * inv);
-        v.y = pack_half2(acc[i + 2] * inv, acc[i + 3] * inv);
-        v.z = pack_half2(acc[i + 4] * inv, acc[i + 5] * inv);
-        v.w = pack_half2(acc[i + 6] * inv, acc[i + 7] * inv);
-        *reinterpret_cast<uint4*>(o + i) = v;
-      }
-    }
-  } else if (warp == 4) {
-    // ------------------------------------------------------------------ MMA issuer
-    constexpr uint32_t idesc_s = umma_idesc_f16(kQT, kKV);
-    constexpr uint32_t idesc_o = umma_idesc_f16_major(kQT, D, false, VF);      // VF: V tile is MN-major (rows = keys)
+    for (int i = 0; i < D / 2; ++i) o[i] = 0.f;
     mbar_wait(q_full, 0);
     for (int j = 0; j < nkv; ++j) {
       const int buf = j & 1;
+      const int kv0 = j * kKV;
       mbar_wait(kv_full(buf), (j >> 1) & 1);
-      tc_fence_after();
-      if (elect_one()) {
+      // ---- S = Q K^T (64 x KV per warpgroup) ----
+      float s[kKV / 2];
+      wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < D / 16; ++k) {
-          const uint64_t ad = umma_desc_kmajor(sbase + L::kQOff + (k >> 2) * (kQT * 128) + (k & 3) * 32, L::kRowB);
-          const uint64_t bd = umma_desc_kmajor(sbase + L::kKOff + buf * L::kKBytes + (k >> 2) * (kKV * 128) + (k & 3) * 32, L::kRowB);
-          umma_f16_ss(tmem_S, ad, bd, idesc_s, k != 0);
-        }
-        umma_commit(s_full);
+      for (int k = 0; k < D / 16; ++k) {
+        const uint64_t ad = gmma_desc_kmajor(sbase + L::kQOff + (k >> 2) * (kQT * 128) + 64 * g * L::kRowB + (k & 3) * 32, L::kRowB);
+        const uint64_t bd = gmma_desc_kmajor(sbase + L::kKOff + buf * L::kKBytes + (k >> 2) * (kKV * 128) + (k & 3) * 32, L::kRowB);
+        wgmma_ss<0, 0>(s, ad, bd, k != 0);
       }
-      __syncwarp();
-      mbar_wait(p_full, j & 1);
-      tc_fence_after();
-      if (elect_one()) {
+      wgmma_commit();
+      wgmma_wait<0>();
+      // ---- online softmax on the fragments: s[i] is row r_lo + 8*((i>>1)&1), key kv0 + 8*(i>>2) + 2*(l&3) + (i&1) ----
+      const bool full = kv0 + kKV <= N;       // every key of the tile is valid: no masking
+      if (!full) {
 #pragma unroll
-        for (int k = 0; k < kKV / 16; ++k) {
-          const uint64_t ad = umma_desc_sw128(sbase + L::kPOff + (k >> 2) * (kQT * 128)) + uint64_t(2 * (k & 3));
-          const uint64_t bd = VF ? umma_desc_mnmajor(sbase + L::kVOff + buf * L::kVBytes + k * 16 * L::kRowB, L::kRowB, kKV * 128)
-                                 : umma_desc_sw128(sbase + L::kVOff + buf * L::kVBytes + (k >> 2) * (D * 128)) + uint64_t(2 * (k & 3));
-          umma_f16_ss(tmem_O, ad, bd, idesc_o, k != 0);
-        }
-        umma_commit(o_full);
-        umma_commit(kv_empty(buf));
+        for (int i = 0; i < kKV / 2; ++i)
+          if (kv0 + 8 * (i >> 2) + 2 * (l & 3) + (i & 1) >= N) s[i] = -INFINITY;
       }
-      __syncwarp();
+      float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+      for (int i = 0; i < kKV / 2; ++i) mx[(i >> 1) & 1] = fmaxf(mx[(i >> 1) & 1], s[i]);
+      float corr[2], moff[2], rs[2] = {0.f, 0.f};
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 1));
+        mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 2));   // the four threads of a row agree
+        const float m_new = fmaxf(m_run[h], mx[h]);                      // finite: every tile has >= 1 valid key
+        corr[h] = fast_exp2_t((m_run[h] - m_new) * sl2);
+        moff[h] = m_new * sl2;
+        m_run[h] = m_new;
+      }
+      uint32_t pa[kKV / 16][4];                 // P as the register A operand of the PV wgmma, one set per 16 keys
+#pragma unroll
+      for (int i = 0; i < kKV / 2; i += 2) {
+        const int h = (i >> 1) & 1;
+        const float p0 = fast_exp2_t(fmaf(s[i], sl2, -moff[h]));       // exp2(-inf) = 0 for the masked keys
+        const float p1 = fast_exp2_t(fmaf(s[i + 1], sl2, -moff[h]));
+        __half2 hp = __floats2half2_rn(p0, p1);
+        const float2 hf = __half22float2(hp);            // sum what the PV MMA will actually see
+        rs[h] += hf.x + hf.y;
+        if (TRAIN) {
+          const float ks = 1.f / (1.f - P.p_drop);
+          const int qn = h ? qn1 : qn0, key = kv0 + 8 * (i >> 2) + 2 * (l & 3);
+          const bool k0 = attn_keep(seed, dir, blockIdx.y, qn, key, P.p_drop), k1 = attn_keep(seed, dir, blockIdx.y, qn, key + 1, P.p_drop);
+          hp = __floats2half2_rn(k0 ? hf.x * ks : 0.f, k1 ? hf.y * ks : 0.f);
+        }
+        pa[i >> 3][(i >> 1) & 3] = *reinterpret_cast<const uint32_t*>(&hp);
+      }
+#pragma unroll
+      for (int h = 0; h < 2; ++h) l_run[h] = l_run[h] * corr[h] + rs[h];   // per-thread partial sums; reduced at the end
+#pragma unroll
+      for (int i = 0; i < D / 2; ++i) o[i] *= corr[(i >> 1) & 1];
+      // ---- O += P V ----
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < kKV / 16; ++k) {
+        if (VF) {
+          wgmma_rs<1>(o, pa[k], gmma_desc_mnmajor(sbase + L::kVOff + buf * L::kVBytes + k * 16 * L::kRowB, L::kRowB, kKV * 128), true);
+        } else {
+          wgmma_rs<0>(o, pa[k], gmma_desc_sw128(sbase + L::kVOff + buf * L::kVBytes + (k >> 2) * (D * 128) + (k & 3) * 32), true);
+        }
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      if (l == 0) mbar_arrive(kv_empty(buf));
+    }
+    // ---- normalise and store (heads merged: column head*D) ; zero the pad rows ----
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      l_run[h] += __shfl_xor_sync(0xffffffffu, l_run[h], 1);
+      l_run[h] += __shfl_xor_sync(0xffffffffu, l_run[h], 2);
+    }
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int qn = h ? qn1 : qn0;
+      if (qn < n_pad) {
+        const float inv = qn < N ? 1.f / l_run[h] : 0.f;
+        __half* op = (dir == 0 ? P.out[0] : P.out[1]) + (size_t(b) * n_pad + qn) * C + head * D + 2 * (l & 3);
+#pragma unroll
+        for (int i = 2 * h; i < D / 2; i += 4)
+          *reinterpret_cast<uint32_t*>(op + 8 * (i >> 2)) = pack_half2(o[i] * inv, o[i + 1] * inv);
+      }
     }
   } else if (lane_id() == 0) {
     // ------------------------------------------------------------------ TMA producer (one thread)
@@ -318,12 +234,6 @@ __global__ void __launch_bounds__(192, AttnCfg<D>::kCtas) cross_attn_tma_kernel(
           tma_load_2d(sbase + L::kVOff + buf * L::kVBytes + kb * (D * 128), mv, kv_full(buf), row_b + j * kKV + kb * 64, head * D);
       }
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 4) {
-    tc_fence_after();
-    tmem_dealloc<L::kTmemCols>(tmem);
   }
 }
 
@@ -410,7 +320,7 @@ static int launch_attn_tma(const AttnParams& P, cudaStream_t st) {
     }
   }
   dim3 grid((P.n_pad + kQT - 1) / kQT, P.B * P.heads, 2);
-  launch_k(cross_attn_tma_kernel<D, VF, TRAIN>, dim3(grid), dim3(192), L::kTotal, st, P, maps);
+  launch_k(cross_attn_tma_kernel<D, VF, TRAIN>, dim3(grid), dim3(288), L::kTotal, st, P, maps);
   return check_launch("cross_attention");
 }
 

@@ -1,5 +1,4 @@
-// Shared pieces of the implicit-GEMM conv kernels (one-tile-per-CTA kernel in conv_gemm.cu, persistent kernel in
-// conv_persist.cu): problem descriptors, TMA descriptor bundle, epilogue chunk.
+// Shared pieces of the implicit-GEMM conv kernel (conv_gemm.cu): problem descriptors, TMA descriptor bundle, epilogue chunk.
 #pragma once
 #include "icaf_internal.cuh"
 
@@ -8,7 +7,7 @@ namespace icaf {
 constexpr int BM = 128;
 constexpr int BK = 64;              // 64 halfs = one 128-byte swizzle atom row
 constexpr int kLag = 2;             // cp.async groups kept in flight per gather thread
-constexpr int kThreads = 192;
+constexpr int kThreads = 288;     // epilogue / gather warpgroup, consumer warpgroup, TMA warp
 
 enum AMode { A_GATHER = 0, A_TMA2D = 1, A_TMA4D = 2 };
 
@@ -20,28 +19,17 @@ struct ConvProblem {
   const float* ln_s;        // LN fold: column sums of the gamma-folded filter, fp32 [Cout]
   float2* stats_out;        // EMIT_STATS: (sum, sum of squares) partials of every OUTPUT row, [M][ceil(N/32)]
 };
-// ICAF_DBG(P, bit): compile-time false unless the library is built with -DICAF_PROBE (ICAF_PROBE=1 python -m icafusion_b200.build)
-#ifdef ICAF_PROBE
-#define ICAF_DBG(P, bit) (((P).dbg & (bit)) != 0)
-#else
-#define ICAF_DBG(P, bit) false
-#endif
-
 struct ConvParams {
   ConvProblem p[2];
   int M, N, K, k_pad;
   int B, Hi, Wi, Cin, Ho, Wo, kh, kw, stride, pad;
   int act, epi;
   int a_mode, tw, th, tiles_x, tiles_y;   // A_TMA4D: tile = th x tw output pixels (tw*th <= 128), tiles per image
-  int stages;                             // smem ring depth (runtime: deep rings for small grids, 2 CTAs/SM otherwise)
+  int stages;                             // smem ring depth (runtime: deep rings for small grids, 2 CTAs/SM for BN <= 64)
   int splits;                             // split-K factor = cluster size along x (1 = no cluster); partial sums meet in DSMEM
-  int cblk;                               // A_TMA4D: channels per TMA box = min(Cin, 64); < 64 only in the persistent kernel
-  int halo;                               // conv_pair.cu: 3x3/s1 layers stage three x-shifted (th+2)-row copies per channel block (0 / 1)
-  int dense16;                            // host only: every problem's input has pixel pitch 16 (stem kernel eligibility)
+  int cblk;                               // A_TMA4D: channels per TMA box (64)
   int ln_parts;                           // LN fold: partials per input row (0 = no fold)
   float ln_eps, ln_inv_k;                 // LN fold: epsilon, 1 / (normalised features = K)
-  int dbg;                                // probe builds (-DICAF_PROBE, tools/conv_probe.py): 1 no stores, 2 no activation,
-                                          // 8 no A loads, 16 no B loads, 32 no MMA; always 0 in the shipped library
 };
 struct ConvMaps {          // TMA descriptors, passed by value as a __grid_constant__ kernel parameter
   CUtensorMap w[2];
@@ -153,128 +141,15 @@ __device__ __forceinline__ void epi_chunk(const uint32_t (&acc)[32], const float
   }
 }
 
-// Persistent-kernel flavour of epi_chunk, 16 columns of one output row.  Rows whose output (and residual) are 32-byte
-// aligned are written with one 256-bit store: a full L2 sector per lane and instruction.  `sb`: 16 bias floats (smem).
-// `al`: 2 = 32-byte aligned, 1 = 16-byte aligned, 0 = element-wise loads / stores of the first `ncols` columns (ragged N,
-// odd pitches); the math is shared by the three so the hot loop stays small (instruction cache, tools/conv_probe.py).
-template <int ACT, int RES, int XM = 0>
-__device__ __forceinline__ void epi_chunk16(const uint32_t (&acc)[16], const float* __restrict__ sb, float rbias,
-                                            float alpha, float beta, const __half* __restrict__ rp,
-                                            __half* __restrict__ yp, int al, int ncols, bool do_store, EpiRow& ex, int cb) {
-  auto act = [&](float t) {
-    if (ACT == ICAF_ACT_SILU) t = silu_f(t);
-    if (ACT == ICAF_ACT_GELU) t = gelu_erf_f(t);
-    return t;
-  };
-  float v[16];
-#pragma unroll
-  for (int q = 0; q < 4; ++q) {
-    const float4 b4 = *reinterpret_cast<const float4*>(sb + 4 * q);
-    float a0 = __uint_as_float(acc[4 * q + 0]), a1 = __uint_as_float(acc[4 * q + 1]);
-    float a2 = __uint_as_float(acc[4 * q + 2]), a3 = __uint_as_float(acc[4 * q + 3]);
-    if (XM == 1) {
-      const float4 s4 = __ldg(reinterpret_cast<const float4*>(ex.ln_s + cb + 4 * q));
-      a0 = ex.ln_a * (a0 - ex.ln_mu * s4.x); a1 = ex.ln_a * (a1 - ex.ln_mu * s4.y);
-      a2 = ex.ln_a * (a2 - ex.ln_mu * s4.z); a3 = ex.ln_a * (a3 - ex.ln_mu * s4.w);
-    }
-    v[4 * q + 0] = act(a0 + b4.x + rbias);
-    v[4 * q + 1] = act(a1 + b4.y + rbias);
-    v[4 * q + 2] = act(a2 + b4.z + rbias);
-    v[4 * q + 3] = act(a3 + b4.w + rbias);
-  }
-  if (RES != 0) {
-    uint32_t rr[8];
-    if (al == 2) {
-      ld_global_nc_v8(rp, rr);
-    } else if (al == 1) {
-      uint4 r0 = __ldg(reinterpret_cast<const uint4*>(rp));
-      uint4 r1 = __ldg(reinterpret_cast<const uint4*>(rp + 8));
-      rr[0] = r0.x; rr[1] = r0.y; rr[2] = r0.z; rr[3] = r0.w; rr[4] = r1.x; rr[5] = r1.y; rr[6] = r1.z; rr[7] = r1.w;
-    } else {
-      const unsigned short* rs = reinterpret_cast<const unsigned short*>(rp);
-#pragma unroll
-      for (int e = 0; e < 8; ++e) {
-        const uint32_t lo = 2 * e < ncols ? rs[2 * e] : 0u;
-        const uint32_t hi = 2 * e + 1 < ncols ? rs[2 * e + 1] : 0u;
-        rr[e] = lo | (hi << 16);
-      }
-    }
-#pragma unroll
-    for (int e = 0; e < 8; ++e) {
-      float2 rf = __half22float2(*reinterpret_cast<const __half2*>(&rr[e]));
-      if (RES == 2) {
-        v[2 * e] = alpha * rf.x + beta * v[2 * e];
-        v[2 * e + 1] = alpha * rf.y + beta * v[2 * e + 1];
-      } else {
-        v[2 * e] += rf.x;
-        v[2 * e + 1] += rf.y;
-      }
-    }
-  }
-  uint32_t o[8];
-#pragma unroll
-  for (int e = 0; e < 8; ++e) o[e] = pack_half2(v[2 * e], v[2 * e + 1]);
-  if (XM == 2) {
-#pragma unroll
-    for (int e = 0; e < 8; ++e) {
-      if (2 * e < ncols) {                         // ragged tails: only the columns that exist
-        const float2 w = __half22float2(*reinterpret_cast<const __half2*>(&o[e]));
-        ex.sum += w.x; ex.sumsq += w.x * w.x;
-        if (2 * e + 1 < ncols) { ex.sum += w.y; ex.sumsq += w.y * w.y; }
-      }
-    }
-  }
-  if (do_store) {
-    if (al == 2) {
-      st_global_v8(yp, o);
-    } else if (al == 1) {
-      *reinterpret_cast<uint4*>(yp) = make_uint4(o[0], o[1], o[2], o[3]);
-      *reinterpret_cast<uint4*>(yp + 8) = make_uint4(o[4], o[5], o[6], o[7]);
-    } else {
-      unsigned short* ys = reinterpret_cast<unsigned short*>(yp);
-#pragma unroll
-      for (int e = 0; e < 8; ++e) {
-        if (2 * e < ncols) ys[2 * e] = (unsigned short)(o[e] & 0xffffu);
-        if (2 * e + 1 < ncols) ys[2 * e + 1] = (unsigned short)(o[e] >> 16);
-      }
-    }
-  }
-}
-
-__device__ __forceinline__ ConvProblem pick_problem_stem(const ConvProblem (&p)[2], int z) {
-  ConvProblem r = p[0];
-  if (z) r = p[1];
-  return r;
-}
-
 // Host-side launch plan: everything the dispatcher decides before it touches CUDA.  icaf_conv2d_plan (host only, no
 // device needed) exposes it so that a CPU test can walk every layer geometry through the dispatcher's invariants.
 struct ConvPlan {
-  int kernel;                     // ICAF_KERNEL_TC / _PERSIST / _PAIR
+  int kernel;                     // ICAF_KERNEL_TC
   int bn;                         // output-channel tile width
   unsigned grid_x, grid_y, grid_z, cluster;
   int smem;                       // dynamic shared memory per CTA (bytes)
   int total, m_tiles, m_pairs, n_tiles;
   int sms;                        // SM count the plan was made for
 };
-
-// Each kernel family: plan_* fills the launch shape (and P.stages / P.splits) and checks the kernel's invariants without
-// any CUDA call; launch_* encodes the TMA descriptors and launches exactly that plan.
-// persistent kernel (conv_persist.cu), BN = 32, 64, 128, 256
-template <int BN>
-int plan_persist(ConvParams& P, int n_io, ConvPlan& pl);
-template <int BN>
-int launch_persist(const ConvParams& P, const ConvPlan& pl, const __half* const (&w)[2], const icaf_conv_geom* g, int n_io, cudaStream_t st);
-
-// image-stem kernel (conv_stem.cu): 3x3 / s1 over the 16-channel space-to-depth frame, x-merged rows
-bool stem_eligible(const icaf_conv_geom* g);
-int plan_stem(ConvParams& P, const icaf_conv_geom* g, int n_io, ConvPlan& pl);
-int launch_stem(const ConvParams& P, const ConvPlan& pl, const __half* const (&w)[2], const icaf_conv_geom* g, int n_io, cudaStream_t st);
-
-// CTA-pair kernel (conv_pair.cu): 256 x BN tiles over two SMs, tcgen05.mma.cta_group::2 (BN = 64, 128, 256)
-template <int BN>
-int plan_pair(ConvParams& P, const icaf_conv_geom* g, int n_io, ConvPlan& pl);
-template <int BN>
-int launch_pair(const ConvParams& P, const ConvPlan& pl, const __half* const (&w)[2], const icaf_conv_geom* g, int n_io, cudaStream_t st);
 
 }  // namespace icaf

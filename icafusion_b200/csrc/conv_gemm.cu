@@ -1,27 +1,24 @@
-// Implicit-GEMM Conv(+folded BN)+bias+activation(+residual) / Linear on the 5th-gen tensor cores (tcgen05).
+// Implicit-GEMM Conv(+folded BN)+bias+activation(+residual) / Linear on the Hopper tensor cores (wgmma).
 //
-//   C[M=B*Ho*Wo, N=Cout] = A[M, K=kh*kw*Cin] * W[N, K]^T           fp16 operands, fp32 accumulate in TMEM
+//   C[M=B*Ho*Wo, N=Cout] = A[M, K=kh*kw*Cin] * W[N, K]^T           fp16 operands, fp32 accumulate in registers
 //
 // A is never materialised (no im2col).  Three ways to stage the A tile (128 rows x 64 K) into the 128B-swizzled
-// K-major shared-memory layout the UMMA descriptors expect, picked per layer on the host:
+// K-major shared-memory layout the wgmma descriptors expect, picked per layer on the host:
 //   A_TMA2D  : 1x1 conv / linear -- A is a plain [M][Cin] matrix: one 2-D TMA box per stage.
 //   A_TMA4D  : kxk conv whose 128-row tile is a TH x TW patch of one image and Cin % 64 == 0: one 4-D TMA box
 //              (64 ch, TW*s, TH*s, 1) of the NHWC input per stage at coordinates shifted by the filter tap;
 //              out-of-bounds (= padding) is zero-filled by the TMA unit, the stride is the box traversal stride.
-//              (Cin = 16 / 32: one box per filter tap, 32- / 64-byte swizzle -- persistent and pair kernels only.)
-//   A_GATHER : anything else (Cin = 4 / 8 / odd multiples of 8, Cin < 64 on small grids): producer warps gather 16-byte
-//              channel runs with cp.async (zero-fill), 4 rows x 128 B per warp instruction.
+//   A_GATHER : anything else (Cin = 4 / 8 / 16 / 32 / odd multiples of 8): producer warps gather 16-byte channel runs
+//              with cp.async (zero-fill), 4 rows x 128 B per warp instruction.
 // The filter tile (BN rows x 64 K) always arrives by 2-D TMA.
-// Three kernels share this contract; icaf_conv2d_fwd picks per layer:
-//   conv_gemm_tc_kernel      (this file)     one tile per CTA, split-K over clusters     -- grids below ~2 tiles per SM
-//   conv_gemm_persist_kernel (conv_persist.cu) one CTA per SM looping over tiles         -- many tiles, short K
-//   conv_gemm_pair_kernel    (conv_pair.cu)  CTA pairs (cta_group::2), halo copies for 3x3 -- wide / deep-K layers
-// conv_gemm_tc_kernel: CTA = one 128 x BN output tile, 192 threads:
-//   warps 0-3 : A_GATHER producers, then the epilogue (thread t owns TMEM lane t = output row t)
-//   warp  4   : TMEM allocator + single-thread tcgen05.mma issuer
-//   warp  5   : TMA producer (one elected thread)
-// Pipelines: smem ring full[]/empty[] (producers <-> MMA), accum_full (MMA -> epilogue).  Two CTAs share an SM
-// (BN <= 128) so one CTA's epilogue overlaps the other's main loop.
+// conv_gemm_tc_kernel: CTA = one 128 x BN output tile (BN = 32 / 64 / 128), 288 threads:
+//   warps 0-3 : A_GATHER producers, then the epilogue (thread t owns output row t)
+//   warps 4-7 : one consumer warpgroup: two m64nBNk16 wgmma per 16 K (rows 0-63, 64-127), accumulators in registers,
+//               written to shared memory (the idle ring) once the K loop is done
+//   warp  8   : TMA producer (one elected thread)
+// Pipelines: smem ring full[]/empty[] (producers <-> consumer), named barrier (staged accumulator -> epilogue).  Small
+// tiles (BN <= 64) let two CTAs share an SM so that one CTA's epilogue overlaps the other's main loop.  Split-K: the
+// CTAs of a cluster take a K range each; the leader adds the others' staged tiles through distributed shared memory.
 #include <cstdlib>
 #include <cstring>
 
@@ -35,27 +32,27 @@ struct SmemLayout {
   static constexpr int kABytes = BM * BK * 2;
   static constexpr int kBBytes = BN * BK * 2;
   static constexpr int kStageBytes = kABytes + kBBytes;
-  static constexpr int kTmemCols = BN < 32 ? 32 : BN;
-  // [ring: stages x (A|B)] [barriers 256 B] [bias BN fp32] ; + 1024 B alignment slack
+  static constexpr int kPitch = BN + 4;                       // floats per staged accumulator row (spreads rows over banks)
+  static constexpr int kAccBytes = BM * kPitch * 4;
+  // [ring: stages x (A|B), at least the staged accumulator] [barriers 256 B] [bias BN fp32] ; + 1024 B alignment slack
   static constexpr int kTailBytes = 256 + BN * 4 + 1024;
-  static int total(int stages) { return stages * kStageBytes + kTailBytes; }
+  __host__ __device__ static int region(int stages) { return stages * kStageBytes > kAccBytes ? stages * kStageBytes : kAccBytes; }
+  static int total(int stages) { return region(stages) + kTailBytes; }
 };
 
 // XM: the LayerNorm-fold / row-statistics epilogues (DMFF linears) live in their own instantiation so that the epilogue
-// of every other layer keeps its round-1 size (the hot loops are instruction-cache sensitive).
+// of every other layer stays small (the hot loops are instruction-cache sensitive).
 template <int BN, bool XM>
-__global__ void __launch_bounds__(kThreads, (BN <= 128 ? 2 : 1))
+__global__ void __launch_bounds__(kThreads, (BN <= 64 ? 2 : 1))
 conv_gemm_tc_kernel(const ConvParams P, const __grid_constant__ ConvMaps maps) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   using L = SmemLayout<BN>;
   const int kStages = P.stages;
-  const uint32_t bar_off = uint32_t(kStages) * L::kStageBytes;
+  const uint32_t bar_off = uint32_t(L::region(kStages));
   const uint32_t bar_base = smem_base + bar_off;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (kMaxStages + s); };
-  const uint32_t accum_bar = bar_base + 8u * (2 * kMaxStages);
-  const uint32_t tmem_slot = bar_base + 8u * (2 * kMaxStages + 1);
   uint8_t* smem_gen = smem_raw + (smem_base - smem_u32(smem_raw));
 
   pdl_launch_dependents();
@@ -87,22 +84,18 @@ conv_gemm_tc_kernel(const ConvParams P, const __grid_constant__ ConvMaps maps) {
     const uint32_t nfull = a_mode == A_GATHER ? 129u : 1u;    // 128 gather threads + the TMA thread
     for (int s = 0; s < kStages; ++s) {
       mbar_init(full_bar(s), nfull);
-      mbar_init(empty_bar(s), 1);
+      mbar_init(empty_bar(s), 4);                             // one arrival per consumer warp
     }
-    mbar_init(accum_bar, 1);
     fence_mbar_init();
   }
-  if (warp == 4) tmem_alloc<L::kTmemCols>(tmem_slot);
-  if (warp == 5 && lane_id() == 0) {
+  if (warp == 8 && lane_id() == 0) {
     tma_prefetch_desc(bz ? &maps.w[1] : &maps.w[0]);
     if (a_mode != A_GATHER) tma_prefetch_desc(bz ? &maps.a[1] : &maps.a[0]);
   }
   float* sbias = reinterpret_cast<float*>(smem_gen + bar_off + 256);
-  tc_fence_before();
+  float* sacc = reinterpret_cast<float*>(smem_gen);           // staged accumulator [BM][kPitch], reuses the idle ring
   __syncthreads();
-  tc_fence_after();
-  pdl_wait();   // prologue (barriers, TMEM, descriptor prefetch, bias = parameters only) overlapped the previous kernel
-  const uint32_t tmem_d = *reinterpret_cast<volatile uint32_t*>(smem_gen + bar_off + 8 * (2 * kMaxStages + 1));
+  pdl_wait();   // prologue (barriers, descriptor prefetch) overlapped the previous kernel
 
   if (warp < 4) {
     // Epilogue operands that do not depend on the main loop are fetched now so their DRAM latency hides behind it:
@@ -117,6 +110,10 @@ conv_gemm_tc_kernel(const ConvParams P, const __grid_constant__ ConvMaps maps) {
     if (P.epi & ICAF_EPI_SCALED_RES) { alpha = __ldg(pr.alpha); beta = __ldg(pr.beta); }
     if (a_mode == A_GATHER) {
       // ---------------------------------------------------------------- cp.async gather producers
+      // A stage is handed over once this thread's copies of it have landed and been made visible to the async proxy
+      // (wait_group + fence.proxy.async): `lag` stages stay in flight per thread.  The consumer frees stage j only once
+      // it holds stage j + 1, so the lag must stay below stages - 1.
+      const int lag = kStages - 2 < kLag ? kStages - 2 : kLag;
       const int c = tid & 7;          // 16-byte chunk within the 128-byte K row
       const int r0 = tid >> 3;        // rows r0 + 16*i
       const uint32_t sw = uint32_t(c ^ (r0 & 7)) << 4;
@@ -135,7 +132,7 @@ conv_gemm_tc_kernel(const ConvParams P, const __grid_constant__ ConvMaps maps) {
         iy0[i] = mv ? oy * P.stride - P.pad : -100000;   // invalid rows fall out of bounds -> zero fill
         ix0[i] = ox * P.stride - P.pad;
       }
-      int s = 0;
+      int s = 0, s_done = 0;
       uint32_t ph = 0;
       for (int kb = 0; kb < nkb; ++kb) {
         mbar_wait(empty_bar(s), ph ^ 1);
@@ -153,13 +150,25 @@ conv_gemm_tc_kernel(const ConvParams P, const __grid_constant__ ConvMaps maps) {
           size_t off = ok ? (size_t(base[i] + uint32_t(iy * P.Wi + ix)) * size_t(pr.x_ld) + ch) : 0;
           cp_async16(sa + uint32_t(r0 + 16 * i) * 128u + sw, pr.x + off, ok);
         }
-        cp_async_arrive_on(full_bar(s));     // asynchronous arrival when this thread's chunks have landed: no wait_group
+        cp_async_commit();
+        if (kb >= lag) {
+          if (lag == 2) cp_async_wait<2>(); else if (lag == 1) cp_async_wait<1>(); else cp_async_wait<0>();
+          fence_proxy_async_smem();
+          mbar_arrive(full_bar(s_done));
+          if (++s_done == kStages) s_done = 0;
+        }
         if (++s == kStages) { s = 0; ph ^= 1; }
+      }
+      cp_async_wait<0>();
+      fence_proxy_async_smem();
+      for (int kb = nkb - lag < 0 ? 0 : nkb - lag; kb < nkb; ++kb) {
+        mbar_arrive(full_bar(s_done));
+        if (++s_done == kStages) s_done = 0;
       }
     }
 
     // ------------------------------------------------------------------ epilogue
-    const int row = tid;                   // TMEM lane == tile row
+    const int row = tid;                   // staged accumulator row == tile row
     int m;
     bool mvalid;
     if (a_mode == A_TMA4D) {
@@ -170,7 +179,6 @@ conv_gemm_tc_kernel(const ConvParams P, const __grid_constant__ ConvMaps maps) {
       m = m0 + row;
       mvalid = m < P.M;
     }
-    const uint32_t trow = tmem_d + (uint32_t(warp * 32) << 16);
     const float rbias = ((P.epi & ICAF_EPI_BIAS_ROW) && pr.bias && mvalid) ? __ldg(pr.bias + m) : 0.f;
     __half* yrow = pr.y + size_t(mvalid ? m : 0) * pr.y_ld;
     const __half* rrow = pr.res ? pr.res + size_t(mvalid ? m : 0) * pr.res_ld : nullptr;
@@ -181,54 +189,35 @@ conv_gemm_tc_kernel(const ConvParams P, const __grid_constant__ ConvMaps maps) {
 #pragma unroll
     for (int i = 0; i < (BN + 127) / 128; ++i)
       if (tid + 128 * i < BN) sbias[tid + 128 * i] = bias_r[i];
-    named_bar_sync(1, 128);                // bias tile visible to the four epilogue warps
     EpiRow ex;
     ex.sum = ex.sumsq = 0.f; ex.ln_a = 1.f; ex.ln_mu = 0.f; ex.ln_s = nullptr;
     if (XM) {
       ex.ln_s = pr.ln_s ? pr.ln_s + n0 : nullptr;
       if (P.ln_parts > 0) epi_row_ln(ex, P, pr, m, mvalid);   // row statistics: fetched while the main loop still runs
     }
-    mbar_wait(accum_bar, 0);
-    tc_fence_after();
+    // the staged accumulators (of every CTA of the cluster) and the bias tile are complete
+    if (splits > 1) { cluster_arrive(); cluster_wait(); } else { named_bar_sync(1, 256); }
     // XM: 9 / 10 = LayerNorm folded into this GEMM (no activation / GELU); 11 = scaled residual + statistics of the output rows
     const int mode_act = XM ? (P.ln_parts > 0 ? (P.act == ICAF_ACT_GELU ? 10 : 9) : 11) : P.act * 3 + mode;
-    if (splits > 1) {
-      // ---- split-K reduction through distributed shared memory ----
-      // Every CTA's ring is idle once its accumulator is complete.  Barrier A: all accumulators done (so the leader's
-      // ring may be overwritten); CTAs 1..S-1 then push their fp32 partial tile into the leader's ring; barrier B:
-      // the leader adds them to its own accumulator and runs the real epilogue.
-      constexpr int kPitch = BN + 4;                 // floats per staged row (+4: spreads the rows over the banks)
-      cluster_arrive();
-      cluster_wait();
-      if (crank != 0) {
-        const uint32_t dst0 = map_to_cta(smem_base, 0) + uint32_t(((crank - 1) * BM + row) * kPitch) * 4u;
-#pragma unroll 1
-        for (int cb = 0; cb < BN; cb += 32) {
-          uint32_t acc[32];
-          __syncwarp();
-          tmem_ld32(trow + cb, acc);
-          tmem_ld_wait();
-#pragma unroll
-          for (int q = 0; q < 8; ++q)
-            st_cluster_v4(dst0 + uint32_t(cb + 4 * q) * 4u, acc[4 * q], acc[4 * q + 1], acc[4 * q + 2], acc[4 * q + 3]);
-        }
-      }
-      cluster_arrive();
-      cluster_wait();
-    }
     if (crank == 0) {
-      const float* part = reinterpret_cast<const float*>(smem_gen) + size_t(row) * (BN + 4);
+      const float* arow = sacc + size_t(row) * L::kPitch;
+      const uint32_t arow_s = smem_u32(arow);
 #pragma unroll 1
       for (int cb = 0; cb < BN; cb += 32) {
         uint32_t acc[32];
-        __syncwarp();
-        tmem_ld32(trow + cb, acc);      // .sync.aligned: executed by the whole (converged) warp
-        tmem_ld_wait();
+#pragma unroll
+        for (int q = 0; q < 8; ++q) {
+          const float4 v = *reinterpret_cast<const float4*>(arow + cb + 4 * q);
+          acc[4 * q] = __float_as_uint(v.x); acc[4 * q + 1] = __float_as_uint(v.y);
+          acc[4 * q + 2] = __float_as_uint(v.z); acc[4 * q + 3] = __float_as_uint(v.w);
+        }
+        // ---- split-K reduction: the other CTAs' staged partial tiles, read through distributed shared memory ----
         for (int r = 1; r < splits; ++r) {
-          const float4* pp = reinterpret_cast<const float4*>(part + size_t(r - 1) * BM * (BN + 4) + cb);
+          const uint32_t peer = map_to_cta(arow_s, uint32_t(r)) + uint32_t(cb) * 4u;
 #pragma unroll
           for (int q = 0; q < 8; ++q) {
-            float4 v = pp[q];
+            float4 v;
+            ld_cluster_v4(peer + 16u * q, v);
             acc[4 * q] = __float_as_uint(__uint_as_float(acc[4 * q]) + v.x);
             acc[4 * q + 1] = __float_as_uint(__uint_as_float(acc[4 * q + 1]) + v.y);
             acc[4 * q + 2] = __float_as_uint(__uint_as_float(acc[4 * q + 2]) + v.z);
@@ -267,30 +256,42 @@ conv_gemm_tc_kernel(const ConvParams P, const __grid_constant__ ConvMaps maps) {
       }
       if (XM && mode_act == 11 && mvalid && n0 < P.N) epi_row_emit(ex, P, pr, m, n0, min(n0 + BN, P.N));
     }
-  } else if (warp == 4) {
-    // ------------------------------------------------------------------ MMA issuer
-    constexpr uint32_t idesc = umma_idesc_f16(BM, BN);
-    int s = 0;
+    if (splits > 1) { cluster_arrive(); cluster_wait(); }   // the peers' staged tiles stay alive until the leader has read them
+  } else if (warp < 8) {
+    // ------------------------------------------------------------------ consumer warpgroup (wgmma)
+    float acc0[BN / 2], acc1[BN / 2];
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) { acc0[i] = 0.f; acc1[i] = 0.f; }
+    int s = 0, s_prev = 0;
     uint32_t ph = 0;
     for (int kb = 0; kb < nkb; ++kb) {
       mbar_wait(full_bar(s), ph);
-      tc_fence_after();
-      if (elect_one()) {
-        const uint32_t sa = smem_base + s * L::kStageBytes;
-        const uint64_t ad = umma_desc_sw128(sa);
-        const uint64_t bd = umma_desc_sw128(sa + L::kABytes);
+      const uint32_t sa = smem_base + s * L::kStageBytes;
+      wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < BK / 16; ++k)
-          umma_f16_ss(tmem_d, ad + uint64_t(2 * k), bd + uint64_t(2 * k), idesc, (kb | k) != 0);
-        umma_commit(empty_bar(s));
-        if (kb == nkb - 1) umma_commit(accum_bar);
+      for (int k = 0; k < BK / 16; ++k) {
+        const uint64_t bd = gmma_desc_sw128(sa + L::kABytes + 32 * k);
+        wgmma_ss<0, 0>(acc0, gmma_desc_sw128(sa + 32 * k), bd, (kb | k) != 0);
+        wgmma_ss<0, 0>(acc1, gmma_desc_sw128(sa + 64 * 128 + 32 * k), bd, (kb | k) != 0);
       }
-      __syncwarp();
+      wgmma_commit();
+      wgmma_wait<1>();                                  // the previous stage's MMAs are done: hand it back
+      if (kb > 0 && lane_id() == 0) mbar_arrive(empty_bar(s_prev));
+      s_prev = s;
       if (++s == kStages) { s = 0; ph ^= 1; }
     }
-    if (splits > 1) { cluster_arrive(); cluster_wait(); cluster_arrive(); cluster_wait(); }
+    wgmma_wait<0>();
+    // the ring is idle now (every stage consumed): stage the accumulator tile as rows for the epilogue warps
+    const int t = tid - 128, w = t >> 5, l = t & 31;
+#pragma unroll
+    for (int i = 0; i < BN / 2; i += 2) {
+      const int r = 16 * w + (l >> 2) + 8 * ((i >> 1) & 1), col = 8 * (i >> 2) + 2 * (l & 3);
+      *reinterpret_cast<float2*>(sacc + size_t(r) * L::kPitch + col) = make_float2(acc0[i], acc0[i + 1]);
+      *reinterpret_cast<float2*>(sacc + size_t(r + 64) * L::kPitch + col) = make_float2(acc1[i], acc1[i + 1]);
+    }
+    if (splits > 1) { cluster_arrive(); cluster_wait(); cluster_arrive(); cluster_wait(); } else { named_bar_sync(1, 256); }
   } else {
-    // ------------------------------------------------------------------ TMA producer (warp 5, one thread)
+    // ------------------------------------------------------------------ TMA producer (warp 8, one thread)
     if (elect_one()) {
       const CUtensorMap* mw = bz ? &maps.w[1] : &maps.w[0];
       const CUtensorMap* ma = bz ? &maps.a[1] : &maps.a[0];
@@ -317,12 +318,6 @@ conv_gemm_tc_kernel(const ConvParams P, const __grid_constant__ ConvMaps maps) {
     }
     __syncwarp();
     if (splits > 1) { cluster_arrive(); cluster_wait(); cluster_arrive(); cluster_wait(); }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 4) {
-    tc_fence_after();
-    tmem_dealloc<L::kTmemCols>(tmem_d);
   }
 }
 
@@ -359,11 +354,6 @@ __global__ void conv_gemm_simt_kernel(const SimtParams S) {
   pr.y[size_t(m) * pr.y_ld + n] = __float2half_rn(acc);
 }
 
-#ifdef ICAF_PROBE
-static int g_dbg = 0, g_dbg_bn = 0;       // probe builds only: see icaf_debug_set below
-#else
-constexpr int g_dbg = 0, g_dbg_bn = 0;
-#endif
 // Geometry half of the argument check (host only): everything the planner needs, no pointers.
 static int fill_geom(const icaf_conv_geom* g, int n_io, ConvParams& P) {
   if (!g || n_io < 1 || n_io > 2) return set_error(ICAF_ERR_BAD_ARG, "conv2d: need 1 or 2 problems");
@@ -385,9 +375,8 @@ static int fill_geom(const icaf_conv_geom* g, int n_io, ConvParams& P) {
   P.M = int(M); P.N = g->Cout; P.K = g->kh * g->kw * g->Cin; P.k_pad = g->k_pad;
   P.B = g->B; P.Hi = g->Hi; P.Wi = g->Wi; P.Cin = g->Cin; P.Ho = g->Ho; P.Wo = g->Wo;
   P.kh = g->kh; P.kw = g->kw; P.stride = g->stride; P.pad = g->pad; P.act = g->act; P.epi = g->epi;
-  P.a_mode = A_GATHER; P.tw = P.th = P.tiles_x = P.tiles_y = 0; P.stages = 2; P.splits = 1; P.cblk = 64; P.halo = 0; P.dbg = g_dbg;
+  P.a_mode = A_GATHER; P.tw = P.th = P.tiles_x = P.tiles_y = 0; P.stages = 2; P.splits = 1; P.cblk = 64;
   P.ln_parts = 0; P.ln_eps = 0.f; P.ln_inv_k = 0.f;
-  P.dense16 = 1;                          // plan-only calls have no pointers: assume a dense input frame
   memset(P.p, 0, sizeof(P.p));
   return ICAF_OK;
 }
@@ -414,7 +403,6 @@ static int fill_params(const icaf_conv_geom* g, const icaf_conv_io* io, int n_io
                          (g->epi & ICAF_EPI_LN_FOLD) ? s.ln_colsum : nullptr,
                          (g->epi & ICAF_EPI_EMIT_STATS) ? (float2*)s.stats_out : nullptr};
     if (i == 0 && (g->epi & ICAF_EPI_LN_FOLD)) { P.ln_parts = s.ln_parts; P.ln_eps = s.ln_eps; P.ln_inv_k = 1.0f / float(P.K); }
-    if (i < n_io && s.x_ld != 16) P.dense16 = 0;
     w[i] = (const __half*)s.w;
   }
   return ICAF_OK;
@@ -426,7 +414,7 @@ static void plan_a_mode(const icaf_conv_geom* g, ConvParams& P) {
     P.a_mode = A_TMA2D;
     return;
   }
-  if ((g->Cin % 64 == 0 || g->Cin == 32 || g->Cin == 16) && g->stride <= 2) {
+  if (g->Cin % 64 == 0 && g->stride <= 2) {
     // tile = th x tw output pixels of one image, tw | Wo, tw*th <= 128: maximise the fraction of useful MMA rows
     int best_tw = 0, best_th = 0;
     double best_u = 0.0;
@@ -441,7 +429,6 @@ static void plan_a_mode(const icaf_conv_geom* g, ConvParams& P) {
     }
     if (best_u >= 0.6) {
       P.a_mode = A_TMA4D; P.tw = best_tw; P.th = best_th; P.tiles_x = g->Wo / best_tw; P.tiles_y = (g->Ho + best_th - 1) / best_th;
-      P.cblk = g->Cin < 64 ? g->Cin : 64;
     }
   }
 }
@@ -456,9 +443,10 @@ static int plan_tc(ConvParams& P, int n_io, ConvPlan& pl) {
     return set_error(ICAF_ERR_BAD_ARG, "conv2d(tc): 4-D tiles must cover the map with at most 128 pixels each, 64-channel blocks");
   unsigned gx = unsigned(mt), gy = unsigned((P.N + BN - 1) / BN), gz = unsigned(n_io);
   // Ring depth: a grid that fits in one wave gets the whole SM (deep ring: the K loop is latency-bound at small M);
-  // otherwise two CTAs share an SM so that one CTA's epilogue overlaps the other's main loop.
+  // otherwise two CTAs of the narrow tiles share an SM so that one CTA's epilogue overlaps the other's main loop (BN = 128
+  // keeps one CTA per SM: its 128 accumulator registers per consumer thread leave no room for a second one).
   const long long ctas = (long long)gx * gy * gz;
-  const int budget = (ctas <= pl.sms || BN > 128) ? kSmemCap : (kSmemCap / 2 - 1024);
+  const int budget = (ctas <= pl.sms || BN > 64) ? kSmemCap : (kSmemCap / 2 - 1024);
   int stages = (budget - L::kTailBytes) / L::kStageBytes;
   const int nkb = P.k_pad / BK;
   if (stages > nkb) stages = nkb;
@@ -470,14 +458,11 @@ static int plan_tc(ConvParams& P, int n_io, ConvPlan& pl) {
     splits = int(pl.sms / ctas);
     if (splits > 8) splits = 8;                    // portable cluster size
     if (splits > nkb / 4) splits = nkb / 4;        // >= 4 K blocks per CTA
-    const int per_split = BM * (BN + 4) * 4;       // staged fp32 partial tile in the leader's ring
-    while (splits > 1 && (splits - 1) * per_split > stages * L::kStageBytes) --splits;
     if (splits < 1) splits = 1;
   }
   if (splits > 1) {
     const int per = (nkb + splits - 1) / splits;
     if (stages > per) stages = per < 2 ? 2 : per;
-    while ((splits - 1) * (BM * (BN + 4) * 4) > stages * L::kStageBytes) ++stages;   // keep room for the partial tiles
     gx *= splits;
   }
   if (stages > kMaxStages || L::total(stages) > kSmemCap)
@@ -518,104 +503,21 @@ static int launch_tc(const ConvParams& P, const ConvPlan& pl, const __half* cons
 }
 
 // ---------------------------------------------------------------------------------------------------
-// The dispatcher, host only: staging mode, tile shapes, kernel family and tile width for one layer geometry.  No CUDA call.
-// pair_mode: -1 = the ICAF_PAIR environment switch (default 1), 0 = never CTA pairs, 1 = heuristic, 2 = pairs wherever they can run.
-static int env_pair_mode() {
-  static const int v = []() { const char* e = getenv("ICAF_PAIR"); return !e ? 1 : (e[0] == '0' ? 0 : (e[0] == 'a' ? 2 : 1)); }();
-  return v;
-}
-
-static int plan_conv(const icaf_conv_geom* g, int n_io, int sms, int pair_mode, ConvParams& P, ConvPlan& pl) {
+// The dispatcher, host only: staging mode, tile shape and tile width for one layer geometry.  No CUDA call.
+// (`pair_mode` of icaf_conv2d_plan selects CTA-pair kernels on architectures that have them; sm_90a has none.)
+static int plan_conv(const icaf_conv_geom* g, int n_io, int sms, ConvParams& P, ConvPlan& pl) {
   memset(&pl, 0, sizeof(pl));
   pl.sms = sms;
   if (sms < 1) return set_error(ICAF_ERR_BAD_ARG, "conv2d: SM count must be positive");
   plan_a_mode(g, P);
-  // Tile width: the widest BN that still yields at least ~one CTA per SM (two waves for the 1-CTA/SM BN=256); small
-  // problems take BN=32 so that more SMs share the K loop.
+  // Tile width: the widest BN that still yields at least ~one CTA per SM; small problems take BN = 32 so that more SMs
+  // share the K loop (and split it over clusters when even that leaves most SMs idle).
   const long long mt = P.a_mode == A_TMA4D ? (long long)P.B * P.tiles_x * P.tiles_y : (P.M + BM - 1) / BM;
   auto ctas = [&](int bn) { return mt * ((P.N + bn - 1) / bn) * n_io; };
-  // CTA pairs (conv_pair.cu): two SMs share one 256 x BN tile and each loads only half of the filter tile.  Measured
-  // (yolov5l batch 16, profiles/): always a win at BN = 256 once a wave of clusters is full (or half full with a deep K
-  // loop); at BN = 128 / 64 only for the deep-K (3x3) layers -- the short-K 1x1 layers are HBM / epilogue bound and lose
-  // to the pair's extra synchronisation.  ICAF_PAIR=0 disables it, ICAF_PAIR=all forces it wherever it can run (tests).
-  const int pair_env = pair_mode < 0 ? env_pair_mode() : pair_mode;
-  const bool pair_ok = pair_env && (P.a_mode == A_TMA2D || (P.a_mode == A_TMA4D && P.cblk == 64));
-  const int nkb_all = P.k_pad / BK;
-  auto pair_wanted = [&](int b) {
-    if (!pair_ok || b < 64) return false;
-    if (pair_env == 2) return true;
-    const long long pairs = ctas(b) / 2;
-    if (b == 256) return pairs >= sms / 2 || (pairs >= sms / 4 && nkb_all >= 32);
-    return pairs >= sms / 2 && nkb_all >= 8;
-  };
-  // 3x3 / stride 1 layers the pair kernel can run with halo copies (conv_pair.cu): once those have removed most of the
-  // activation traffic, BN = 128 pairs beat BN = 256 (probe: 50 vs 52-54 us on M20480 N256 K2304, 54 vs 63 us on the P5 layer:
-  // finer wave balance, four accumulator buffers)
-  static const bool halo_on = []() { const char* e = getenv("ICAF_HALO"); return !(e && e[0] == '0'); }();
-  static const bool bres_on = []() { const char* e = getenv("ICAF_HALO"); return !(e && e[0] == '1'); }();   // ICAF_HALO=1: copies, no resident filter
-  const bool halo64 = pair_ok && halo_on && P.a_mode == A_TMA4D && P.cblk == 64 && g->kh == 3 && g->kw == 3 && g->stride == 1 &&
-                      g->pad == 1 && g->Cin % 64 == 0 &&
-                      double(g->Wo) * g->Ho >= 0.6 * (double((g->Wo + 7) / 8) * ((g->Ho + 15) / 16) * 128.0);
   int bn = 32;
-  if (halo64 && P.N >= 128 && pair_wanted(128)) bn = 128;
-  else if (P.N >= 256 && (ctas(256) >= 2 * sms || pair_wanted(256))) bn = 256;
-  else if (P.N > 64 && ctas(128) >= sms) bn = 128;
+  if (P.N > 64 && ctas(128) >= sms) bn = 128;
   else if (P.N > 32 && ctas(64) >= sms) bn = 64;
-  if (g_dbg_bn) bn = g_dbg_bn;
-  // Many tiles per SM: the persistent kernel overlaps main loop and epilogue across tiles (conv_persist.cu).
-  static const bool persist_on = []() { const char* e = getenv("ICAF_PERSISTENT"); return !(e && e[0] == '0'); }();
-  const bool persistent = persist_on && ctas(bn) >= 2 * sms && P.a_mode != A_GATHER;   // both operands by TMA
-  if (P.a_mode == A_TMA4D && P.cblk < 64 && !persistent) {      // small-Cin TMA staging exists in the persistent kernel only
-    P.a_mode = A_GATHER; P.tw = P.th = P.tiles_x = P.tiles_y = 0; P.cblk = 64;
-  }
-  // (A wave-tail scheme -- peel total % SMs tiles off into a split-K cluster launch -- was measured and dropped: these
-  // layers are bound by chip-wide L2->SM bandwidth, so a partly filled last wave just streams the same bytes through
-  // fewer, faster CTAs; the second launch only added its fixed cost: 65 -> 87 us on the 320-tile P4 3x3 layer.)
-  // The image stem (3x3 / s1 over the 16-channel space-to-depth frame) has its own kernel once a wave of tiles exists
-  // (conv_stem.cu: x-merged rows, four accumulators per tile, resident filter).  ICAF_STEM=0 keeps the generic kernels.
-  static const bool stem_on = []() { const char* e = getenv("ICAF_STEM"); return !(e && e[0] == '0'); }();
-  if (stem_on && P.dense16 && stem_eligible(g) &&
-      (long long)g->B * ((g->Wo / 4 + 7) / 8) * ((g->Ho + 15) / 16) * n_io >= sms / 2)
-    return plan_stem(P, g, n_io, pl);
-  if (pair_env && halo_on && P.a_mode == A_TMA4D && P.cblk < 64 && g->kh == 3 && g->kw == 3 && g->stride == 1 && g->pad == 1) {
-    // 16- / 32-channel 3x3 layers (the image stem over the space-to-depth frame): CTA pairs + halo copies, 64-wide tiles
-    const int tx = (g->Wo + 7) / 8, ty = (g->Ho + 15) / 16;
-    const long long pairs = (long long)g->B * tx * ty * ((P.N + 63) / 64) * n_io / 2;
-    if (double(g->Wo) * g->Ho >= 0.6 * (double(tx) * ty * 128.0) && (pair_env == 2 || pairs >= sms / 2)) {
-      P.halo = (bres_on && P.N <= 64) ? 2 : 1;           // 2: the filter (one 64-wide N tile, one channel block) stays resident
-      P.tw = 8;
-      P.th = 16;
-      P.tiles_x = tx;
-      P.tiles_y = ty;
-      return plan_pair<64>(P, g, n_io, pl);
-    }
-  }
-  if (pair_wanted(bn) && P.a_mode != A_GATHER) {
-    // 3x3 / stride 1 layers on 16 x 8 pixel tiles: every activation row is fetched three times instead of nine (conv_pair.cu)
-    if (halo64) {   // tiles may hang over the right / bottom edge (P5: 16 x 20)
-      // (resident filter, halo mode 2, measured slower here: 233 vs 209 us at Cin = 64, N = 64)
-      P.halo = 1;
-      P.tw = 8;
-      P.th = 16;
-      P.tiles_x = (g->Wo + 7) / 8;
-      P.tiles_y = (g->Ho + 15) / 16;
-    }
-    switch (bn) {
-      case 256: return plan_pair<256>(P, g, n_io, pl);
-      case 128: return plan_pair<128>(P, g, n_io, pl);
-      default: return plan_pair<64>(P, g, n_io, pl);
-    }
-  }
-  if (persistent) {
-    switch (bn) {
-      case 256: return plan_persist<256>(P, n_io, pl);
-      case 128: return plan_persist<128>(P, n_io, pl);
-      case 64: return plan_persist<64>(P, n_io, pl);
-      default: return plan_persist<32>(P, n_io, pl);
-    }
-  }
   switch (bn) {
-    case 256: return plan_tc<256>(P, n_io, pl);
     case 128: return plan_tc<128>(P, n_io, pl);
     case 64: return plan_tc<64>(P, n_io, pl);
     default: return plan_tc<32>(P, n_io, pl);
@@ -626,10 +528,6 @@ static int plan_conv(const icaf_conv_geom* g, int n_io, int sms, int pair_mode, 
 
 using namespace icaf;
 
-#ifdef ICAF_PROBE
-// Probe builds only (not part of the ABI, absent from the shipped library): kernel-stage switches + forced tile width.
-extern "C" void icaf_debug_set(int dbg, int bn) { g_dbg = dbg; g_dbg_bn = bn; }
-#endif
 
 extern "C" int icaf_conv2d_plan(const icaf_conv_geom* g, int n_io, int sm_count, int pair_mode, icaf_conv_plan* out) {
   if (!out) return set_error(ICAF_ERR_BAD_ARG, "conv2d_plan: null output");
@@ -637,11 +535,12 @@ extern "C" int icaf_conv2d_plan(const icaf_conv_geom* g, int n_io, int sm_count,
   int rc = fill_geom(g, n_io, P);
   if (rc) return rc;
   ConvPlan pl;
-  rc = plan_conv(g, n_io, sm_count, pair_mode, P, pl);
+  (void)pair_mode;
+  rc = plan_conv(g, n_io, sm_count, P, pl);
   if (rc) return rc;
   out->kernel = pl.kernel; out->bn = pl.bn; out->a_mode = P.a_mode;
   out->tile_w = P.tw; out->tile_h = P.th; out->tiles_x = P.tiles_x; out->tiles_y = P.tiles_y;
-  out->cblk = P.cblk; out->halo = P.halo; out->stages = P.stages; out->splits = P.splits;
+  out->cblk = P.cblk; out->halo = 0; out->stages = P.stages; out->splits = P.splits;
   out->grid_x = int(pl.grid_x); out->grid_y = int(pl.grid_y); out->grid_z = int(pl.grid_z); out->cluster = int(pl.cluster);
   out->smem_bytes = pl.smem; out->work_items = pl.total;
   return ICAF_OK;
@@ -653,25 +552,14 @@ extern "C" int icaf_conv2d_fwd(const icaf_conv_geom* g, const icaf_conv_io* io, 
   int rc = fill_params(g, io, n_io, P, w);
   if (rc) return rc;
   ConvPlan pl;
-  rc = plan_conv(g, n_io, sm_count_cached(), -1, P, pl);
+  rc = plan_conv(g, n_io, sm_count_cached(), P, pl);
   if (rc) return rc;
   cudaStream_t st = (cudaStream_t)stream;
-  const int key = pl.kernel * 1000 + pl.bn;
-  switch (key) {
-    case ICAF_KERNEL_PAIR * 1000 + 256: return launch_pair<256>(P, pl, w, g, n_io, st);
-    case ICAF_KERNEL_PAIR * 1000 + 128: return launch_pair<128>(P, pl, w, g, n_io, st);
-    case ICAF_KERNEL_PAIR * 1000 + 64: return launch_pair<64>(P, pl, w, g, n_io, st);
-    case ICAF_KERNEL_PERSIST * 1000 + 256: return launch_persist<256>(P, pl, w, g, n_io, st);
-    case ICAF_KERNEL_PERSIST * 1000 + 128: return launch_persist<128>(P, pl, w, g, n_io, st);
-    case ICAF_KERNEL_PERSIST * 1000 + 64: return launch_persist<64>(P, pl, w, g, n_io, st);
-    case ICAF_KERNEL_PERSIST * 1000 + 32: return launch_persist<32>(P, pl, w, g, n_io, st);
-    case ICAF_KERNEL_TC * 1000 + 256: return launch_tc<256>(P, pl, w, g, n_io, st);
-    case ICAF_KERNEL_TC * 1000 + 128: return launch_tc<128>(P, pl, w, g, n_io, st);
-    case ICAF_KERNEL_TC * 1000 + 64: return launch_tc<64>(P, pl, w, g, n_io, st);
-    case ICAF_KERNEL_TC * 1000 + 32: return launch_tc<32>(P, pl, w, g, n_io, st);
-    case ICAF_KERNEL_STEM * 1000 + 64:
-    case ICAF_KERNEL_STEM * 1000 + 32: return launch_stem(P, pl, w, g, n_io, st);
-    default: return set_error(ICAF_ERR_BAD_ARG, "conv2d: the planner produced an unknown kernel / tile width");
+  switch (pl.bn) {
+    case 128: return launch_tc<128>(P, pl, w, g, n_io, st);
+    case 64: return launch_tc<64>(P, pl, w, g, n_io, st);
+    case 32: return launch_tc<32>(P, pl, w, g, n_io, st);
+    default: return set_error(ICAF_ERR_BAD_ARG, "conv2d: the planner produced an unknown tile width");
   }
 }
 

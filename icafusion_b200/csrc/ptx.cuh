@@ -1,6 +1,6 @@
-// Thin inline-PTX wrappers for the sm_100a features the kernels use:
-// mbarrier, cp.async (LDGSTS), TMA (cp.async.bulk.tensor), tcgen05 (alloc / mma / commit / ld), proxy fences.
-// Bit layouts follow the PTX ISA (sm_100a) -- the same encodings CUTLASS' cute/arch/mma_sm100_desc.hpp documents.
+// Thin inline-PTX wrappers for the sm_90a features the kernels use:
+// mbarrier, cp.async (LDGSTS), TMA (cp.async.bulk.tensor), wgmma (descriptors / mma_async / fences), clusters, proxy fences.
+// Bit layouts follow the PTX ISA (sm_90a) -- the same encodings CUTLASS' cute/arch/mma_sm90_desc.hpp documents.
 #pragma once
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
@@ -70,7 +70,7 @@ __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepc
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 
 // ------------------------------------------------------------------ proxy fences
-// generic-proxy smem writes (st.shared / completed cp.async) -> visible to the async proxy (UMMA, TMA)
+// generic-proxy smem writes (st.shared / completed cp.async) -> visible to the async proxy (wgmma, TMA)
 __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
@@ -81,7 +81,6 @@ __device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, bool v
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(n) : "memory");
 }
 // Arrive on `bar` (counts as this thread's arrival, .noinc) once every cp.async this thread has issued so far has landed.
-// Non-blocking: the producer keeps issuing; this is how CUTLASS' sm100 cp.async mainloops hand stages to tcgen05.mma.
 __device__ __forceinline__ void cp_async_arrive_on(uint32_t bar) {
   asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(bar) : "memory");
 }
@@ -109,114 +108,112 @@ __device__ __forceinline__ void tma_load_4d(uint32_t dst, const void* tmap, uint
       : "memory");
 }
 
-// ------------------------------------------------------------------ tcgen05: TMEM allocation
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_alloc(uint32_t smem_dst) {   // one full warp
-  static_assert(kCols >= 32 && kCols <= 512 && (kCols & (kCols - 1)) == 0, "TMEM columns: power of two in [32,512]");
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_dst), "n"(kCols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {    // same warp that allocated
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(kCols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// ------------------------------------------------------------------ tcgen05: descriptors
-// Instruction descriptor, kind::f16, fp16 A/B (K-major both), fp32 accumulate.
-//  [4,6) D format 1=f32 | [7,10) A fmt 0=f16 | [10,13) B fmt 0=f16 | 15 A major 0=K | 16 B major 0=K
-//  [17,23) N>>3 | [24,29) M>>4
-__host__ __device__ constexpr uint32_t umma_idesc_f16(int M, int N) {
-  return (1u << 4) | (uint32_t(N >> 3) << 17) | (uint32_t(M >> 4) << 24);
-}
-// Shared-memory matrix descriptor for a K-major tile stored as rows of 128 B (64 halfs) with the 128-byte swizzle:
-// 8-row groups are 1024 B apart (SBO), LBO unused for swizzled K-major. bits [46,48) = 1 (sm_100 version),
-// [61,64) = 2 (SWIZZLE_128B). The tile base must be 1024-B aligned; stepping K by 16 halfs adds 32 B to the start.
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t saddr) {
-  uint64_t d = 0;
-  d |= uint64_t((saddr & 0x3FFFF) >> 4);        // start address  [0,14)
-  d |= uint64_t(1) << 16;                       // LBO (ignored)  [16,30)
-  d |= uint64_t(1024 >> 4) << 32;               // SBO            [32,46)
-  d |= uint64_t(1) << 46;                       // version
-  d |= uint64_t(2) << 61;                       // SWIZZLE_128B
-  return d;
-}
-
-// K-major tile whose rows are `row_bytes` (32 / 64 / 128) wide with the matching 32B / 64B / 128B swizzle: 8-row groups are
-// 8*row_bytes apart.  layout type field: 2 = SWIZZLE_128B, 4 = SWIZZLE_64B, 6 = SWIZZLE_32B.
-__device__ __forceinline__ uint64_t umma_desc_kmajor(uint32_t saddr, uint32_t row_bytes) {
-  const uint64_t lt = row_bytes == 128 ? 2 : (row_bytes == 64 ? 4 : 6);
+// ------------------------------------------------------------------ wgmma (4th-gen tensor cores, sm_90a)
+// Shared-memory matrix descriptor.  [0,14) start >> 4 | [16,30) LBO >> 4 | [32,46) SBO >> 4 | [62,64) layout:
+// 1 = SWIZZLE_128B, 2 = SWIZZLE_64B, 3 = SWIZZLE_32B (CUTLASS' GmmaDescriptor).  Swizzled tiles keep their 1024-byte
+// (512 / 256) atom alignment; stepping K by 16 halfs inside a K-major atom row adds 32 B to the start address.
+__device__ __forceinline__ uint64_t gmma_layout(uint32_t row_bytes) { return row_bytes == 128 ? 1 : (row_bytes == 64 ? 2 : 3); }
+// K-major tile whose rows are `row_bytes` (32 / 64 / 128) wide with the matching swizzle: 8-row groups are 8*row_bytes apart.
+__device__ __forceinline__ uint64_t gmma_desc_kmajor(uint32_t saddr, uint32_t row_bytes) {
   uint64_t d = 0;
   d |= uint64_t((saddr & 0x3FFFF) >> 4);
-  d |= uint64_t(1) << 16;
+  d |= uint64_t(1) << 16;                                   // LBO: unused by swizzled K-major layouts
   d |= uint64_t((8 * row_bytes) >> 4) << 32;
-  d |= uint64_t(1) << 46;
-  d |= lt << 61;
+  d |= gmma_layout(row_bytes) << 62;
   return d;
 }
-
-// MN-major operand tile (the M / N index is the contiguous one): rows of `row_bytes` (32 / 64 / 128) hold 16 / 32 / 64
-// consecutive M|N elements of ONE k, consecutive k are consecutive rows, 8-row groups are 8*row_bytes apart (SBO); the next
-// block of 64 (32, 16) M|N elements starts `lbo_bytes` further (LBO).  This is the layout a TMA box (cols = M|N, rows = k)
-// with the matching swizzle produces -- CUTLASS' Layout_MN_SW{32,64,128}_Atom.  One MMA (K = 16) spans two 8-row groups:
-// advance the start address by 16 * row_bytes per K step.  Needs the matching "major" bit in the instruction descriptor.
-__device__ __forceinline__ uint64_t umma_desc_mnmajor(uint32_t saddr, uint32_t row_bytes, uint32_t lbo_bytes) {
-  const uint64_t lt = row_bytes == 128 ? 2 : (row_bytes == 64 ? 4 : 6);
+__device__ __forceinline__ uint64_t gmma_desc_sw128(uint32_t saddr) { return gmma_desc_kmajor(saddr, 128); }
+// MN-major operand tile (the M / N index is the contiguous one): rows of `row_bytes` hold 16 / 32 / 64 consecutive M|N
+// elements of ONE k, consecutive k are consecutive rows, 8-row groups are 8*row_bytes apart (SBO); the next block of
+// 64 (32, 16) M|N elements starts `lbo_bytes` further (LBO).  This is the layout a TMA box (cols = M|N, rows = k) with the
+// matching swizzle produces.  One MMA (K = 16) spans two 8-row groups: advance the start by 16 * row_bytes per K step.
+// Needs the transpose flag of the wgmma for that operand.
+__device__ __forceinline__ uint64_t gmma_desc_mnmajor(uint32_t saddr, uint32_t row_bytes, uint32_t lbo_bytes) {
   uint64_t d = 0;
   d |= uint64_t((saddr & 0x3FFFF) >> 4);
   d |= uint64_t((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= uint64_t((8 * row_bytes) >> 4) << 32;
-  d |= uint64_t(1) << 46;
-  d |= lt << 61;
+  d |= gmma_layout(row_bytes) << 62;
   return d;
 }
-// kind::f16 instruction descriptor with MN-major A and / or B (bit 15 / bit 16)
-__host__ __device__ constexpr uint32_t umma_idesc_f16_major(int M, int N, bool a_mn, bool b_mn) {
-  return (1u << 4) | (a_mn ? (1u << 15) : 0u) | (b_mn ? (1u << 16) : 0u) | (uint32_t(N >> 3) << 17) | (uint32_t(M >> 4) << 24);
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+
+// D(64 x N, fp32, registers of the issuing warpgroup) (+)= A(64 x 16) * B(N x 16)^T, fp16 operands.
+//   wgmma_ss<TA, TB>: A and B from shared memory (descriptors); TA / TB = 1 for an MN-major operand.
+//   wgmma_rs<TB>    : A from registers (the accumulator layout of a previous wgmma, packed to half2: see below).
+// Accumulator layout (thread t of the warpgroup, w = t / 32, l = t % 32): d[i] is row 16w + l/4 + 8*((i >> 1) & 1),
+// column 8*(i >> 2) + 2*(l % 4) + (i & 1).  The register A operand of K-step kk is {d[8kk..8kk+1], d[8kk+2..+3],
+// d[8kk+4..+5], d[8kk+6..+7]} of a 64 x 16k accumulator, each pair packed to one half2.
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_ss(float (&d)[8], uint64_t ad, uint64_t bd, bool acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, %11, %12;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "l"(ad), "l"(bd), "r"(uint32_t(acc)), "n"(TA), "n"(TB));
+}
+template <int TB>
+__device__ __forceinline__ void wgmma_rs(float (&d)[8], const uint32_t (&a)[4], uint64_t bd, bool acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %13, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7}, {%8, %9, %10, %11}, %12, p, 1, 1, %14;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bd), "r"(uint32_t(acc)), "n"(TB));
 }
 
-// D[tmem] (+)= A[smem] * B[smem]^T ; issued by ONE thread.
-__device__ __forceinline__ void umma_f16_ss(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                            bool accumulate) {
-  uint32_t acc = accumulate ? 1u : 0u;
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_ss(float (&d)[16], uint64_t ad, uint64_t bd, bool acc) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(acc)
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, %19, %20;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(ad), "l"(bd), "r"(uint32_t(acc)), "n"(TA), "n"(TB));
 }
-// Arrive on an mbarrier when all tcgen05 ops issued so far by this thread have completed.
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
+template <int TB>
+__device__ __forceinline__ void wgmma_rs(float (&d)[16], const uint32_t (&a)[4], uint64_t bd, bool acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %21, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, {%16, %17, %18, %19}, %20, p, 1, 1, %22;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bd), "r"(uint32_t(acc)), "n"(TB));
 }
 
-// TMEM -> registers: this warp's 32 lanes x 32 consecutive fp32 columns (thread i gets lane base+i).
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_ss(float (&d)[32], uint64_t ad, uint64_t bd, bool acc) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-        "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-        "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, %35, %36;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(ad), "l"(bd), "r"(uint32_t(acc)), "n"(TA), "n"(TB));
 }
-// 16-column flavour (the persistent kernel double-buffers these against the epilogue math).
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
+template <int TB>
+__device__ __forceinline__ void wgmma_rs(float (&d)[32], const uint32_t (&a)[4], uint64_t bd, bool acc) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1, %38;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bd), "r"(uint32_t(acc)), "n"(TB));
 }
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_ss(float (&d)[64], uint64_t ad, uint64_t bd, bool acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, %67, %68;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(ad), "l"(bd), "r"(uint32_t(acc)), "n"(TA), "n"(TB));
+}
+template <int TB>
+__device__ __forceinline__ void wgmma_rs(float (&d)[64], const uint32_t (&a)[4], uint64_t bd, bool acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %69, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, {%64, %65, %66, %67}, %68, p, 1, 1, %70;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bd), "r"(uint32_t(acc)), "n"(TB));
+}
 
 __device__ __forceinline__ void prefetch_l2(const void* p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
@@ -240,15 +237,8 @@ __device__ __forceinline__ void st_cluster_v4(uint32_t addr, uint32_t a, uint32_
   asm volatile("st.shared::cluster.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
 }
 
-// ------------------------------------------------------------------ 256-bit global accesses (sm_100: LDG/STG.E.ENL2.256)
-// One full 32-byte L2 sector per lane and instruction; the pointer must be 32-byte aligned.
-__device__ __forceinline__ void st_global_v8(void* p, const uint32_t (&o)[8]) {
-  asm volatile("st.global.v8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(p), "r"(o[0]), "r"(o[1]), "r"(o[2]), "r"(o[3]),
-               "r"(o[4]), "r"(o[5]), "r"(o[6]), "r"(o[7]) : "memory");
-}
-__device__ __forceinline__ void ld_global_nc_v8(const void* p, uint32_t (&o)[8]) {
-  asm volatile("ld.global.nc.v8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];" : "=r"(o[0]), "=r"(o[1]), "=r"(o[2]), "=r"(o[3]),
-               "=r"(o[4]), "=r"(o[5]), "=r"(o[6]), "=r"(o[7]) : "l"(p));
+__device__ __forceinline__ void ld_cluster_v4(uint32_t addr, float4& v) {
+  asm volatile("ld.shared::cluster.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr) : "memory");
 }
 
 // ------------------------------------------------------------------ counter-based dropout mask of the attention probabilities

@@ -1,15 +1,15 @@
-// Convolution / linear weight gradient on the tcgen05 tensor cores (training step, train.py:344 `scaler.scale(loss).backward()`
+// Convolution / linear weight gradient on the Hopper tensor cores (training step, train.py:344 `scaler.scale(loss).backward()`
 // -> the wgrad of every nn.Conv2d / nn.Linear of the hot path):
 //     dW[n][ky][kx][c] = sum_{b,oy,ox} dY[b,oy,ox,n] * X[b, oy*s - p + ky, ox*s - p + kx, c]
 // As a GEMM the reduction runs over PIXELS, so both operands are "MN-major": a tile of 128 pixels x 64 channels arrives by
 // one TMA box exactly as it lies in the NHWC tensor (rows = pixels = the K index, channels contiguous) -- no transpose, no
 // im2col: the tap shift and the padding are the box coordinates / out-of-bounds zero fill, the stride is the box traversal
-// stride, like in the forward kernels.
+// stride, like in the forward kernels.  wgmma reads both operands transposed (MN-major descriptors).
 //   CTA work item = (128-wide n tile, <=128-wide c tile, filter tap, split): it walks its share of the 16 x 8 pixel tiles of
 //   the output map (one ring stage = dY box(es) + X box(es) of one tile, 8 MMAs of K = 16 pixels each), accumulates
-//   D[128 n][c tile] in TMEM and writes one fp32 partial; wgrad_reduce_kernel sums the splits in a fixed order into the
+//   D[128 n][c tile] in registers and writes one fp32 partial; wgrad_reduce_kernel sums the splits in a fixed order into the
 //   (Cout, Cin, kh, kw) fp32 gradient (deterministic: no atomics).
-// 192 threads: warps 0-3 epilogue, warp 4 TMEM + MMA issue, warp 5 TMA producer.
+// 288 threads: warps 0-7 two consumer warpgroups (n rows 0-63 / 64-127 of the tile), warp 8 TMA producer.
 #include <cstring>
 
 #include "icaf_internal.cuh"
@@ -30,14 +30,50 @@ struct WgradParams {
 };
 struct WgradMaps { CUtensorMap dy; CUtensorMap x; };
 
-__global__ void __launch_bounds__(192, 1) wgrad_kernel(const WgradParams P, const __grid_constant__ WgradMaps maps) {
+// CW = channels of the tile (16, 32, 64 or 128): the N of the wgmma
+template <int CW>
+__device__ __forceinline__ void wgrad_consume(const WgradParams& P, uint32_t smem_base, uint32_t bar_base, int mt_begin, int mt_end,
+                                              int split, int tap, int n0, int c0) {
+  auto full_bar = [&](int s) { return bar_base + 8u * s; };
+  auto empty_bar = [&](int s) { return bar_base + 8u * (4 + s); };
+  const int warp = threadIdx.x >> 5, g = warp >> 2, w = warp & 3, l = threadIdx.x & 31;
+  const uint32_t x_row_bytes = uint32_t(P.c_blk) * 2u;      // 128 B, or 64 / 32 B for 32- / 16-channel maps
+  const uint32_t x_blk_bytes = 128u * x_row_bytes;
+  float acc[CW / 2];
+#pragma unroll
+  for (int i = 0; i < CW / 2; ++i) acc[i] = 0.f;
+  int s = 0;
+  uint32_t ph = 0;
+  for (int mt = mt_begin; mt < mt_end; ++mt) {
+    mbar_wait(full_bar(s), ph);
+    const uint32_t sa = smem_base + s * kWStageBytes;
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {                       // 16 pixels per MMA: two 8-row groups of each operand
+      const uint64_t ad = gmma_desc_mnmajor(sa + g * kWTile + k * 16 * 128, 128, kWTile);
+      const uint64_t bd = gmma_desc_mnmajor(sa + 2 * kWTile + k * 16 * x_row_bytes, x_row_bytes, x_blk_bytes);
+      wgmma_ss<1, 1>(acc, ad, bd, true);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    if (l == 0) mbar_arrive(empty_bar(s));
+    if (++s == kWStages) { s = 0; ph ^= 1; }
+  }
+  // ---- epilogue: acc[i] is n row 64g + 16w + l/4 + 8*((i>>1)&1), channel 8*(i>>2) + 2*(l&3) + (i&1) ----
+#pragma unroll
+  for (int i = 0; i < CW / 2; i += 2) {
+    const int n = n0 + 64 * g + 16 * w + (l >> 2) + 8 * ((i >> 1) & 1);
+    float* dst = P.partial + ((size_t(split) * P.n_pad + n) * P.taps + tap) * P.c_pad + c0 + 8 * (i >> 2) + 2 * (l & 3);
+    *reinterpret_cast<float2*>(dst) = make_float2(acc[i], acc[i + 1]);   // an empty split writes zeros
+  }
+}
+
+__global__ void __launch_bounds__(288, 1) wgrad_kernel(const WgradParams P, const __grid_constant__ WgradMaps maps) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  uint8_t* smem_gen = smem_raw + (smem_base - smem_u32(smem_raw));
   const uint32_t bar_base = smem_base + kWStages * kWStageBytes;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (4 + s); };
-  const uint32_t accum_bar = bar_base + 64, tmem_slot = bar_base + 72;
 
   pdl_launch_dependents();
   const int warp = threadIdx.x >> 5, tid = threadIdx.x;
@@ -54,21 +90,16 @@ __global__ void __launch_bounds__(192, 1) wgrad_kernel(const WgradParams P, cons
   const int mt_begin = int((long long)P.m_tiles * split / P.splits), mt_end = int((long long)P.m_tiles * (split + 1) / P.splits);
 
   if (tid == 0) {
-    for (int s = 0; s < kWStages; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), 1); }
-    mbar_init(accum_bar, 1);
+    for (int s = 0; s < kWStages; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), 8); }   // 8 consumer warps
     fence_mbar_init();
   }
-  if (warp == 4) tmem_alloc<128>(tmem_slot);
-  if (warp == 5 && lane_id() == 0) { tma_prefetch_desc(&maps.dy); tma_prefetch_desc(&maps.x); }
-  tc_fence_before();
+  if (warp == 8 && lane_id() == 0) { tma_prefetch_desc(&maps.dy); tma_prefetch_desc(&maps.x); }
   __syncthreads();
-  tc_fence_after();
   pdl_wait();
-  const uint32_t tmem_d = *reinterpret_cast<volatile uint32_t*>(smem_gen + kWStages * kWStageBytes + 72);
-  const uint32_t x_row_bytes = uint32_t(P.c_blk) * 2u;      // 128 B, or 64 / 32 B for 32- / 16-channel maps
+  const uint32_t x_row_bytes = uint32_t(P.c_blk) * 2u;
   const uint32_t x_blk_bytes = 128u * x_row_bytes;
 
-  if (warp == 5) {
+  if (warp == 8) {
     if (lane_id() == 0) {
       int s = 0;
       uint32_t ph = 0;
@@ -92,57 +123,13 @@ __global__ void __launch_bounds__(192, 1) wgrad_kernel(const WgradParams P, cons
         if (++s == kWStages) { s = 0; ph ^= 1; }
       }
     }
-  } else if (warp == 4) {
-    const uint32_t idesc = umma_idesc_f16_major(128, cw, true, true);
-    int s = 0;
-    uint32_t ph = 0;
-    bool first = true;
-    for (int mt = mt_begin; mt < mt_end; ++mt) {
-      mbar_wait(full_bar(s), ph);
-      tc_fence_after();
-      if (elect_one()) {
-        const uint32_t sa = smem_base + s * kWStageBytes;
-#pragma unroll
-        for (int k = 0; k < 8; ++k) {                       // 16 pixels per MMA: two 8-row groups of each operand
-          const uint64_t ad = umma_desc_mnmajor(sa + k * 16 * 128, 128, kWTile);
-          const uint64_t bd = umma_desc_mnmajor(sa + 2 * kWTile + k * 16 * x_row_bytes, x_row_bytes, x_blk_bytes);
-          umma_f16_ss(tmem_d, ad, bd, idesc, !(first && k == 0));
-        }
-        umma_commit(empty_bar(s));
-      }
-      __syncwarp();
-      first = false;
-      if (++s == kWStages) { s = 0; ph ^= 1; }
-    }
-    if (elect_one()) umma_commit(accum_bar);
-    __syncwarp();
   } else {
-    // ------------------------------------------------------------------ epilogue: TMEM lane = n row of the tile
-    mbar_wait(accum_bar, 0);
-    tc_fence_after();
-    const int n = n0 + tid;
-    float* dst = P.partial + ((size_t(split) * P.n_pad + n) * P.taps + tap) * P.c_pad + c0;
-    const uint32_t trow = tmem_d + (uint32_t(warp * 32) << 16);
-    const bool any = mt_end > mt_begin;
-    for (int cb = 0; cb < cw; cb += 16) {
-      uint32_t acc[16];
-      __syncwarp();
-      tmem_ld16(trow + cb, acc);
-      tmem_ld_wait();
-      if (n < P.n_pad) {
-#pragma unroll
-        for (int q = 0; q < 4; ++q)
-          *reinterpret_cast<float4*>(dst + cb + 4 * q) = any ? make_float4(__uint_as_float(acc[4 * q]), __uint_as_float(acc[4 * q + 1]),
-                                                                           __uint_as_float(acc[4 * q + 2]), __uint_as_float(acc[4 * q + 3]))
-                                                             : make_float4(0.f, 0.f, 0.f, 0.f);
-      }
+    switch (cw) {      // multiples of c_blk: 128 / 64 for 64-channel blocks, else the whole (16 / 32 channel) map
+      case 128: wgrad_consume<128>(P, smem_base, bar_base, mt_begin, mt_end, split, tap, n0, c0); break;
+      case 64: wgrad_consume<64>(P, smem_base, bar_base, mt_begin, mt_end, split, tap, n0, c0); break;
+      case 32: wgrad_consume<32>(P, smem_base, bar_base, mt_begin, mt_end, split, tap, n0, c0); break;
+      default: wgrad_consume<16>(P, smem_base, bar_base, mt_begin, mt_end, split, tap, n0, c0); break;
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 4) {
-    tc_fence_after();
-    tmem_dealloc<128>(tmem_d);
   }
 }
 
@@ -308,7 +295,7 @@ extern "C" int icaf_conv2d_wgrad(const icaf_conv_geom* g, const void* x, int64_t
   static bool configured[kMaxDevices] = {false};
   if (int r2 = configure_smem(wgrad_kernel, kWSmem, configured, "wgrad: cudaFuncSetAttribute")) return r2;
   cudaStream_t st = (cudaStream_t)stream;
-  launch_k(wgrad_kernel, dim3(pl.grid), dim3(192), (size_t)kWSmem, st, P, maps);
+  launch_k(wgrad_kernel, dim3(pl.grid), dim3(288), (size_t)kWSmem, st, P, maps);
   if (int r3 = check_launch("conv2d_wgrad")) return r3;
   if (P.taps == 1) {
     launch_k(wgrad_reduce_flat_kernel, dim3((unsigned)(((long long)g->Cout * g->Cin + 255) / 256)), dim3(256), 0, st, (const float*)P.partial, dw, P.splits, P.n_pad,

@@ -319,6 +319,8 @@ class Model(nn.Module):
         if "_ir_start" not in self.__dict__:       # an unpickled checkpoint (models/experimental.py:118) never ran __init__
             self._plan_streams()
             self._plan_concats()
+        if not (ops.on_device(rgb) and ops.on_device(ir)):     # before any stream lookup: torch rejects a CPU device there
+            raise RuntimeError("icafusion_b200 runs on CUDA tensors only (no CPU fallback)")
         layers = list(self.model)
         y: List = [None] * len(layers)
         dev = rgb.device

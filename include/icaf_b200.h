@@ -1,5 +1,5 @@
 /*
- * icaf_b200 -- C ABI of the B200 (sm_100a) kernels for the ICAFusion hot path:
+ * icaf_b200 -- C ABI of the H100 (sm_90a) kernels for the ICAFusion hot path:
  * the two-stream CSPDarknet Conv+BN+SiLU backbone and the DMFF cross-attention fusion block.
  *
  * The reference (chanchanchan97/ICAFusion) is pure Python/PyTorch and has no FFI of its own; these
@@ -58,7 +58,7 @@ long long icaf_kernel_launches(void);
 int icaf_sm_count(void);
 
 /* ---------------------------------------------------------------------------------------------
- * Implicit-GEMM convolution / linear layer on the tcgen05 tensor cores.
+ * Implicit-GEMM convolution / linear layer on the Hopper tensor cores (wgmma).
  *   y[b,oy,ox,n] = epi( sum_{ky,kx,c} x[b, oy*s-p+ky, ox*s-p+kx, c] * w[n][(ky*kw+kx)*Cin + c] + bias[n] )
  * Replaces: Conv.forward / Conv.fuseforward (models/common.py:56-60: nn.Conv2d -> BatchNorm2d -> SiLU,
  * BN folded as utils/torch_utils.py:182-202), nn.Linear calls of CrossAttention / MLP
@@ -95,25 +95,21 @@ int icaf_conv2d_fwd(const icaf_conv_geom* g, const icaf_conv_io* io, int n_io, v
 
 /* The dispatcher's decision for one layer geometry, computed on the HOST only (no device, no stream, no pointers):
  * which kernel family runs it, with which tile shapes, grid and shared memory.  icaf_conv2d_fwd launches exactly the
- * plan this returns for (geometry, n_io, SM count of the current device, ICAF_PAIR switch); the same invariant checks
- * run in both, so a GPU-less test can walk every layer of a model through the dispatcher (tests/test_abi_cpu.py).
- * pair_mode: -1 = environment default (ICAF_PAIR), 0 = never CTA pairs, 1 = heuristic, 2 = pairs wherever possible. */
+ * plan this returns for (geometry, n_io, SM count of the current device); the same invariant checks run in both, so a
+ * GPU-less test can walk every layer of a model through the dispatcher (tests/test_abi_cpu.py).
+ * pair_mode: accepted for ABI stability and ignored (sm_90a has no CTA-pair MMA). */
 #define ICAF_KERNEL_TC 0      /* one 128 x BN tile per CTA, split-K clusters   (conv_gemm.cu)    */
-#define ICAF_KERNEL_PERSIST 1 /* one CTA per SM looping over tiles              (conv_persist.cu) */
-#define ICAF_KERNEL_PAIR 2    /* CTA pairs, tcgen05 cta_group::2, halo copies   (conv_pair.cu)    */
-#define ICAF_KERNEL_STEM 3    /* image stem over the space-to-depth frame, x-merged rows (conv_stem.cu); the plan
-                                 assumes a dense frame (pixel pitch 16), which icaf_conv2d_fwd checks on the pointers */
 typedef struct {
   int kernel;                            /* ICAF_KERNEL_*                                                     */
-  int bn;                                /* output-channel tile width (32/64/128/256)                         */
+  int bn;                                /* output-channel tile width (32/64/128)                             */
   int a_mode;                            /* activation staging: 0 cp.async gather, 1 2-D TMA, 2 4-D TMA       */
   int tile_w, tile_h, tiles_x, tiles_y;  /* 4-D TMA: output-pixel tile and tiles per image                    */
   int cblk;                              /* channels per TMA box                                              */
-  int halo;                              /* pair kernel: 0 tap boxes, 1 x-shifted halo copies, 2 + resident filter */
+  int halo;                              /* always 0 (halo copies belong to CTA-pair kernels)                 */
   int stages, splits;                    /* smem ring depth; split-K factor (= cluster size of the tc kernel) */
   int grid_x, grid_y, grid_z, cluster;   /* launch shape                                                      */
   int smem_bytes;                        /* dynamic shared memory per CTA                                     */
-  int work_items;                        /* tiles (tc/persist) or tile pairs (pair) the grid iterates over    */
+  int work_items;                        /* output tiles the grid covers                                      */
 } icaf_conv_plan;
 int icaf_conv2d_plan(const icaf_conv_geom* g, int n_io, int sm_count, int pair_mode, icaf_conv_plan* out);
 
@@ -261,7 +257,7 @@ int icaf_compute_loss_bwd(const void* const* p, int p_fp32, int p_ld, const int*
  * ------------------------------------------------------------------------------------------- */
 /* Weight gradient dW[n][c][ky][kx] (fp32, PyTorch layout) = (accumulate ? dW : 0) + scale * sum_pixels dy[.., n] * x[.. shifted .., c]
  * of the convolution / linear layer described by `g` (Cin 16, 32 or a multiple of 64; Cout % 8 == 0; stride 1 or 2).
- * x, dy: fp16 NHWC views (pixel pitch x_ld / dy_ld).  tcgen05 GEMM over pixels with both operands MN-major, split over
+ * x, dy: fp16 NHWC views (pixel pitch x_ld / dy_ld).  wgmma GEMM over pixels with both operands MN-major, split over
  * the pixel range, splits summed in a fixed order (deterministic).  scale: 1 / loss scale.  workspace: caller owned,
  * icaf_conv2d_wgrad_workspace_bytes(g) bytes, 16-byte aligned. */
 size_t icaf_conv2d_wgrad_workspace_bytes(const icaf_conv_geom* g);

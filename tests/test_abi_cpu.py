@@ -62,8 +62,7 @@ def test_missing_library_fails_loudly(monkeypatch, tmp_path):
 
 
 def test_shipped_library_has_no_probe_hooks_and_counts_launches():
-    """The stage switches of tools/conv_probe.py exist only in -DICAF_PROBE builds; the shipped library exports exactly the
-    header's symbols.  The launch tally behind bench.py's `gpu_launches` starts at zero and does not move on rejected calls."""
+    """The library exports no debug hook (icaf_debug_set) beyond the header's symbols.  The launch tally behind bench.py's `gpu_launches` starts at zero and does not move on rejected calls."""
     from icafusion_b200 import _lib
     L = _lib.lib()
     assert not hasattr(L, "icaf_debug_set")
@@ -100,36 +99,18 @@ def _dry_geometries(size: str, B: int, H: int = 512, W: int = 640):
 def _check_plan(g, n, pl, sms, tag):
     from icafusion_b200 import _lib
     where = f"{tag}: kernel {pl.kernel} bn {pl.bn} a_mode {pl.a_mode} halo {pl.halo}"
-    assert pl.kernel in (_lib.KERNEL_TC, _lib.KERNEL_PERSIST, _lib.KERNEL_PAIR, _lib.KERNEL_STEM) and pl.bn in (32, 64, 128, 256), where
+    assert pl.kernel == _lib.KERNEL_TC and pl.bn in (32, 64, 128), where
     assert 0 < pl.smem_bytes <= 227 * 1024, where
     assert pl.grid_x >= 1 and pl.grid_y >= 1 and pl.grid_z >= 1 and pl.stages >= 1, where
     ctas = pl.grid_x * pl.grid_y * pl.grid_z
-    if pl.kernel == _lib.KERNEL_STEM:      # the space-to-depth image stem: 16 rows x 8 super-pixels (= 32 pixels) per tile
-        assert (g.Cin, g.kh, g.kw, g.stride, g.pad) == (16, 3, 3, 1, 1) and g.Cout <= pl.bn <= 64 and g.Wo % 4 == 0, where
-        assert (pl.tile_w, pl.tile_h) == (32, 16) and pl.tiles_x * 32 >= g.Wo and pl.tiles_y * 16 >= g.Ho, where
-        assert pl.cluster == 1 and pl.grid_x <= sms and pl.work_items == g.B * pl.tiles_x * pl.tiles_y * n, where
-        return
     if pl.a_mode == 2:       # 4-D TMA tiles cover the output map with <= 128 pixels per tile
         assert 1 <= pl.tile_w * pl.tile_h <= 128, where
         assert pl.tiles_x * pl.tile_w >= g.Wo and pl.tiles_y * pl.tile_h >= g.Ho, where
         assert (pl.tiles_x - 1) * pl.tile_w < g.Wo and (pl.tiles_y - 1) * pl.tile_h < g.Ho, where
-        assert pl.cblk in (16, 32, 64) and g.Cin % pl.cblk == 0, where
-    if pl.halo:
-        assert pl.kernel == _lib.KERNEL_PAIR and pl.a_mode == 2 and (g.kh, g.kw, g.stride, g.pad) == (3, 3, 1, 1), where
-        assert (pl.tile_w, pl.tile_h) == (8, 16), where
-        assert (pl.tiles_x, pl.tiles_y) == ((g.Wo + 7) // 8, (g.Ho + 15) // 16), where
-    if pl.halo == 2:
-        assert g.Cin <= 64 and g.Cout <= pl.bn, where
-    if pl.kernel == _lib.KERNEL_PAIR:
-        assert pl.cluster == 2 and pl.grid_x % 2 == 0 and pl.grid_x <= sms and pl.a_mode in (1, 2), where
-        assert pl.grid_x // 2 <= pl.work_items, where
-    elif pl.kernel == _lib.KERNEL_PERSIST:
-        assert pl.cluster == 1 and pl.grid_x <= sms and pl.a_mode in (1, 2) and pl.grid_x <= pl.work_items, where
-    else:
-        assert pl.cluster == pl.splits and 1 <= pl.splits <= 8 and pl.grid_x % pl.splits == 0, where
-        if pl.a_mode == 2:
-            assert pl.cblk == 64, where
-        assert ctas == pl.work_items * pl.splits, where
+        assert pl.cblk == 64 and g.Cin % pl.cblk == 0, where
+    assert pl.halo == 0, where
+    assert pl.cluster == pl.splits and 1 <= pl.splits <= 8 and pl.grid_x % pl.splits == 0, where
+    assert ctas == pl.work_items * pl.splits, where
 
 
 @pytest.mark.parametrize("size,B", [("s", 1), ("s", 16), ("l", 1), ("l", 16)])
@@ -140,18 +121,16 @@ def test_dispatcher_plans_every_layer_geometry(size, B):
     assert len(geoms) >= 25 and n_calls >= 60
     kernels = set()
     for g, n, tag in geoms:
-        for sms in (148, 132):
+        for sms in (132, 148):
             for pair_mode in (0, 1, 2):
                 pl = _lib.ConvPlan()
                 rc = L.icaf_conv2d_plan(ctypes.byref(g), n, sms, pair_mode, ctypes.byref(pl))
                 assert rc == 0, f"{tag} (sms {sms}, pair mode {pair_mode}): {L.icaf_last_error().decode()}"
                 _check_plan(g, n, pl, sms, tag)
-                if pair_mode == 0:
-                    assert pl.kernel != _lib.KERNEL_PAIR
-                if sms == 148 and pair_mode == 1:
-                    kernels.add((pl.kernel, pl.halo))
-    if (size, B) == ("l", 16):     # the compute-bound config exercises every kernel family (tc, persistent, pair with and without halo copies, stem)
-        assert {(0, 0), (1, 0), (2, 0), (2, 1), (3, 0)} <= kernels, kernels
+                if sms == 132 and pair_mode == 1:
+                    kernels.add((pl.bn, pl.a_mode))
+    if (size, B) == ("l", 16):     # the compute-bound config exercises every tile width and every activation staging mode
+        assert {32, 64, 128} <= {k[0] for k in kernels} and {0, 1, 2} <= {k[1] for k in kernels}, kernels
 
 
 def test_dispatcher_plan_matches_small_and_odd_geometries():
@@ -168,11 +147,11 @@ def test_dispatcher_plan_matches_small_and_odd_geometries():
         for n in (1, 2):
             for pair_mode in (0, 1, 2):
                 pl = _lib.ConvPlan()
-                rc = L.icaf_conv2d_plan(ctypes.byref(g), n, 148, pair_mode, ctypes.byref(pl))
+                rc = L.icaf_conv2d_plan(ctypes.byref(g), n, 132, pair_mode, ctypes.byref(pl))
                 assert rc == 0, L.icaf_last_error().decode()
-                _check_plan(g, n, pl, 148, f"B{B} {Hi}x{Wi} {Cin}->{Cout} k{k}s{s}")
+                _check_plan(g, n, pl, 132, f"B{B} {Hi}x{Wi} {Cin}->{Cout} k{k}s{s}")
     bad = _lib.ConvGeom(1, 8, 8, 12, 8, 8, 16, 1, 1, 1, 0, 64, 32, 0, 0)
-    assert L.icaf_conv2d_plan(ctypes.byref(bad), 1, 148, -1, ctypes.byref(_lib.ConvPlan())) == 2
+    assert L.icaf_conv2d_plan(ctypes.byref(bad), 1, 132, -1, ctypes.byref(_lib.ConvPlan())) == 2
     assert L.icaf_conv2d_plan(ctypes.byref(g), 1, 0, -1, ctypes.byref(_lib.ConvPlan())) == 1
 
 
@@ -201,9 +180,9 @@ def test_training_step_dry_run_plans_every_geometry(size, B):
                 continue
             seen.add(key)
             pl = _lib.ConvPlan()
-            rc = L.icaf_conv2d_plan(ctypes.byref(g), n, 148, -1, ctypes.byref(pl))
+            rc = L.icaf_conv2d_plan(ctypes.byref(g), n, 132, -1, ctypes.byref(pl))
             assert rc == 0, f"{work['tag']}: {L.icaf_last_error().decode()}"
-            _check_plan(g, n, pl, 148, work["tag"])
+            _check_plan(g, n, pl, 132, work["tag"])
     n_bn = sum(isinstance(x, torch.nn.BatchNorm2d) for x in m.modules())
     assert count["icaf_bn_act_fwd"] == count["icaf_bn_act_bwd"] == n_bn
     # one weight gradient per Conv / Detect conv / live Linear (the three q, k, v projections of a modality share one GEMM)

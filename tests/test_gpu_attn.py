@@ -1,4 +1,4 @@
-"""Flash cross-attention (tcgen05) vs the CPU oracle and vs the on-device CUDA-core reference."""
+"""Flash cross-attention (wgmma) vs the CPU oracle and vs the on-device CUDA-core reference."""
 import math
 
 import pytest
@@ -37,7 +37,7 @@ def test_cross_attention(cuda_device, B, N, C):
     r_v = _oracle(qk_i, qk_v, vt_v, B, N, n_pad, C, h)      # RGB output: IR queries on RGB keys/values (common.py:670,682)
     r_i = _oracle(qk_v, qk_i, vt_i, B, N, n_pad, C, h)
     es, eo = max(err(s_v[:, :N], r_v), err(s_i[:, :N], r_i)), max(err(o_v[:, :N], r_v), err(o_i[:, :N], r_i))
-    print(f"\n[attention B{B} N{N} C{C} d{C // h}] tcgen05 {eo:.2e}  cuda-core {es:.2e}  (tol {TOL:.0e})")
+    print(f"\n[attention B{B} N{N} C{C} d{C // h}] wgmma {eo:.2e}  cuda-core {es:.2e}  (tol {TOL:.0e})")
     assert es < TOL, "CUDA-core reference disagrees with the oracle"
     assert eo < TOL
     if n_pad > N:
@@ -62,6 +62,6 @@ def test_cross_attention_fused_qkv(cuda_device, B, N, C):
     r_v = _oracle(qkv_i[:, :, :2 * C], qkv_v[:, :, :2 * C], vt(qkv_v), B, N, n_pad, C, h)
     r_i = _oracle(qkv_v[:, :, :2 * C], qkv_i[:, :, :2 * C], vt(qkv_i), B, N, n_pad, C, h)
     es, eo = max(err(s_v[:, :N], r_v), err(s_i[:, :N], r_i)), max(err(o_v[:, :N], r_v), err(o_i[:, :N], r_i))
-    print(f"\n[attention fused-qkv B{B} N{N} C{C} d{C // h}] tcgen05 {eo:.2e}  cuda-core {es:.2e}  (tol {TOL:.0e})")
+    print(f"\n[attention fused-qkv B{B} N{N} C{C} d{C // h}] wgmma {eo:.2e}  cuda-core {es:.2e}  (tol {TOL:.0e})")
     assert es < TOL, "CUDA-core reference disagrees with the oracle"
     assert eo < TOL

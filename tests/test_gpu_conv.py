@@ -1,4 +1,4 @@
-"""tcgen05 implicit-GEMM conv / linear kernel vs the CPU oracle (torch fp32 conv on the same fp16-rounded
+"""wgmma implicit-GEMM conv / linear kernel vs the CPU oracle (torch fp32 conv on the same fp16-rounded
 operands) and vs the on-device CUDA-core reference.  All calls go through the C ABI."""
 import pytest
 import torch
@@ -42,28 +42,28 @@ CASES = [
     (1, 32, 16, 20, 96, 1, 1, 0, 1),      # 1x1 via 2-D TMA with Cin < 64 and N not a multiple of the tile (TMA zero fill)
     (2, 64, 32, 40, 128, 3, 2, 1, 1),     # 3x3 stride 2 via 4-D TMA (traversal stride 2, negative start coordinate)
     (2, 128, 32, 40, 64, 3, 1, 1, 1),     # 3x3 stride 1 via 4-D TMA, tile 16 rows x 8 cols, two K blocks per tap
-    (16, 64, 32, 40, 512, 1, 1, 0, 1),    # BN=256 tiles (1 CTA/SM, 256 TMEM columns)
+    (16, 64, 32, 40, 512, 1, 1, 0, 1),    # BN=128 tiles, one CTA per SM (128 accumulator registers per consumer thread)
     (1, 64, 16, 20, 64, 3, 1, 1, 1),      # 20-wide map: 6x20 tiles (120 of 128 MMA rows, last tile hangs over the map), split-K
     (2, 128, 16, 20, 128, 3, 2, 1, 1),    # stride 2 onto an 8x10 map: 10-wide tiles
     (1, 512, 16, 20, 512, 3, 1, 1, 1),    # P5 of yolov5l at batch 1: 72 K blocks over an 8-CTA cluster (DSMEM split-K reduction)
     (1, 2048, 1, 104, 512, 1, 1, 0, 0),   # MLP fc2 shape (rows as pixels): K=2048, split-K over clusters, 2-D TMA
-    (8, 64, 64, 80, 64, 3, 1, 1, 1),      # 3x3/s1 on 64 channels, 640 tiles of 16x8: CTA-pair kernel with halo copies, BN=64
+    (8, 64, 64, 80, 64, 3, 1, 1, 1),      # 3x3/s1 on 64 channels, 640 4-D TMA tiles, BN=64 (two CTAs per SM)
     (8, 3, 128, 160, 32, 6, 2, 2, 1),     # 320 tiles, cp.async gather (6x6 image stem on the packed NHWC4 image), BN=32
-    (4, 128, 64, 80, 256, 3, 2, 1, 1),    # persistent, 4-D TMA stride 2, BN=128, 18 K blocks per tile
-    (3, 64, 100, 84, 96, 1, 1, 0, 2),     # persistent, 2-D TMA, ragged M (25200 rows) and N (96), GELU
-    (8, 32, 64, 80, 64, 3, 1, 1, 1),      # persistent, small-Cin TMA staging: per-tap boxes of 32 channels, 64-byte swizzle
+    (4, 128, 64, 80, 256, 3, 2, 1, 1),    # 4-D TMA stride 2, BN=128, 18 K blocks per tile
+    (3, 64, 100, 84, 96, 1, 1, 0, 2),     # 2-D TMA, ragged M (25200 rows) and N (96), GELU
+    (8, 32, 64, 80, 64, 3, 1, 1, 1),      # 32 channels: cp.async gather, one K block spans two taps
     (8, 32, 128, 160, 64, 3, 2, 1, 1),    # ... stride 2 (yolov5s layer 1 geometry)
-    (8, 16, 64, 80, 32, 3, 1, 1, 1),      # ... 16 channels, 32-byte swizzle, K = 144 (tail K block holds one tap)
+    (8, 16, 64, 80, 32, 3, 1, 1, 1),      # ... 16 channels, K = 144 (tail K block holds one tap)
     (1, 16, 16, 20, 32, 3, 1, 1, 1),      # 16 channels on a small grid: cp.async gather path
-    (16, 256, 32, 40, 256, 3, 1, 1, 1),   # 320 BN=128 persistent tiles on 148 SMs (ragged last wave), 36 K blocks, N split over both epilogue column halves
-    (19, 1024, 32, 64, 256, 1, 1, 0, 0),  # 304 BN=256 tiles -> CTA-pair kernel (cta_group::2), 2-D TMA, K=1024, no activation
-    (32, 128, 32, 40, 256, 3, 1, 1, 1),   # CTA-pair kernel, 4-D TMA (16x8 tiles), 320 M tiles = 160 pairs
-    (1, 64, 301, 128, 512, 1, 1, 0, 1),   # CTA-pair kernel, odd M-tile count (301): the last pair's peer tile is all padding
-    (99, 64, 16, 24, 256, 3, 1, 1, 1),    # CTA-pair kernel, 4-D TMA, 297 M tiles: peer tile past the last image
-    (16, 512, 16, 20, 512, 3, 1, 1, 1),   # yolov5l P5 at batch 16: CTA pairs + halo copies, 16x8 tiles hang over the 20-wide map
-    (4, 16, 128, 160, 64, 3, 1, 1, 1),    # space-to-depth stem kernel (x-merged rows), N = 64, 200 tiles
-    (12, 16, 50, 36, 48, 3, 1, 1, 0),     # stem kernel, ragged: 9 super-pixels per row (tiles hang over), 50 rows, N = 48, no activation
-    (2, 16, 256, 320, 32, 3, 1, 1, 1),    # stem kernel at the yolov5s frame size, N = 32
+    (16, 256, 32, 40, 256, 3, 1, 1, 1),   # 640 BN=128 tiles on 132 SMs (ragged last wave), 36 K blocks
+    (19, 1024, 32, 64, 256, 1, 1, 0, 0),  # 2-D TMA, K=1024, no activation
+    (32, 128, 32, 40, 256, 3, 1, 1, 1),   # 4-D TMA (16x8 tiles), 320 M tiles
+    (1, 64, 301, 128, 512, 1, 1, 0, 1),   # odd M-tile count (301)
+    (99, 64, 16, 24, 256, 3, 1, 1, 1),    # 4-D TMA, 297 M tiles
+    (16, 512, 16, 20, 512, 3, 1, 1, 1),   # yolov5l P5 at batch 16: 6x20 tiles, the last tile row of each image hangs over
+    (4, 16, 128, 160, 64, 3, 1, 1, 1),    # image stem over the space-to-depth frame (16 channels, gather), N = 64
+    (12, 16, 50, 36, 48, 3, 1, 1, 0),     # stem geometry, ragged: 36-wide map, 50 rows, N = 48, no activation
+    (2, 16, 256, 320, 32, 3, 1, 1, 1),    # stem geometry at the yolov5s frame size, N = 32
 ]
 
 
@@ -79,7 +79,7 @@ def test_conv_matches_oracle(cuda_device, case):
     torch.cuda.synchronize()
     ref = _ref(x, w, b, s, p, act)
     e_simt, e_tc = err(nchw(y_simt), ref), err(nchw(y), ref)
-    print(f"\n[conv {case}] tcgen05 {e_tc:.2e}  cuda-core {e_simt:.2e}")
+    print(f"\n[conv {case}] wgmma {e_tc:.2e}  cuda-core {e_simt:.2e}")
     assert e_simt < TOL, "CUDA-core reference kernel disagrees with the oracle"
     assert e_tc < TOL
     assert err(y, y_simt) < TOL
@@ -107,24 +107,8 @@ def test_grouped_residual_and_slices(cuda_device):
         assert float(xs[i][..., :C].abs().max()) == 0 and float(xs[i][..., 2 * C:].abs().max()) == 0   # neighbours untouched
 
 
-def test_conv_suite_with_pairs_everywhere(cuda_device):
-    """The same conv cases with ICAF_PAIR=all: the CTA-pair kernel (BN 64/128/256, 2-D and 4-D TMA, ragged N, odd tile
-    counts, single-pair grids) replaces every persistent / one-tile launch it can run, and the DMFF block tests with it
-    (row bias, GELU, learnable-coefficient residual epilogues).  The switch is read once per process, hence the subprocess."""
-    import os
-    import subprocess
-    import sys
-    if os.environ.get("ICAF_PAIR") == "all":
-        pytest.skip("already inside the pairs-everywhere run")
-    env = dict(os.environ, ICAF_PAIR="all")
-    here = os.path.dirname(os.path.abspath(__file__))
-    r = subprocess.run([sys.executable, "-m", "pytest", os.path.abspath(__file__), os.path.join(here, "test_gpu_dmff.py"), "-q", "-m", "gpu",
-                        "-x", "-k", "matches_oracle or grouped or dmff"], env=env, capture_output=True, text=True, timeout=900)
-    assert r.returncode == 0, r.stdout[-3000:] + r.stderr[-2000:]
-
-
 def test_pair_kernel_grouped_residual(cuda_device):
-    """CTA-pair kernel with two problems per launch (RGB / IR streams) and the fused Bottleneck residual."""
+    """Wide-tile (BN = 128) launch with two problems (RGB / IR streams) and the fused Bottleneck residual."""
     from icafusion_b200 import ops
     B, C, H, W = 16, 256, 32, 40
     xs, packs, ress, refs = [], [], [], []
@@ -142,8 +126,8 @@ def test_pair_kernel_grouped_residual(cuda_device):
 
 @pytest.mark.parametrize("B,H,W,Cout", [(1, 64, 80, 32), (8, 256, 320, 32), (2, 128, 160, 64)])
 def test_stem_space_to_depth(cuda_device, B, H, W, Cout):
-    """Image stem Conv(3, c, 6, 2, 2) run as a 3x3/s1/p1 conv over the space-to-depth image (small grid: gather path,
-    large grid: persistent kernel with 16-channel TMA boxes) vs the plain 6x6 stride-2 convolution on the CPU."""
+    """Image stem Conv(3, c, 6, 2, 2) run as a 3x3/s1/p1 conv over the 16-channel space-to-depth image (cp.async gather
+    path) vs the plain 6x6 stride-2 convolution on the CPU."""
     from icafusion_b200 import ops
     x, w, b = _mk(B, 3, H, W, Cout, 6, 2, 2, seed=5)
     pk = ops.pack_stem_weight(w.float(), b, 1, device=cuda_device)
@@ -156,7 +140,7 @@ def test_stem_space_to_depth(cuda_device, B, H, W, Cout):
 
 
 def test_persistent_grouped_residual(cuda_device):
-    """Persistent kernel with two problems per launch, fused residual and channel-slice output (640 tiles)."""
+    """Many tiles (640) with two problems per launch, fused residual and channel-slice output."""
     from icafusion_b200 import ops
     B, C, H, W = 8, 64, 64, 80
     packs, xin, ress, outs, refs = [], [], [], [], []

@@ -11,7 +11,8 @@ from icafusion_b200.common import AdaptivePool2d, Conv
 from icafusion_b200.yolo_test import fuse_conv_and_bn
 from oracle import icaf_oracle as O
 from oracle import synth
-from oracle.ref_shim import REF_ROOT, reference_available
+
+from conftest import GOLDEN
 
 
 @pytest.mark.parametrize("size", ["s", "l"])
@@ -31,13 +32,14 @@ def test_state_dict_layout_matches_reference(size):
     assert abs(n_params / 1e6 - (23.26 if size == "s" else 120.25)) < 0.01     # SURVEY.md section 8(a)
 
 
-@pytest.mark.skipif(not reference_available(), reason="reference tree only exists in the build container")
 @pytest.mark.parametrize("size", ["s", "l"])
 def test_generated_cfg_equals_reference_yaml(size):
-    import yaml
-    with open(os.path.join(REF_ROOT, "models", "transformer", f"yolov5{size}_Transfusion_kaist.yaml")) as f:
-        ref = yaml.safe_load(f)
-    mine = transfusion_kaist_cfg(size)
+    """transfusion_kaist_cfg == the reference's YAML (models/transformer/yolov5{s,l}_Transfusion_kaist.yaml as parsed by
+    yaml.safe_load, stored in tests/golden/reference_yaml.json by oracle/gen_golden_dropin.py)."""
+    import json
+    with open(os.path.join(GOLDEN, "reference_yaml.json")) as f:
+        ref = json.load(f)[size]
+    mine = json.loads(json.dumps(transfusion_kaist_cfg(size)))      # the same JSON round trip (tuples -> lists)
     for k in ("nc", "depth_multiple", "width_multiple", "anchors", "backbone", "head"):
         assert mine[k] == ref[k], k
 
