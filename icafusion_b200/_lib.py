@@ -32,7 +32,7 @@ class ConvIO(C.Structure):
 class ConvPlan(C.Structure):
     _fields_ = [(n, C.c_int) for n in ("kernel", "bn", "a_mode", "tile_w", "tile_h", "tiles_x", "tiles_y", "cblk", "halo",
                                        "stages", "splits", "grid_x", "grid_y", "grid_z", "cluster", "smem_bytes",
-                                       "work_items")]
+                                       "work_items", "ctas")]
 
 
 class LossHyp(C.Structure):

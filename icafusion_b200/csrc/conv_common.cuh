@@ -30,6 +30,7 @@ struct ConvParams {
   int cblk;                               // A_TMA4D: channels per TMA box (64)
   int ln_parts;                           // LN fold: partials per input row (0 = no fold)
   float ln_eps, ln_inv_k;                 // LN fold: epsilon, 1 / (normalised features = K)
+  int m_tiles, n_tiles, tiles;            // persistent kernel: tile grid (m, n, problem) and its product
 };
 struct ConvMaps {          // TMA descriptors, passed by value as a __grid_constant__ kernel parameter
   CUtensorMap w[2];
@@ -150,6 +151,8 @@ struct ConvPlan {
   int smem;                       // dynamic shared memory per CTA (bytes)
   int total, m_tiles, m_pairs, n_tiles;
   int sms;                        // SM count the plan was made for
+  bool persist;                   // conv_gemm_persist_kernel: `ctas` CTAs walk the grid_x * grid_y * grid_z tiles
+  int ctas;                       // CTAs the launch starts
 };
 
 }  // namespace icaf

@@ -19,6 +19,8 @@
 // Pipelines: smem ring full[]/empty[] (producers <-> consumer), named barrier (staged accumulator -> epilogue).  Small
 // tiles (BN <= 64) let two CTAs share an SM so that one CTA's epilogue overlaps the other's main loop.  Split-K: the
 // CTAs of a cluster take a K range each; the leader adds the others' staged tiles through distributed shared memory.
+// conv_gemm_persist_kernel: BN = 128 grids of more than one wave with TMA-staged A -- one persistent CTA per SM, a TMA
+// producer warpgroup and two consumer warpgroups that take turns on the main loop (see its own comment below).
 #include <cstdlib>
 #include <cstring>
 
@@ -322,6 +324,253 @@ conv_gemm_tc_kernel(const ConvParams P, const __grid_constant__ ConvMaps maps) {
 }
 
 // ---------------------------------------------------------------------------------------------------
+// conv_gemm_persist_kernel: the 128 x 128 tile of grids that take more than one wave (TMA-staged A, no split-K).
+// grid = min(tiles, SMs) CTAs; CTA c walks the tiles c, c + G, c + 2G, ... of the whole launch, n-tile fastest, then
+// m-tile, then problem, so that the CTAs resident at the same time read the same A rows.  384 threads:
+//   warpgroup 0    : TMA producer (one elected thread), running straight on from one tile's K blocks into the next one's
+//   warpgroups 1, 2: consumers; warpgroup 1 + (j % 2) owns the CTA's j-th tile.  An ordering barrier hands the main loop
+//                    from one consumer to the other, so one warpgroup's epilogue runs while the other's MMAs run.  The
+//                    epilogue stages the accumulators through the warpgroup's own smem buffer 32 columns at a time
+//                    (thread t owns tile row t).
+// The main loop (MMA sequence, K order) and the epilogue arithmetic are those of conv_gemm_tc_kernel<128, XM>.
+constexpr int kPersistThreads = 384;
+struct PersistLayout {
+  static constexpr int kStageBytes = SmemLayout<128>::kStageBytes;
+  static constexpr int kPitch = 32 + 4;                        // floats per staged row of a 32-column chunk
+  static constexpr int kChunkBytes = BM * kPitch * 4;
+  // [ring: stages x (A|B)] [2 x staged chunk] [barriers 256 B] [2 x bias 128 fp32] ; + 1024 B alignment slack
+  __host__ __device__ static int bar_off(int stages) { return stages * kStageBytes + 2 * kChunkBytes; }
+  static int total(int stages) { return bar_off(stages) + 256 + 2 * 128 * 4 + 1024; }
+};
+
+struct TileOrigin { int z, n0, m0, tb, oy0, ox0; };
+__device__ __forceinline__ TileOrigin tile_origin(const ConvParams& P, int t) {
+  TileOrigin o;
+  const int r = t / P.n_tiles;
+  const int mtile = r % P.m_tiles;
+  o.n0 = (t - r * P.n_tiles) * 128;
+  o.z = r / P.m_tiles;
+  o.m0 = mtile * BM; o.tb = 0; o.oy0 = 0; o.ox0 = 0;
+  if (P.a_mode == A_TMA4D) {
+    const int per_img = P.tiles_x * P.tiles_y;
+    o.m0 = 0;
+    o.tb = mtile / per_img;
+    const int u = mtile - o.tb * per_img;
+    o.oy0 = (u / P.tiles_x) * P.th;
+    o.ox0 = (u % P.tiles_x) * P.tw;
+  }
+  return o;
+}
+
+// columns [32 CC, 32 CC + 32) of the warpgroup's accumulators -> staged rows (accumulator layout: see ptx.cuh)
+template <int CC>
+__device__ __forceinline__ void stage_chunk(const float (&acc0)[64], const float (&acc1)[64], float* sacc, int w, int l) {
+#pragma unroll
+  for (int i = 16 * CC; i < 16 * CC + 16; i += 2) {
+    const int r = 16 * w + (l >> 2) + 8 * ((i >> 1) & 1), col = 8 * (i >> 2) - 32 * CC + 2 * (l & 3);
+    *reinterpret_cast<float2*>(sacc + r * PersistLayout::kPitch + col) = make_float2(acc0[i], acc0[i + 1]);
+    *reinterpret_cast<float2*>(sacc + (r + 64) * PersistLayout::kPitch + col) = make_float2(acc1[i], acc1[i + 1]);
+  }
+}
+
+template <bool XM>
+__global__ void __launch_bounds__(kPersistThreads, 1)
+conv_gemm_persist_kernel(const ConvParams P, const __grid_constant__ ConvMaps maps) {
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  using L = SmemLayout<128>;
+  using PL = PersistLayout;
+  const int kStages = P.stages;
+  const uint32_t bar_off = uint32_t(PL::bar_off(kStages));
+  const uint32_t bar_base = smem_base + bar_off;
+  auto full_bar = [&](int s) { return bar_base + 8u * s; };
+  auto empty_bar = [&](int s) { return bar_base + 8u * (kMaxStages + s); };
+  auto order_bar = [&](int c) { return bar_base + 8u * (2 * kMaxStages + c); };   // consumer c may start its main loop
+  uint8_t* smem_gen = smem_raw + (smem_base - smem_u32(smem_raw));
+
+  pdl_launch_dependents();
+  const int tid = threadIdx.x;
+  const int wg = tid >> 7;
+  const int nkb = P.k_pad / BK;
+  const int a_mode = P.a_mode;
+  if (tid == 0) {
+    for (int s = 0; s < kStages; ++s) {
+      mbar_init(full_bar(s), 1);
+      mbar_init(empty_bar(s), 4);                             // one arrival per warp of the consuming warpgroup
+    }
+    mbar_init(order_bar(0), 4);
+    mbar_init(order_bar(1), 4);
+    fence_mbar_init();
+  }
+  if (tid == 32) {
+    tma_prefetch_desc(&maps.w[0]);
+    tma_prefetch_desc(&maps.a[0]);
+    if (P.tiles > P.m_tiles * P.n_tiles) { tma_prefetch_desc(&maps.w[1]); tma_prefetch_desc(&maps.a[1]); }
+  }
+  __syncthreads();
+  pdl_wait();   // prologue (barriers, descriptor prefetch) overlapped the previous kernel
+
+  if (wg == 0) {
+    // ------------------------------------------------------------------ TMA producer (warp 0, one thread)
+    setmaxnreg_dec<40>();
+    if (tid < 32 && elect_one()) {
+      const uint32_t a_bytes = a_mode == A_TMA2D ? L::kABytes : uint32_t(P.tw * P.th) * 128u;
+      const uint32_t bytes = L::kBBytes + a_bytes;
+      int s = 0;
+      uint32_t ph = 0;
+      for (int tile = blockIdx.x; tile < P.tiles; tile += gridDim.x) {
+        const TileOrigin o = tile_origin(P, tile);
+        const CUtensorMap* mw = o.z ? &maps.w[1] : &maps.w[0];
+        const CUtensorMap* ma = o.z ? &maps.a[1] : &maps.a[0];
+        for (int kb = 0; kb < nkb; ++kb) {
+          mbar_wait_quiet(empty_bar(s), ph ^ 1);
+          const uint32_t sa = smem_base + s * L::kStageBytes;
+          mbar_arrive_expect_tx(full_bar(s), bytes);
+          tma_load_2d(sa + L::kABytes, mw, full_bar(s), kb * BK, o.n0);
+          if (a_mode == A_TMA2D) {
+            tma_load_2d(sa, ma, full_bar(s), kb * BK, o.m0);
+          } else {
+            const int k0 = kb * BK;
+            const int tap = k0 / P.Cin;
+            const int ch = k0 - tap * P.Cin;
+            const int ky = tap / P.kw, kx = tap - ky * P.kw;
+            tma_load_4d(sa, ma, full_bar(s), ch, o.ox0 * P.stride - P.pad + kx, o.oy0 * P.stride - P.pad + ky, o.tb);
+          }
+          if (++s == kStages) { s = 0; ph ^= 1; }
+        }
+      }
+    }
+    return;
+  }
+
+  // -------------------------------------------------------------------- consumer warpgroups (wgmma + epilogue)
+  setmaxnreg_inc<232>();
+  const int c = wg - 1;
+  const int t = tid & 127, w = t >> 5, l = t & 31;
+  const int bar_id = 2 + c;                                   // warpgroup-local named barrier
+  float* sacc = reinterpret_cast<float*>(smem_gen + kStages * L::kStageBytes + c * PL::kChunkBytes);
+  float* sbias = reinterpret_cast<float*>(smem_gen + bar_off + 256 + c * 128 * 4);
+  for (int tile = blockIdx.x + c * gridDim.x; tile < P.tiles; tile += 2 * gridDim.x) {
+    const int j = (tile - int(blockIdx.x)) / int(gridDim.x);  // ordinal of the tile among this CTA's tiles
+    const TileOrigin o = tile_origin(P, tile);
+    const ConvProblem pr = pick_problem(P, o.z);
+    const int n0 = o.n0;
+    // Epilogue operands that do not depend on the main loop are fetched now so their DRAM latency hides behind it:
+    // bias slice and (alpha, beta) into registers, this thread's residual row into L2.
+    const float bias_r = (pr.bias && !(P.epi & ICAF_EPI_BIAS_ROW) && n0 + t < P.N) ? __ldg(pr.bias + n0 + t) : 0.f;
+    float alpha = 0.f, beta = 1.f;
+    if (P.epi & ICAF_EPI_SCALED_RES) { alpha = __ldg(pr.alpha); beta = __ldg(pr.beta); }
+    const int row = t;
+    int m;
+    bool mvalid;
+    if (a_mode == A_TMA4D) {
+      const int ry = row / P.tw, rx = row - ry * P.tw;
+      m = (o.tb * P.Ho + o.oy0 + ry) * P.Wo + o.ox0 + rx;
+      mvalid = ry < P.th && o.oy0 + ry < P.Ho;    // tw divides Wo; the last tile row of an image may hang over
+    } else {
+      m = o.m0 + row;
+      mvalid = m < P.M;
+    }
+    const float rbias = ((P.epi & ICAF_EPI_BIAS_ROW) && pr.bias && mvalid) ? __ldg(pr.bias + m) : 0.f;
+    __half* yrow = pr.y + size_t(mvalid ? m : 0) * pr.y_ld;
+    const __half* rrow = pr.res ? pr.res + size_t(mvalid ? m : 0) * pr.res_ld : nullptr;
+    const int mode = (P.epi & ICAF_EPI_SCALED_RES) ? 2 : (rrow ? 1 : 0);
+    if (rrow && mvalid) {
+      for (int cb = 0; cb < 128 && n0 + cb < P.N; cb += 64) prefetch_l2(rrow + n0 + cb);
+    }
+    EpiRow ex;
+    ex.sum = ex.sumsq = 0.f; ex.ln_a = 1.f; ex.ln_mu = 0.f; ex.ln_s = nullptr;
+    if (XM) {
+      ex.ln_s = pr.ln_s ? pr.ln_s + n0 : nullptr;
+      if (P.ln_parts > 0) epi_row_ln(ex, P, pr, m, mvalid);
+    }
+
+    // ---- main loop.  Tile j's K blocks are ring blocks j*nkb ... j*nkb + nkb - 1.  Waiting for the other consumer's
+    // turn also guarantees that every earlier ring block has been seen full, so the parity waits below cannot alias.
+    float acc0[64], acc1[64];
+#pragma unroll
+    for (int i = 0; i < 64; ++i) { acc0[i] = 0.f; acc1[i] = 0.f; }
+    const int g0 = j * nkb;
+    int s = g0 % kStages, s_prev = s;
+    uint32_t ph = uint32_t(g0 / kStages) & 1u;
+    if (j > 0) mbar_wait_quiet(order_bar(c), uint32_t((j >> 1) - (1 - c)) & 1u);
+    for (int kb = 0; kb < nkb; ++kb) {
+      mbar_wait_quiet(full_bar(s), ph);
+      const uint32_t sa = smem_base + s * L::kStageBytes;
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < BK / 16; ++k) {
+        const uint64_t bd = gmma_desc_sw128(sa + L::kABytes + 32 * k);
+        wgmma_ss<0, 0>(acc0, gmma_desc_sw128(sa + 32 * k), bd, (kb | k) != 0);
+        wgmma_ss<0, 0>(acc1, gmma_desc_sw128(sa + 64 * 128 + 32 * k), bd, (kb | k) != 0);
+      }
+      wgmma_commit();
+      wgmma_wait<1>();                                  // the previous stage's MMAs are done: hand it back
+      if (kb > 0 && l == 0) mbar_arrive(empty_bar(s_prev));
+      s_prev = s;
+      if (++s == kStages) { s = 0; ph ^= 1; }
+    }
+    if (l == 0) mbar_arrive(order_bar(c ^ 1));          // every MMA of this tile is issued: the other consumer's turn
+    wgmma_wait<0>();
+    if (l == 0) mbar_arrive(empty_bar(s_prev));
+
+    // ---- epilogue, 32 columns at a time
+    // XM: 9 / 10 = LayerNorm folded into this GEMM (no activation / GELU); 11 = scaled residual + statistics of the output rows
+    const int mode_act = XM ? (P.ln_parts > 0 ? (P.act == ICAF_ACT_GELU ? 10 : 9) : 11) : P.act * 3 + mode;
+    const float* arow = sacc + size_t(row) * PL::kPitch;
+#pragma unroll 1
+    for (int cc = 0; cc < 4; ++cc) {
+      named_bar_sync(bar_id, 128);                      // the previous chunk (or tile) has been read out
+      if (cc == 0) sbias[t] = bias_r;
+      switch (cc) {
+        case 0: stage_chunk<0>(acc0, acc1, sacc, w, l); break;
+        case 1: stage_chunk<1>(acc0, acc1, sacc, w, l); break;
+        case 2: stage_chunk<2>(acc0, acc1, sacc, w, l); break;
+        default: stage_chunk<3>(acc0, acc1, sacc, w, l); break;
+      }
+      named_bar_sync(bar_id, 128);
+      const int cb = 32 * cc;
+      const int nb = n0 + cb;
+      if (mvalid && nb < P.N) {
+        uint32_t acc[32];
+#pragma unroll
+        for (int q = 0; q < 8; ++q) {
+          const float4 v = *reinterpret_cast<const float4*>(arow + 4 * q);
+          acc[4 * q] = __float_as_uint(v.x); acc[4 * q + 1] = __float_as_uint(v.y);
+          acc[4 * q + 2] = __float_as_uint(v.z); acc[4 * q + 3] = __float_as_uint(v.w);
+        }
+        const int ncols = min(32, P.N - nb);
+        const bool vec = ncols == 32 && ((reinterpret_cast<uintptr_t>(yrow + nb) & 15) == 0) &&
+                         (!rrow || (reinterpret_cast<uintptr_t>(rrow + nb) & 15) == 0);
+        const float* sb = sbias + cb;
+        const __half* rp = rrow ? rrow + nb : nullptr;
+        __half* yp = yrow + nb;
+        if (XM) {
+          switch (mode_act) {
+            case 9: epi_chunk<0, 0, 1>(acc, sb, rbias, alpha, beta, rp, yp, vec, ncols, ex, cb); break;
+            case 10: epi_chunk<2, 0, 1>(acc, sb, rbias, alpha, beta, rp, yp, vec, ncols, ex, cb); break;
+            default: epi_chunk<0, 2, 2>(acc, sb, rbias, alpha, beta, rp, yp, vec, ncols, ex, cb); break;
+          }
+        } else {
+          switch (mode_act) {
+            case 0: epi_chunk<0, 0>(acc, sb, rbias, alpha, beta, rp, yp, vec, ncols, ex, cb); break;
+            case 1: epi_chunk<0, 1>(acc, sb, rbias, alpha, beta, rp, yp, vec, ncols, ex, cb); break;
+            case 2: epi_chunk<0, 2>(acc, sb, rbias, alpha, beta, rp, yp, vec, ncols, ex, cb); break;
+            case 3: epi_chunk<1, 0>(acc, sb, rbias, alpha, beta, rp, yp, vec, ncols, ex, cb); break;
+            case 4: epi_chunk<1, 1>(acc, sb, rbias, alpha, beta, rp, yp, vec, ncols, ex, cb); break;
+            case 5: epi_chunk<1, 2>(acc, sb, rbias, alpha, beta, rp, yp, vec, ncols, ex, cb); break;
+            case 6: epi_chunk<2, 0>(acc, sb, rbias, alpha, beta, rp, yp, vec, ncols, ex, cb); break;
+            case 7: epi_chunk<2, 1>(acc, sb, rbias, alpha, beta, rp, yp, vec, ncols, ex, cb); break;
+            default: epi_chunk<2, 2>(acc, sb, rbias, alpha, beta, rp, yp, vec, ncols, ex, cb); break;
+          }
+        }
+      }
+    }
+    if (XM && mode_act == 11 && mvalid && n0 < P.N) epi_row_emit(ex, P, pr, m, n0, min(n0 + 128, P.N));
+  }
+}
+
+// ---------------------------------------------------------------------------------------------------
 // CUDA-core reference with the identical contract (tests only).
 struct SimtParams { ConvParams P; const __half* w[2]; };
 __global__ void conv_gemm_simt_kernel(const SimtParams S) {
@@ -377,6 +626,7 @@ static int fill_geom(const icaf_conv_geom* g, int n_io, ConvParams& P) {
   P.kh = g->kh; P.kw = g->kw; P.stride = g->stride; P.pad = g->pad; P.act = g->act; P.epi = g->epi;
   P.a_mode = A_GATHER; P.tw = P.th = P.tiles_x = P.tiles_y = 0; P.stages = 2; P.splits = 1; P.cblk = 64;
   P.ln_parts = 0; P.ln_eps = 0.f; P.ln_inv_k = 0.f;
+  P.m_tiles = P.n_tiles = P.tiles = 0;
   memset(P.p, 0, sizeof(P.p));
   return ICAF_OK;
 }
@@ -473,14 +723,29 @@ static int plan_tc(ConvParams& P, int n_io, ConvPlan& pl) {
   pl.grid_x = gx; pl.grid_y = gy; pl.grid_z = gz; pl.cluster = unsigned(splits);
   pl.smem = L::total(stages);
   pl.total = int(ctas); pl.m_tiles = mt; pl.m_pairs = 0; pl.n_tiles = int(gy);
+  pl.persist = false; pl.ctas = int(gx * gy * gz);
   return ICAF_OK;
 }
 
-template <int BN, bool XM>
-static int launch_tc_x(const ConvParams& P, const ConvPlan& pl, const __half* const (&w)[2], const icaf_conv_geom* g, int n_io, cudaStream_t st) {
-  static bool configured[kMaxDevices] = {false};
-  if (int rc = configure_smem(conv_gemm_tc_kernel<BN, XM>, 227 * 1024, configured, "conv2d: cudaFuncSetAttribute")) return rc;
-  ConvMaps maps;
+// A 128 x 128 plan with TMA-staged A, no split-K and more tiles than SMs runs on conv_gemm_persist_kernel: one CTA per SM
+// walks the tiles, so the ring fill and the epilogue of one tile overlap the main loop of the next.  The ring takes what
+// the staged chunks leave of the 227 KB (it is not clamped to the K loop: it runs on across tiles).
+static int plan_persist(ConvParams& P, ConvPlan& pl) {
+  constexpr int kSmemCap = 227 * 1024;
+  int stages = kMaxStages;
+  while (stages > 2 && PersistLayout::total(stages) > kSmemCap) --stages;
+  if (PersistLayout::total(stages) > kSmemCap)
+    return set_error(ICAF_ERR_BAD_ARG, "conv2d(persist): shared-memory plan exceeds 227 KB");
+  P.stages = stages;
+  P.m_tiles = pl.m_tiles; P.n_tiles = pl.n_tiles; P.tiles = pl.total;
+  pl.persist = true;
+  pl.ctas = pl.total < pl.sms ? pl.total : pl.sms;
+  pl.smem = PersistLayout::total(stages);
+  return ICAF_OK;
+}
+
+template <int BN>
+static int encode_maps(const ConvParams& P, const __half* const (&w)[2], const icaf_conv_geom* g, int n_io, ConvMaps& maps) {
   memset(&maps, 0, sizeof(maps));
   for (int i = 0; i < n_io; ++i) {
     int rc = encode_tmap_2d(&maps.w[i], w[i], (uint64_t)P.k_pad, (uint64_t)g->w_rows, (uint64_t)P.k_pad * 2, BK, BN);
@@ -494,12 +759,34 @@ static int launch_tc_x(const ConvParams& P, const ConvPlan& pl, const __half* co
     if (rc) return rc;
   }
   if (n_io == 1) { maps.w[1] = maps.w[0]; maps.a[1] = maps.a[0]; }
+  return ICAF_OK;
+}
+
+template <int BN, bool XM>
+static int launch_tc_x(const ConvParams& P, const ConvPlan& pl, const __half* const (&w)[2], const icaf_conv_geom* g, int n_io, cudaStream_t st) {
+  static bool configured[kMaxDevices] = {false};
+  if (int rc = configure_smem(conv_gemm_tc_kernel<BN, XM>, 227 * 1024, configured, "conv2d: cudaFuncSetAttribute")) return rc;
+  ConvMaps maps;
+  if (int rc = encode_maps<BN>(P, w, g, n_io, maps)) return rc;
   launch_kc(conv_gemm_tc_kernel<BN, XM>, dim3(pl.grid_x, pl.grid_y, pl.grid_z), dim3(kThreads), (size_t)pl.smem, st, pl.cluster, P, maps);
   return check_launch("conv2d_fwd");
 }
 template <int BN>
 static int launch_tc(const ConvParams& P, const ConvPlan& pl, const __half* const (&w)[2], const icaf_conv_geom* g, int n_io, cudaStream_t st) {
   return (P.epi & (ICAF_EPI_LN_FOLD | ICAF_EPI_EMIT_STATS)) ? launch_tc_x<BN, true>(P, pl, w, g, n_io, st) : launch_tc_x<BN, false>(P, pl, w, g, n_io, st);
+}
+
+template <bool XM>
+static int launch_persist_x(const ConvParams& P, const ConvPlan& pl, const __half* const (&w)[2], const icaf_conv_geom* g, int n_io, cudaStream_t st) {
+  static bool configured[kMaxDevices] = {false};
+  if (int rc = configure_smem(conv_gemm_persist_kernel<XM>, 227 * 1024, configured, "conv2d: cudaFuncSetAttribute")) return rc;
+  ConvMaps maps;
+  if (int rc = encode_maps<128>(P, w, g, n_io, maps)) return rc;
+  launch_k(conv_gemm_persist_kernel<XM>, dim3(unsigned(pl.ctas)), dim3(kPersistThreads), (size_t)pl.smem, st, P, maps);
+  return check_launch("conv2d_fwd");
+}
+static int launch_persist(const ConvParams& P, const ConvPlan& pl, const __half* const (&w)[2], const icaf_conv_geom* g, int n_io, cudaStream_t st) {
+  return (P.epi & (ICAF_EPI_LN_FOLD | ICAF_EPI_EMIT_STATS)) ? launch_persist_x<true>(P, pl, w, g, n_io, st) : launch_persist_x<false>(P, pl, w, g, n_io, st);
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -518,7 +805,10 @@ static int plan_conv(const icaf_conv_geom* g, int n_io, int sms, ConvParams& P, 
   if (P.N > 64 && ctas(128) >= sms) bn = 128;
   else if (P.N > 32 && ctas(64) >= sms) bn = 64;
   switch (bn) {
-    case 128: return plan_tc<128>(P, n_io, pl);
+    case 128: {
+      if (int rc = plan_tc<128>(P, n_io, pl)) return rc;
+      return (P.a_mode != A_GATHER && P.splits == 1 && pl.total > sms) ? plan_persist(P, pl) : ICAF_OK;
+    }
     case 64: return plan_tc<64>(P, n_io, pl);
     default: return plan_tc<32>(P, n_io, pl);
   }
@@ -542,7 +832,7 @@ extern "C" int icaf_conv2d_plan(const icaf_conv_geom* g, int n_io, int sm_count,
   out->tile_w = P.tw; out->tile_h = P.th; out->tiles_x = P.tiles_x; out->tiles_y = P.tiles_y;
   out->cblk = P.cblk; out->halo = 0; out->stages = P.stages; out->splits = P.splits;
   out->grid_x = int(pl.grid_x); out->grid_y = int(pl.grid_y); out->grid_z = int(pl.grid_z); out->cluster = int(pl.cluster);
-  out->smem_bytes = pl.smem; out->work_items = pl.total;
+  out->smem_bytes = pl.smem; out->work_items = pl.total; out->ctas = pl.ctas;
   return ICAF_OK;
 }
 
@@ -556,7 +846,7 @@ extern "C" int icaf_conv2d_fwd(const icaf_conv_geom* g, const icaf_conv_io* io, 
   if (rc) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   switch (pl.bn) {
-    case 128: return launch_tc<128>(P, pl, w, g, n_io, st);
+    case 128: return pl.persist ? launch_persist(P, pl, w, g, n_io, st) : launch_tc<128>(P, pl, w, g, n_io, st);
     case 64: return launch_tc<64>(P, pl, w, g, n_io, st);
     case 32: return launch_tc<32>(P, pl, w, g, n_io, st);
     default: return set_error(ICAF_ERR_BAD_ARG, "conv2d: the planner produced an unknown tile width");

@@ -62,6 +62,14 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
     }
   }
 }
+// The same bound without the report: a call (printf) reachable while wgmma groups are in flight makes ptxas serialise
+// every wgmma of the function (warning C7510), so wgmma loops wait with this one.
+__device__ __forceinline__ void mbar_wait_quiet(uint32_t bar, uint32_t parity) {
+  uint32_t spins = 0;
+  while (!mbar_try_wait(bar, parity)) {
+    if (++spins > ICAF_SPIN_LIMIT) __trap();
+  }
+}
 
 // ------------------------------------------------------------------ programmatic dependent launch (PDL)
 // launch_dependents: the next kernel in the stream may start its prologue now; wait: block until every kernel this
@@ -219,6 +227,13 @@ __device__ __forceinline__ void prefetch_l2(const void* p) { asm volatile("prefe
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
+
+// ------------------------------------------------------------------ per-warpgroup register budget (warp specialisation)
+// Every thread of the warpgroup executes it; the new limit (multiple of 8, 24..256) holds from here on.
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
 
 // ------------------------------------------------------------------ thread-block clusters / distributed shared memory
 __device__ __forceinline__ uint32_t cluster_ctarank() {

@@ -98,7 +98,8 @@ int icaf_conv2d_fwd(const icaf_conv_geom* g, const icaf_conv_io* io, int n_io, v
  * plan this returns for (geometry, n_io, SM count of the current device); the same invariant checks run in both, so a
  * GPU-less test can walk every layer of a model through the dispatcher (tests/test_abi_cpu.py).
  * pair_mode: accepted for ABI stability and ignored (sm_90a has no CTA-pair MMA). */
-#define ICAF_KERNEL_TC 0      /* one 128 x BN tile per CTA, split-K clusters   (conv_gemm.cu)    */
+#define ICAF_KERNEL_TC 0      /* wgmma implicit GEMM, 128 x BN tiles (conv_gemm.cu): one tile per CTA with split-K
+                                 clusters, or, for BN = 128 grids of more than one wave, `ctas` persistent CTAs       */
 typedef struct {
   int kernel;                            /* ICAF_KERNEL_*                                                     */
   int bn;                                /* output-channel tile width (32/64/128)                             */
@@ -107,9 +108,11 @@ typedef struct {
   int cblk;                              /* channels per TMA box                                              */
   int halo;                              /* always 0 (halo copies belong to CTA-pair kernels)                 */
   int stages, splits;                    /* smem ring depth; split-K factor (= cluster size of the tc kernel) */
-  int grid_x, grid_y, grid_z, cluster;   /* launch shape                                                      */
+  int grid_x, grid_y, grid_z, cluster;   /* tile grid (m tiles x splits, n tiles, problems); cluster size     */
   int smem_bytes;                        /* dynamic shared memory per CTA                                     */
   int work_items;                        /* output tiles the grid covers                                      */
+  int ctas;                              /* CTAs the launch starts: the tile grid's product, or at most the
+                                            SM count when persistent CTAs walk the tiles                      */
 } icaf_conv_plan;
 int icaf_conv2d_plan(const icaf_conv_geom* g, int n_io, int sm_count, int pair_mode, icaf_conv_plan* out);
 
