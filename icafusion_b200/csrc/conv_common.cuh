@@ -1,4 +1,5 @@
-// Shared pieces of the implicit-GEMM conv kernel (conv_gemm.cu): problem descriptors, TMA descriptor bundle, epilogue chunk.
+// Shared pieces of the implicit-GEMM conv kernels (conv_gemm.cu): problem descriptors, TMA descriptor bundle, tile origin,
+// and the epilogue (staged-row load, chunk dispatch).
 #pragma once
 #include "icaf_internal.cuh"
 
@@ -47,6 +48,22 @@ __device__ __forceinline__ ConvProblem pick_problem(const ConvParams& P, unsigne
   r.ln_stats = z ? P.p[1].ln_stats : P.p[0].ln_stats; r.ln_s = z ? P.p[1].ln_s : P.p[0].ln_s;
   r.stats_out = z ? P.p[1].stats_out : P.p[0].stats_out;
   return r;
+}
+
+// Origin of an output tile: linear rows from m0 (gather / 2-D), or a th x tw patch at (oy0, ox0) of image tb (4-D).
+struct TileOrigin { int m0, tb, oy0, ox0; };
+// The origin of m-tile `mtile`, into four scalars rather than a TileOrigin: the one-tile kernel keeps them apart, and
+// ptxas allocates its registers differently when they start out as one struct.
+__device__ __forceinline__ void tile_origin(const ConvParams& P, int mtile, int& m0, int& tb, int& oy0, int& ox0) {
+  m0 = mtile * BM; tb = 0; oy0 = 0; ox0 = 0;
+  if (P.a_mode == A_TMA4D) {
+    const int per_img = P.tiles_x * P.tiles_y;
+    m0 = 0;
+    tb = mtile / per_img;
+    const int t = mtile - tb * per_img;
+    oy0 = (t / P.tiles_x) * P.th;
+    ox0 = (t % P.tiles_x) * P.tw;
+  }
 }
 
 // Per-row extras of an epilogue thread.  XM = 1 (LayerNorm folded into this GEMM, common.py:660,665,749-750): the filter
@@ -142,6 +159,43 @@ __device__ __forceinline__ void epi_chunk(const uint32_t (&acc)[32], const float
   }
 }
 
+// 32 staged fp32 accumulators of one row (16-byte aligned) as the bit patterns epi_chunk takes
+__device__ __forceinline__ void load_staged(uint32_t (&acc)[32], const float* p) {
+#pragma unroll
+  for (int q = 0; q < 8; ++q) {
+    const float4 v = *reinterpret_cast<const float4*>(p + 4 * q);
+    acc[4 * q] = __float_as_uint(v.x); acc[4 * q + 1] = __float_as_uint(v.y);
+    acc[4 * q + 2] = __float_as_uint(v.z); acc[4 * q + 3] = __float_as_uint(v.w);
+  }
+}
+
+// One chunk through the epi_chunk specialisation of the row's mode.  The activation / residual mode is warp-uniform, so
+// it is dispatched once per chunk to straight-line code.  mode_act = 3 * ACT + RES; XM: 9 / 10 = LayerNorm folded into
+// this GEMM (no activation / GELU), 11 = scaled residual + statistics of the output rows.
+template <bool XM>
+__device__ __forceinline__ void epi_dispatch(int mode_act, const uint32_t (&acc)[32], const float* sb, float rbias, float alpha,
+                                             float beta, const __half* rp, __half* yp, bool vec, int ncols, EpiRow& ex, int cb) {
+  if (XM) {
+    switch (mode_act) {
+      case 9: epi_chunk<0, 0, 1>(acc, sb, rbias, alpha, beta, rp, yp, vec, ncols, ex, cb); break;
+      case 10: epi_chunk<2, 0, 1>(acc, sb, rbias, alpha, beta, rp, yp, vec, ncols, ex, cb); break;
+      default: epi_chunk<0, 2, 2>(acc, sb, rbias, alpha, beta, rp, yp, vec, ncols, ex, cb); break;
+    }
+  } else {
+    switch (mode_act) {
+      case 0: epi_chunk<0, 0>(acc, sb, rbias, alpha, beta, rp, yp, vec, ncols, ex, cb); break;
+      case 1: epi_chunk<0, 1>(acc, sb, rbias, alpha, beta, rp, yp, vec, ncols, ex, cb); break;
+      case 2: epi_chunk<0, 2>(acc, sb, rbias, alpha, beta, rp, yp, vec, ncols, ex, cb); break;
+      case 3: epi_chunk<1, 0>(acc, sb, rbias, alpha, beta, rp, yp, vec, ncols, ex, cb); break;
+      case 4: epi_chunk<1, 1>(acc, sb, rbias, alpha, beta, rp, yp, vec, ncols, ex, cb); break;
+      case 5: epi_chunk<1, 2>(acc, sb, rbias, alpha, beta, rp, yp, vec, ncols, ex, cb); break;
+      case 6: epi_chunk<2, 0>(acc, sb, rbias, alpha, beta, rp, yp, vec, ncols, ex, cb); break;
+      case 7: epi_chunk<2, 1>(acc, sb, rbias, alpha, beta, rp, yp, vec, ncols, ex, cb); break;
+      default: epi_chunk<2, 2>(acc, sb, rbias, alpha, beta, rp, yp, vec, ncols, ex, cb); break;
+    }
+  }
+}
+
 // Host-side launch plan: everything the dispatcher decides before it touches CUDA.  icaf_conv2d_plan (host only, no
 // device needed) exposes it so that a CPU test can walk every layer geometry through the dispatcher's invariants.
 struct ConvPlan {
@@ -149,7 +203,7 @@ struct ConvPlan {
   int bn;                         // output-channel tile width
   unsigned grid_x, grid_y, grid_z, cluster;
   int smem;                       // dynamic shared memory per CTA (bytes)
-  int total, m_tiles, m_pairs, n_tiles;
+  int tiles, m_tiles, n_tiles;    // output tiles of the launch (icaf_conv_plan.work_items) = m_tiles * n_tiles * problems
   int sms;                        // SM count the plan was made for
   bool persist;                   // conv_gemm_persist_kernel: `ctas` CTAs walk the grid_x * grid_y * grid_z tiles
   int ctas;                       // CTAs the launch starts

@@ -21,6 +21,8 @@
 // CTAs of a cluster take a K range each; the leader adds the others' staged tiles through distributed shared memory.
 // conv_gemm_persist_kernel: BN = 128 grids of more than one wave with TMA-staged A -- one persistent CTA per SM, a TMA
 // producer warpgroup and two consumer warpgroups that take turns on the main loop (see its own comment below).
+// The two kernels share the TMA producer stage (load_stage), the main loop (mma_loop), the tile origin and the staged-row
+// load and epi_chunk dispatch of the epilogue, so they compute bit-identical tiles.
 #include <cstdlib>
 #include <cstring>
 
@@ -41,6 +43,56 @@ struct SmemLayout {
   __host__ __device__ static int region(int stages) { return stages * kStageBytes > kAccBytes ? stages * kStageBytes : kAccBytes; }
   static int total(int stages) { return region(stages) + kTailBytes; }
 };
+
+// ---------------------------------------------------------------------------------------------------
+// Producer and main-loop pieces of both wgmma kernels (the epilogue pieces are in conv_common.cuh).
+
+// TMA producer, one K block `kb` of the tile into the ring stage at `sa`: the filter box (BN rows from n0) and, unless the
+// gather producers fill A, the A box -- 2-D rows from m0, or the 4-D box of the tile's patch shifted by the block's filter
+// tap.  kTmaA: the launch never gathers A, so an A that is not 2-D is 4-D.
+template <int BN, bool kTmaA>
+__device__ __forceinline__ void load_stage(const ConvParams& P, int a_mode, uint32_t sa, uint32_t bar, uint32_t bytes,
+                                           const CUtensorMap* mw, const CUtensorMap* ma, int kb, int n0, const TileOrigin& o) {
+  mbar_arrive_expect_tx(bar, bytes);
+  tma_load_2d(sa + SmemLayout<BN>::kABytes, mw, bar, kb * BK, n0);
+  if (a_mode == A_TMA2D) {
+    tma_load_2d(sa, ma, bar, kb * BK, o.m0);
+  } else if (kTmaA || a_mode == A_TMA4D) {
+    const int k0 = kb * BK;
+    const int tap = k0 / P.Cin;
+    const int ch = k0 - tap * P.Cin;
+    const int ky = tap / P.kw, kx = tap - ky * P.kw;
+    tma_load_4d(sa, ma, bar, ch, o.ox0 * P.stride - P.pad + kx, o.oy0 * P.stride - P.pad + ky, o.tb);
+  }
+}
+
+// Consumer warpgroup main loop over the tile's nkb K blocks, from ring stage s0 at phase ph0: per stage, wait for it to
+// fill, issue two m64nBNk16 wgmma per 16 K (tile rows 0-63 into acc0, 64-127 into acc1), then hand back the previous
+// stage, whose MMAs are done once this stage's are the only ones in flight.  Returns the last stage, which is still in
+// use until the caller's final wgmma_wait.  kQuiet: wait without the printf report (see mbar_wait_quiet).
+template <int BN, bool kQuiet, class FullBar, class HandBack>
+__device__ __forceinline__ int mma_loop(float (&acc0)[BN / 2], float (&acc1)[BN / 2], uint32_t smem_base, int kStages, int nkb,
+                                        int s0, uint32_t ph0, FullBar full_bar, HandBack hand_back) {
+  int s = s0, s_prev = s0;
+  uint32_t ph = ph0;
+  for (int kb = 0; kb < nkb; ++kb) {
+    if (kQuiet) mbar_wait_quiet(full_bar(s), ph); else mbar_wait(full_bar(s), ph);
+    const uint32_t sa = smem_base + s * SmemLayout<BN>::kStageBytes;
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < BK / 16; ++k) {
+      const uint64_t bd = gmma_desc_sw128(sa + SmemLayout<BN>::kABytes + 32 * k);
+      wgmma_ss<0, 0>(acc0, gmma_desc_sw128(sa + 32 * k), bd, (kb | k) != 0);
+      wgmma_ss<0, 0>(acc1, gmma_desc_sw128(sa + 64 * 128 + 32 * k), bd, (kb | k) != 0);
+    }
+    wgmma_commit();
+    wgmma_wait<1>();
+    if (kb > 0) hand_back(s_prev);
+    s_prev = s;
+    if (++s == kStages) { s = 0; ph ^= 1; }
+  }
+  return s_prev;
+}
 
 // XM: the LayerNorm-fold / row-statistics epilogues (DMFF linears) live in their own instantiation so that the epilogue
 // of every other layer stays small (the hot loops are instruction-cache sensitive).
@@ -71,16 +123,9 @@ conv_gemm_tc_kernel(const ConvParams P, const __grid_constant__ ConvMaps maps) {
   const int nkb_all = P.k_pad / BK;
   const int kb_begin = (nkb_all * int(crank)) / splits;
   const int nkb = (nkb_all * (int(crank) + 1)) / splits - kb_begin;
-  // tile origin: linear rows (gather / 2-D) or a th x tw patch of image tb (4-D)
-  int m0 = mtile * BM, tb = 0, oy0 = 0, ox0 = 0;
-  if (a_mode == A_TMA4D) {
-    const int per_img = P.tiles_x * P.tiles_y;
-    m0 = 0;
-    tb = mtile / per_img;
-    const int t = mtile - tb * per_img;
-    oy0 = (t / P.tiles_x) * P.th;
-    ox0 = (t % P.tiles_x) * P.tw;
-  }
+  int m0, tb, oy0, ox0;
+  tile_origin(P, mtile, m0, tb, oy0, ox0);
+  const TileOrigin o{m0, tb, oy0, ox0};
 
   if (tid == 0) {
     const uint32_t nfull = a_mode == A_GATHER ? 129u : 1u;    // 128 gather threads + the TMA thread
@@ -123,7 +168,7 @@ conv_gemm_tc_kernel(const ConvParams P, const __grid_constant__ ConvMaps maps) {
       int iy0[8], ix0[8];
 #pragma unroll
       for (int i = 0; i < 8; ++i) {
-        int m = m0 + r0 + 16 * i;
+        int m = o.m0 + r0 + 16 * i;
         bool mv = m < P.M;
         int mm = mv ? m : 0;
         int ox = mm % P.Wo;
@@ -207,12 +252,7 @@ conv_gemm_tc_kernel(const ConvParams P, const __grid_constant__ ConvMaps maps) {
 #pragma unroll 1
       for (int cb = 0; cb < BN; cb += 32) {
         uint32_t acc[32];
-#pragma unroll
-        for (int q = 0; q < 8; ++q) {
-          const float4 v = *reinterpret_cast<const float4*>(arow + cb + 4 * q);
-          acc[4 * q] = __float_as_uint(v.x); acc[4 * q + 1] = __float_as_uint(v.y);
-          acc[4 * q + 2] = __float_as_uint(v.z); acc[4 * q + 3] = __float_as_uint(v.w);
-        }
+        load_staged(acc, arow + cb);
         // ---- split-K reduction: the other CTAs' staged partial tiles, read through distributed shared memory ----
         for (int r = 1; r < splits; ++r) {
           const uint32_t peer = map_to_cta(arow_s, uint32_t(r)) + uint32_t(cb) * 4u;
@@ -234,26 +274,7 @@ conv_gemm_tc_kernel(const ConvParams P, const __grid_constant__ ConvMaps maps) {
           const float* sb = sbias + cb;
           const __half* rp = rrow ? rrow + nb : nullptr;
           __half* yp = yrow + nb;
-          // act / residual mode are warp-uniform: dispatch once per chunk to straight-line specialisations
-          if (XM) {
-            switch (mode_act) {
-              case 9: epi_chunk<0, 0, 1>(acc, sb, rbias, alpha, beta, rp, yp, vec, ncols, ex, cb); break;
-              case 10: epi_chunk<2, 0, 1>(acc, sb, rbias, alpha, beta, rp, yp, vec, ncols, ex, cb); break;
-              default: epi_chunk<0, 2, 2>(acc, sb, rbias, alpha, beta, rp, yp, vec, ncols, ex, cb); break;
-            }
-          } else {
-            switch (mode_act) {
-              case 0: epi_chunk<0, 0>(acc, sb, rbias, alpha, beta, rp, yp, vec, ncols, ex, cb); break;
-              case 1: epi_chunk<0, 1>(acc, sb, rbias, alpha, beta, rp, yp, vec, ncols, ex, cb); break;
-              case 2: epi_chunk<0, 2>(acc, sb, rbias, alpha, beta, rp, yp, vec, ncols, ex, cb); break;
-              case 3: epi_chunk<1, 0>(acc, sb, rbias, alpha, beta, rp, yp, vec, ncols, ex, cb); break;
-              case 4: epi_chunk<1, 1>(acc, sb, rbias, alpha, beta, rp, yp, vec, ncols, ex, cb); break;
-              case 5: epi_chunk<1, 2>(acc, sb, rbias, alpha, beta, rp, yp, vec, ncols, ex, cb); break;
-              case 6: epi_chunk<2, 0>(acc, sb, rbias, alpha, beta, rp, yp, vec, ncols, ex, cb); break;
-              case 7: epi_chunk<2, 1>(acc, sb, rbias, alpha, beta, rp, yp, vec, ncols, ex, cb); break;
-              default: epi_chunk<2, 2>(acc, sb, rbias, alpha, beta, rp, yp, vec, ncols, ex, cb); break;
-            }
-          }
+          epi_dispatch<XM>(mode_act, acc, sb, rbias, alpha, beta, rp, yp, vec, ncols, ex, cb);
         }
       }
       if (XM && mode_act == 11 && mvalid && n0 < P.N) epi_row_emit(ex, P, pr, m, n0, min(n0 + BN, P.N));
@@ -264,24 +285,8 @@ conv_gemm_tc_kernel(const ConvParams P, const __grid_constant__ ConvMaps maps) {
     float acc0[BN / 2], acc1[BN / 2];
 #pragma unroll
     for (int i = 0; i < BN / 2; ++i) { acc0[i] = 0.f; acc1[i] = 0.f; }
-    int s = 0, s_prev = 0;
-    uint32_t ph = 0;
-    for (int kb = 0; kb < nkb; ++kb) {
-      mbar_wait(full_bar(s), ph);
-      const uint32_t sa = smem_base + s * L::kStageBytes;
-      wgmma_fence();
-#pragma unroll
-      for (int k = 0; k < BK / 16; ++k) {
-        const uint64_t bd = gmma_desc_sw128(sa + L::kABytes + 32 * k);
-        wgmma_ss<0, 0>(acc0, gmma_desc_sw128(sa + 32 * k), bd, (kb | k) != 0);
-        wgmma_ss<0, 0>(acc1, gmma_desc_sw128(sa + 64 * 128 + 32 * k), bd, (kb | k) != 0);
-      }
-      wgmma_commit();
-      wgmma_wait<1>();                                  // the previous stage's MMAs are done: hand it back
-      if (kb > 0 && lane_id() == 0) mbar_arrive(empty_bar(s_prev));
-      s_prev = s;
-      if (++s == kStages) { s = 0; ph ^= 1; }
-    }
+    mma_loop<BN, false>(acc0, acc1, smem_base, kStages, nkb, 0, 0u, full_bar,
+                        [&](int s) { if (lane_id() == 0) mbar_arrive(empty_bar(s)); });   // one arrival per consumer warp
     wgmma_wait<0>();
     // the ring is idle now (every stage consumed): stage the accumulator tile as rows for the epilogue warps
     const int t = tid - 128, w = t >> 5, l = t & 31;
@@ -303,18 +308,7 @@ conv_gemm_tc_kernel(const ConvParams P, const __grid_constant__ ConvMaps maps) {
       uint32_t ph = 0;
       for (int kb = 0; kb < nkb; ++kb) {
         mbar_wait(empty_bar(s), ph ^ 1);
-        const uint32_t sa = smem_base + s * L::kStageBytes;
-        mbar_arrive_expect_tx(full_bar(s), bytes);
-        tma_load_2d(sa + L::kABytes, mw, full_bar(s), (kb_begin + kb) * BK, n0);
-        if (a_mode == A_TMA2D) {
-          tma_load_2d(sa, ma, full_bar(s), (kb_begin + kb) * BK, m0);
-        } else if (a_mode == A_TMA4D) {
-          const int k0 = (kb_begin + kb) * BK;
-          const int tap = k0 / P.Cin;
-          const int ch = k0 - tap * P.Cin;
-          const int ky = tap / P.kw, kx = tap - ky * P.kw;
-          tma_load_4d(sa, ma, full_bar(s), ch, ox0 * P.stride - P.pad + kx, oy0 * P.stride - P.pad + ky, tb);
-        }
+        load_stage<BN, false>(P, a_mode, smem_base + s * L::kStageBytes, full_bar(s), bytes, mw, ma, kb_begin + kb, n0, o);
         if (++s == kStages) { s = 0; ph ^= 1; }
       }
     }
@@ -332,7 +326,6 @@ conv_gemm_tc_kernel(const ConvParams P, const __grid_constant__ ConvMaps maps) {
 //                    from one consumer to the other, so one warpgroup's epilogue runs while the other's MMAs run.  The
 //                    epilogue stages the accumulators through the warpgroup's own smem buffer 32 columns at a time
 //                    (thread t owns tile row t).
-// The main loop (MMA sequence, K order) and the epilogue arithmetic are those of conv_gemm_tc_kernel<128, XM>.
 constexpr int kPersistThreads = 384;
 struct PersistLayout {
   static constexpr int kStageBytes = SmemLayout<128>::kStageBytes;
@@ -343,23 +336,16 @@ struct PersistLayout {
   static int total(int stages) { return bar_off(stages) + 256 + 2 * 128 * 4 + 1024; }
 };
 
-struct TileOrigin { int z, n0, m0, tb, oy0, ox0; };
-__device__ __forceinline__ TileOrigin tile_origin(const ConvParams& P, int t) {
-  TileOrigin o;
+// tile t of the launch: n-tile fastest, then m-tile, then problem z
+struct PersistTile { int z, n0; TileOrigin o; };
+__device__ __forceinline__ PersistTile persist_tile(const ConvParams& P, int t) {
+  PersistTile pt;
   const int r = t / P.n_tiles;
   const int mtile = r % P.m_tiles;
-  o.n0 = (t - r * P.n_tiles) * 128;
-  o.z = r / P.m_tiles;
-  o.m0 = mtile * BM; o.tb = 0; o.oy0 = 0; o.ox0 = 0;
-  if (P.a_mode == A_TMA4D) {
-    const int per_img = P.tiles_x * P.tiles_y;
-    o.m0 = 0;
-    o.tb = mtile / per_img;
-    const int u = mtile - o.tb * per_img;
-    o.oy0 = (u / P.tiles_x) * P.th;
-    o.ox0 = (u % P.tiles_x) * P.tw;
-  }
-  return o;
+  pt.n0 = (t - r * P.n_tiles) * 128;
+  pt.z = r / P.m_tiles;
+  tile_origin(P, mtile, pt.o.m0, pt.o.tb, pt.o.oy0, pt.o.ox0);
+  return pt;
 }
 
 // columns [32 CC, 32 CC + 32) of the warpgroup's accumulators -> staged rows (accumulator layout: see ptx.cuh)
@@ -419,23 +405,12 @@ conv_gemm_persist_kernel(const ConvParams P, const __grid_constant__ ConvMaps ma
       int s = 0;
       uint32_t ph = 0;
       for (int tile = blockIdx.x; tile < P.tiles; tile += gridDim.x) {
-        const TileOrigin o = tile_origin(P, tile);
-        const CUtensorMap* mw = o.z ? &maps.w[1] : &maps.w[0];
-        const CUtensorMap* ma = o.z ? &maps.a[1] : &maps.a[0];
+        const PersistTile pt = persist_tile(P, tile);
+        const CUtensorMap* mw = pt.z ? &maps.w[1] : &maps.w[0];
+        const CUtensorMap* ma = pt.z ? &maps.a[1] : &maps.a[0];
         for (int kb = 0; kb < nkb; ++kb) {
           mbar_wait_quiet(empty_bar(s), ph ^ 1);
-          const uint32_t sa = smem_base + s * L::kStageBytes;
-          mbar_arrive_expect_tx(full_bar(s), bytes);
-          tma_load_2d(sa + L::kABytes, mw, full_bar(s), kb * BK, o.n0);
-          if (a_mode == A_TMA2D) {
-            tma_load_2d(sa, ma, full_bar(s), kb * BK, o.m0);
-          } else {
-            const int k0 = kb * BK;
-            const int tap = k0 / P.Cin;
-            const int ch = k0 - tap * P.Cin;
-            const int ky = tap / P.kw, kx = tap - ky * P.kw;
-            tma_load_4d(sa, ma, full_bar(s), ch, o.ox0 * P.stride - P.pad + kx, o.oy0 * P.stride - P.pad + ky, o.tb);
-          }
+          load_stage<128, true>(P, a_mode, smem_base + s * L::kStageBytes, full_bar(s), bytes, mw, ma, kb, pt.n0, pt.o);
           if (++s == kStages) { s = 0; ph ^= 1; }
         }
       }
@@ -452,9 +427,10 @@ conv_gemm_persist_kernel(const ConvParams P, const __grid_constant__ ConvMaps ma
   float* sbias = reinterpret_cast<float*>(smem_gen + bar_off + 256 + c * 128 * 4);
   for (int tile = blockIdx.x + c * gridDim.x; tile < P.tiles; tile += 2 * gridDim.x) {
     const int j = (tile - int(blockIdx.x)) / int(gridDim.x);  // ordinal of the tile among this CTA's tiles
-    const TileOrigin o = tile_origin(P, tile);
-    const ConvProblem pr = pick_problem(P, o.z);
-    const int n0 = o.n0;
+    const PersistTile pt = persist_tile(P, tile);
+    const ConvProblem pr = pick_problem(P, pt.z);
+    const int n0 = pt.n0;
+    const TileOrigin& o = pt.o;
     // Epilogue operands that do not depend on the main loop are fetched now so their DRAM latency hides behind it:
     // bias slice and (alpha, beta) into registers, this thread's residual row into L2.
     const float bias_r = (pr.bias && !(P.epi & ICAF_EPI_BIAS_ROW) && n0 + t < P.N) ? __ldg(pr.bias + n0 + t) : 0.f;
@@ -490,29 +466,15 @@ conv_gemm_persist_kernel(const ConvParams P, const __grid_constant__ ConvMaps ma
     float acc0[64], acc1[64];
 #pragma unroll
     for (int i = 0; i < 64; ++i) { acc0[i] = 0.f; acc1[i] = 0.f; }
+    auto hand_back = [&](int s) { if (l == 0) mbar_arrive(empty_bar(s)); };   // one arrival per consumer warp
     const int g0 = j * nkb;
-    int s = g0 % kStages, s_prev = s;
-    uint32_t ph = uint32_t(g0 / kStages) & 1u;
+    const int s0 = g0 % kStages;
+    const uint32_t ph0 = uint32_t(g0 / kStages) & 1u;
     if (j > 0) mbar_wait_quiet(order_bar(c), uint32_t((j >> 1) - (1 - c)) & 1u);
-    for (int kb = 0; kb < nkb; ++kb) {
-      mbar_wait_quiet(full_bar(s), ph);
-      const uint32_t sa = smem_base + s * L::kStageBytes;
-      wgmma_fence();
-#pragma unroll
-      for (int k = 0; k < BK / 16; ++k) {
-        const uint64_t bd = gmma_desc_sw128(sa + L::kABytes + 32 * k);
-        wgmma_ss<0, 0>(acc0, gmma_desc_sw128(sa + 32 * k), bd, (kb | k) != 0);
-        wgmma_ss<0, 0>(acc1, gmma_desc_sw128(sa + 64 * 128 + 32 * k), bd, (kb | k) != 0);
-      }
-      wgmma_commit();
-      wgmma_wait<1>();                                  // the previous stage's MMAs are done: hand it back
-      if (kb > 0 && l == 0) mbar_arrive(empty_bar(s_prev));
-      s_prev = s;
-      if (++s == kStages) { s = 0; ph ^= 1; }
-    }
+    const int s_last = mma_loop<128, true>(acc0, acc1, smem_base, kStages, nkb, s0, ph0, full_bar, hand_back);
     if (l == 0) mbar_arrive(order_bar(c ^ 1));          // every MMA of this tile is issued: the other consumer's turn
     wgmma_wait<0>();
-    if (l == 0) mbar_arrive(empty_bar(s_prev));
+    hand_back(s_last);
 
     // ---- epilogue, 32 columns at a time
     // XM: 9 / 10 = LayerNorm folded into this GEMM (no activation / GELU); 11 = scaled residual + statistics of the output rows
@@ -533,37 +495,14 @@ conv_gemm_persist_kernel(const ConvParams P, const __grid_constant__ ConvMaps ma
       const int nb = n0 + cb;
       if (mvalid && nb < P.N) {
         uint32_t acc[32];
-#pragma unroll
-        for (int q = 0; q < 8; ++q) {
-          const float4 v = *reinterpret_cast<const float4*>(arow + 4 * q);
-          acc[4 * q] = __float_as_uint(v.x); acc[4 * q + 1] = __float_as_uint(v.y);
-          acc[4 * q + 2] = __float_as_uint(v.z); acc[4 * q + 3] = __float_as_uint(v.w);
-        }
+        load_staged(acc, arow);
         const int ncols = min(32, P.N - nb);
         const bool vec = ncols == 32 && ((reinterpret_cast<uintptr_t>(yrow + nb) & 15) == 0) &&
                          (!rrow || (reinterpret_cast<uintptr_t>(rrow + nb) & 15) == 0);
         const float* sb = sbias + cb;
         const __half* rp = rrow ? rrow + nb : nullptr;
         __half* yp = yrow + nb;
-        if (XM) {
-          switch (mode_act) {
-            case 9: epi_chunk<0, 0, 1>(acc, sb, rbias, alpha, beta, rp, yp, vec, ncols, ex, cb); break;
-            case 10: epi_chunk<2, 0, 1>(acc, sb, rbias, alpha, beta, rp, yp, vec, ncols, ex, cb); break;
-            default: epi_chunk<0, 2, 2>(acc, sb, rbias, alpha, beta, rp, yp, vec, ncols, ex, cb); break;
-          }
-        } else {
-          switch (mode_act) {
-            case 0: epi_chunk<0, 0>(acc, sb, rbias, alpha, beta, rp, yp, vec, ncols, ex, cb); break;
-            case 1: epi_chunk<0, 1>(acc, sb, rbias, alpha, beta, rp, yp, vec, ncols, ex, cb); break;
-            case 2: epi_chunk<0, 2>(acc, sb, rbias, alpha, beta, rp, yp, vec, ncols, ex, cb); break;
-            case 3: epi_chunk<1, 0>(acc, sb, rbias, alpha, beta, rp, yp, vec, ncols, ex, cb); break;
-            case 4: epi_chunk<1, 1>(acc, sb, rbias, alpha, beta, rp, yp, vec, ncols, ex, cb); break;
-            case 5: epi_chunk<1, 2>(acc, sb, rbias, alpha, beta, rp, yp, vec, ncols, ex, cb); break;
-            case 6: epi_chunk<2, 0>(acc, sb, rbias, alpha, beta, rp, yp, vec, ncols, ex, cb); break;
-            case 7: epi_chunk<2, 1>(acc, sb, rbias, alpha, beta, rp, yp, vec, ncols, ex, cb); break;
-            default: epi_chunk<2, 2>(acc, sb, rbias, alpha, beta, rp, yp, vec, ncols, ex, cb); break;
-          }
-        }
+        epi_dispatch<XM>(mode_act, acc, sb, rbias, alpha, beta, rp, yp, vec, ncols, ex, cb);
       }
     }
     if (XM && mode_act == 11 && mvalid && n0 < P.N) epi_row_emit(ex, P, pr, m, n0, min(n0 + 128, P.N));
@@ -695,8 +634,8 @@ static int plan_tc(ConvParams& P, int n_io, ConvPlan& pl) {
   // Ring depth: a grid that fits in one wave gets the whole SM (deep ring: the K loop is latency-bound at small M);
   // otherwise two CTAs of the narrow tiles share an SM so that one CTA's epilogue overlaps the other's main loop (BN = 128
   // keeps one CTA per SM: its 128 accumulator registers per consumer thread leave no room for a second one).
-  const long long ctas = (long long)gx * gy * gz;
-  const int budget = (ctas <= pl.sms || BN > 64) ? kSmemCap : (kSmemCap / 2 - 1024);
+  const long long tiles = (long long)gx * gy * gz;
+  const int budget = (tiles <= pl.sms || BN > 64) ? kSmemCap : (kSmemCap / 2 - 1024);
   int stages = (budget - L::kTailBytes) / L::kStageBytes;
   const int nkb = P.k_pad / BK;
   if (stages > nkb) stages = nkb;
@@ -704,8 +643,8 @@ static int plan_tc(ConvParams& P, int n_io, ConvPlan& pl) {
   if (stages < 2) stages = 2;
   // Split-K: a grid that leaves most SMs idle on a deep K loop is spread over clusters of `splits` CTAs per tile.
   int splits = 1;
-  if (ctas * 2 <= pl.sms && nkb >= 8) {
-    splits = int(pl.sms / ctas);
+  if (tiles * 2 <= pl.sms && nkb >= 8) {
+    splits = int(pl.sms / tiles);
     if (splits > 8) splits = 8;                    // portable cluster size
     if (splits > nkb / 4) splits = nkb / 4;        // >= 4 K blocks per CTA
     if (splits < 1) splits = 1;
@@ -722,7 +661,7 @@ static int plan_tc(ConvParams& P, int n_io, ConvPlan& pl) {
   pl.kernel = ICAF_KERNEL_TC; pl.bn = BN;
   pl.grid_x = gx; pl.grid_y = gy; pl.grid_z = gz; pl.cluster = unsigned(splits);
   pl.smem = L::total(stages);
-  pl.total = int(ctas); pl.m_tiles = mt; pl.m_pairs = 0; pl.n_tiles = int(gy);
+  pl.tiles = int(tiles); pl.m_tiles = mt; pl.n_tiles = int(gy);
   pl.persist = false; pl.ctas = int(gx * gy * gz);
   return ICAF_OK;
 }
@@ -737,9 +676,9 @@ static int plan_persist(ConvParams& P, ConvPlan& pl) {
   if (PersistLayout::total(stages) > kSmemCap)
     return set_error(ICAF_ERR_BAD_ARG, "conv2d(persist): shared-memory plan exceeds 227 KB");
   P.stages = stages;
-  P.m_tiles = pl.m_tiles; P.n_tiles = pl.n_tiles; P.tiles = pl.total;
+  P.m_tiles = pl.m_tiles; P.n_tiles = pl.n_tiles; P.tiles = pl.tiles;
   pl.persist = true;
-  pl.ctas = pl.total < pl.sms ? pl.total : pl.sms;
+  pl.ctas = pl.tiles < pl.sms ? pl.tiles : pl.sms;
   pl.smem = PersistLayout::total(stages);
   return ICAF_OK;
 }
@@ -762,31 +701,22 @@ static int encode_maps(const ConvParams& P, const __half* const (&w)[2], const i
   return ICAF_OK;
 }
 
-template <int BN, bool XM>
-static int launch_tc_x(const ConvParams& P, const ConvPlan& pl, const __half* const (&w)[2], const icaf_conv_geom* g, int n_io, cudaStream_t st) {
-  static bool configured[kMaxDevices] = {false};
-  if (int rc = configure_smem(conv_gemm_tc_kernel<BN, XM>, 227 * 1024, configured, "conv2d: cudaFuncSetAttribute")) return rc;
+// Launch a planned conv on the kernel the plan picked (XM: the LayerNorm-fold / row-statistics instantiation).  Its
+// shared-memory limit is raised once per device; the filter maps are encoded for the plan's tile width.
+template <int BN>
+static int launch_conv(const ConvParams& P, const ConvPlan& pl, const __half* const (&w)[2], const icaf_conv_geom* g, int n_io,
+                       cudaStream_t st) {
+  const int xm = (P.epi & (ICAF_EPI_LN_FOLD | ICAF_EPI_EMIT_STATS)) ? 1 : 0;
+  void (*kernel)(ConvParams, ConvMaps) = xm ? conv_gemm_tc_kernel<BN, true> : conv_gemm_tc_kernel<BN, false>;
+  if (pl.persist) kernel = xm ? conv_gemm_persist_kernel<true> : conv_gemm_persist_kernel<false>;
+  static bool configured[2][2][kMaxDevices] = {};
+  if (int rc = configure_smem(kernel, 227 * 1024, configured[pl.persist][xm], "conv2d: cudaFuncSetAttribute")) return rc;
   ConvMaps maps;
   if (int rc = encode_maps<BN>(P, w, g, n_io, maps)) return rc;
-  launch_kc(conv_gemm_tc_kernel<BN, XM>, dim3(pl.grid_x, pl.grid_y, pl.grid_z), dim3(kThreads), (size_t)pl.smem, st, pl.cluster, P, maps);
+  // the one-tile kernel takes the tile grid (split-K: in clusters along x); the persistent one `ctas` CTAs
+  const dim3 grid = pl.persist ? dim3(unsigned(pl.ctas)) : dim3(pl.grid_x, pl.grid_y, pl.grid_z);
+  launch_kc(kernel, grid, dim3(pl.persist ? kPersistThreads : kThreads), (size_t)pl.smem, st, pl.cluster, P, maps);
   return check_launch("conv2d_fwd");
-}
-template <int BN>
-static int launch_tc(const ConvParams& P, const ConvPlan& pl, const __half* const (&w)[2], const icaf_conv_geom* g, int n_io, cudaStream_t st) {
-  return (P.epi & (ICAF_EPI_LN_FOLD | ICAF_EPI_EMIT_STATS)) ? launch_tc_x<BN, true>(P, pl, w, g, n_io, st) : launch_tc_x<BN, false>(P, pl, w, g, n_io, st);
-}
-
-template <bool XM>
-static int launch_persist_x(const ConvParams& P, const ConvPlan& pl, const __half* const (&w)[2], const icaf_conv_geom* g, int n_io, cudaStream_t st) {
-  static bool configured[kMaxDevices] = {false};
-  if (int rc = configure_smem(conv_gemm_persist_kernel<XM>, 227 * 1024, configured, "conv2d: cudaFuncSetAttribute")) return rc;
-  ConvMaps maps;
-  if (int rc = encode_maps<128>(P, w, g, n_io, maps)) return rc;
-  launch_k(conv_gemm_persist_kernel<XM>, dim3(unsigned(pl.ctas)), dim3(kPersistThreads), (size_t)pl.smem, st, P, maps);
-  return check_launch("conv2d_fwd");
-}
-static int launch_persist(const ConvParams& P, const ConvPlan& pl, const __half* const (&w)[2], const icaf_conv_geom* g, int n_io, cudaStream_t st) {
-  return (P.epi & (ICAF_EPI_LN_FOLD | ICAF_EPI_EMIT_STATS)) ? launch_persist_x<true>(P, pl, w, g, n_io, st) : launch_persist_x<false>(P, pl, w, g, n_io, st);
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -807,7 +737,7 @@ static int plan_conv(const icaf_conv_geom* g, int n_io, int sms, ConvParams& P, 
   switch (bn) {
     case 128: {
       if (int rc = plan_tc<128>(P, n_io, pl)) return rc;
-      return (P.a_mode != A_GATHER && P.splits == 1 && pl.total > sms) ? plan_persist(P, pl) : ICAF_OK;
+      return (P.a_mode != A_GATHER && P.splits == 1 && pl.tiles > sms) ? plan_persist(P, pl) : ICAF_OK;
     }
     case 64: return plan_tc<64>(P, n_io, pl);
     default: return plan_tc<32>(P, n_io, pl);
@@ -832,7 +762,7 @@ extern "C" int icaf_conv2d_plan(const icaf_conv_geom* g, int n_io, int sm_count,
   out->tile_w = P.tw; out->tile_h = P.th; out->tiles_x = P.tiles_x; out->tiles_y = P.tiles_y;
   out->cblk = P.cblk; out->halo = 0; out->stages = P.stages; out->splits = P.splits;
   out->grid_x = int(pl.grid_x); out->grid_y = int(pl.grid_y); out->grid_z = int(pl.grid_z); out->cluster = int(pl.cluster);
-  out->smem_bytes = pl.smem; out->work_items = pl.total; out->ctas = pl.ctas;
+  out->smem_bytes = pl.smem; out->work_items = pl.tiles; out->ctas = pl.ctas;
   return ICAF_OK;
 }
 
@@ -846,9 +776,9 @@ extern "C" int icaf_conv2d_fwd(const icaf_conv_geom* g, const icaf_conv_io* io, 
   if (rc) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   switch (pl.bn) {
-    case 128: return pl.persist ? launch_persist(P, pl, w, g, n_io, st) : launch_tc<128>(P, pl, w, g, n_io, st);
-    case 64: return launch_tc<64>(P, pl, w, g, n_io, st);
-    case 32: return launch_tc<32>(P, pl, w, g, n_io, st);
+    case 128: return launch_conv<128>(P, pl, w, g, n_io, st);
+    case 64: return launch_conv<64>(P, pl, w, g, n_io, st);
+    case 32: return launch_conv<32>(P, pl, w, g, n_io, st);
     default: return set_error(ICAF_ERR_BAD_ARG, "conv2d: the planner produced an unknown tile width");
   }
 }
