@@ -36,6 +36,8 @@ struct ConvParams {
 struct ConvMaps {          // TMA descriptors, passed by value as a __grid_constant__ kernel parameter
   CUtensorMap w[2];
   CUtensorMap a[2];
+  CUtensorMap y[2];        // persistent kernel, fragment epilogue: output (and residual) tiles, 64-column boxes
+  CUtensorMap res[2];
 };
 
 __device__ __forceinline__ ConvProblem pick_problem(const ConvParams& P, unsigned z) {
@@ -93,41 +95,49 @@ __device__ __forceinline__ void epi_row_emit(const EpiRow& ex, const ConvParams&
   for (int i = s0; i < s1; ++i) sp[i] = i == s0 ? make_float2(ex.sum, ex.sumsq) : make_float2(0.f, 0.f);
 }
 
-// One 32-column chunk of one output row: + bias, activation, residual, fp16 store.
+// One output element before its fp16 rounding: accumulator a + column bias b + row bias, activation, residual rf.
 // ACT: 0 none, 1 SiLU, 2 GELU(erf).  RES: 0 none, 1 y = act(v) + res, 2 y = alpha*res + beta*v.
+// Both epilogues (epi_chunk on staged rows, epi_fragments on the accumulator registers) compute every element with it,
+// so they round identically.
+template <int ACT, int RES>
+__device__ __forceinline__ float epi_value(float a, float b, float rbias, float rf, float alpha, float beta) {
+  float t = a + b + rbias;
+  if (ACT == ICAF_ACT_SILU) t = silu_f(t);
+  if (ACT == ICAF_ACT_GELU) t = gelu_erf_f(t);
+  if (RES == 1) t = t + rf;
+  if (RES == 2) t = alpha * rf + beta * t;
+  return t;
+}
+
+// One 32-column chunk of one output row: + bias, activation, residual, fp16 store (see epi_value).
 template <int ACT, int RES, int XM = 0>
 __device__ __forceinline__ void epi_chunk(const uint32_t (&acc)[32], const float* __restrict__ sb, float rbias,
                                           float alpha, float beta, const __half* __restrict__ rp,
                                           __half* __restrict__ yp, bool vec, int ncols, EpiRow& ex, int cb, bool do_store = true) {
-  auto f = [&](int j) {
+  auto f = [&](int j, float rf) {
     float a = __uint_as_float(acc[j]);
     if (XM == 1) a = ex.ln_a * (a - ex.ln_mu * __ldg(ex.ln_s + cb + j));
-    float t = a + sb[j] + rbias;
-    if (ACT == ICAF_ACT_SILU) t = silu_f(t);
-    if (ACT == ICAF_ACT_GELU) t = gelu_erf_f(t);
-    return t;
+    return epi_value<ACT, RES>(a, sb[j], rbias, rf, alpha, beta);
   };
   if (vec) {
 #pragma unroll
     for (int q = 0; q < 4; ++q) {
-      float v[8];
-#pragma unroll
-      for (int e = 0; e < 8; ++e) v[e] = f(q * 8 + e);
+      float rf[8];
       if (RES != 0) {
         uint4 rr = *reinterpret_cast<const uint4*>(rp + q * 8);
         const __half2* rh = reinterpret_cast<const __half2*>(&rr);
 #pragma unroll
         for (int e = 0; e < 4; ++e) {
-          float2 rf = __half22float2(rh[e]);
-          if (RES == 2) {
-            v[2 * e] = alpha * rf.x + beta * v[2 * e];
-            v[2 * e + 1] = alpha * rf.y + beta * v[2 * e + 1];
-          } else {
-            v[2 * e] += rf.x;
-            v[2 * e + 1] += rf.y;
-          }
+          const float2 r2 = __half22float2(rh[e]);
+          rf[2 * e] = r2.x; rf[2 * e + 1] = r2.y;
         }
+      } else {
+#pragma unroll
+        for (int e = 0; e < 8; ++e) rf[e] = 0.f;
       }
+      float v[8];
+#pragma unroll
+      for (int e = 0; e < 8; ++e) v[e] = f(q * 8 + e, rf[e]);
       uint4 o;
       o.x = pack_half2(v[0], v[1]); o.y = pack_half2(v[2], v[3]);
       o.z = pack_half2(v[4], v[5]); o.w = pack_half2(v[6], v[7]);
@@ -146,11 +156,7 @@ __device__ __forceinline__ void epi_chunk(const uint32_t (&acc)[32], const float
 #pragma unroll
     for (int j = 0; j < 32; ++j) {
       if (j < ncols) {
-        float t = f(j);
-        if (RES != 0) {
-          float rf = __half2float(rp[j]);
-          t = RES == 2 ? alpha * rf + beta * t : t + rf;
-        }
+        const float t = f(j, RES != 0 ? __half2float(rp[j]) : 0.f);
         const __half h = __float2half_rn(t);
         if (XM == 2) { const float w = __half2float(h); ex.sum += w; ex.sumsq += w * w; }
         yp[j] = h;

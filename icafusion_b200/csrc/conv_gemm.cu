@@ -20,9 +20,10 @@
 // tiles (BN <= 64) let two CTAs share an SM so that one CTA's epilogue overlaps the other's main loop.  Split-K: the
 // CTAs of a cluster take a K range each; the leader adds the others' staged tiles through distributed shared memory.
 // conv_gemm_persist_kernel: BN = 128 grids of more than one wave with TMA-staged A -- one persistent CTA per SM, a TMA
-// producer warpgroup and two consumer warpgroups that take turns on the main loop (see its own comment below).
-// The two kernels share the TMA producer stage (load_stage), the main loop (mma_loop), the tile origin and the staged-row
-// load and epi_chunk dispatch of the epilogue, so they compute bit-identical tiles.
+// producer warpgroup and two consumer warpgroups that take turns on the main loop; each consumer runs the epilogue on its
+// accumulator registers and writes the tile with TMA stores (see its own comment below).
+// The two kernels share the TMA producer stage (load_stage), the main loop (mma_loop), the tile origin and the
+// per-element epilogue expression (epi_value), so they compute bit-identical tiles.
 #include <cstdlib>
 #include <cstring>
 
@@ -323,16 +324,24 @@ conv_gemm_tc_kernel(const ConvParams P, const __grid_constant__ ConvMaps maps) {
 // m-tile, then problem, so that the CTAs resident at the same time read the same A rows.  384 threads:
 //   warpgroup 0    : TMA producer (one elected thread), running straight on from one tile's K blocks into the next one's
 //   warpgroups 1, 2: consumers; warpgroup 1 + (j % 2) owns the CTA's j-th tile.  An ordering barrier hands the main loop
-//                    from one consumer to the other, so one warpgroup's epilogue runs while the other's MMAs run.  The
-//                    epilogue stages the accumulators through the warpgroup's own smem buffer 32 columns at a time
-//                    (thread t owns tile row t).
+//                    from one consumer to the other, so one warpgroup's epilogue runs while the other's MMAs run.
+// Each consumer owns a 128 x 128 fp16 output tile in shared memory: two 64-column halves of 128-byte rows, 128B-swizzled
+// (the layout a TMA box of 64 columns x 128 rows has).  The epilogue runs on the accumulator registers (epi_fragments),
+// writes fp16 pairs into the tile with stmatrix and one thread stores each half with a TMA store, which clips the rows and
+// columns outside the output and completes while the warpgroup goes on to its next tile.  A residual tile is TMA-loaded
+// into the same buffer when the tile starts and overwritten in place.  XM (LayerNorm fold / row statistics) keeps the
+// row epilogue of epi_chunk: the accumulators are staged 32 columns at a time through the first 18 KB of the buffer
+// (thread t owns tile row t).
 constexpr int kPersistThreads = 384;
 struct PersistLayout {
   static constexpr int kStageBytes = SmemLayout<128>::kStageBytes;
-  static constexpr int kPitch = 32 + 4;                        // floats per staged row of a 32-column chunk
+  static constexpr int kHalfBytes = BM * 64 * 2;               // one 64-column half of the output tile
+  static constexpr int kOutBytes = 2 * kHalfBytes;             // per consumer, 1024-byte aligned (TMA 128B swizzle)
+  static constexpr int kPitch = 32 + 4;                        // XM: floats per staged row of a 32-column chunk
   static constexpr int kChunkBytes = BM * kPitch * 4;
-  // [ring: stages x (A|B)] [2 x staged chunk] [barriers 256 B] [2 x bias 128 fp32] ; + 1024 B alignment slack
-  __host__ __device__ static int bar_off(int stages) { return stages * kStageBytes + 2 * kChunkBytes; }
+  static_assert(kChunkBytes <= kOutBytes, "the XM staged chunk lives in the output tile");
+  // [ring: stages x (A|B)] [2 x output tile] [barriers 256 B] [2 x bias 128 fp32] ; + 1024 B alignment slack
+  __host__ __device__ static int bar_off(int stages) { return stages * kStageBytes + 2 * kOutBytes; }
   static int total(int stages) { return bar_off(stages) + 256 + 2 * 128 * 4 + 1024; }
 };
 
@@ -359,6 +368,54 @@ __device__ __forceinline__ void stage_chunk(const float (&acc0)[64], const float
   }
 }
 
+// columns [16 PP, 16 PP + 16) of the warpgroup's accumulators: v[0..7] from rows 0-63 (acc0), v[8..15] from rows 64-127
+template <int PP>
+__device__ __forceinline__ void take_cols16(const float (&acc0)[64], const float (&acc1)[64], float (&v)[16]) {
+#pragma unroll
+  for (int e = 0; e < 8; ++e) { v[e] = acc0[8 * PP + e]; v[8 + e] = acc1[8 * PP + e]; }
+}
+
+// Epilogue of 16 columns (take_cols16) on the accumulator registers: epi_value per element, fp16 pairs into the output
+// tile with stmatrix.  Register pair k of v[8h ...] is tile row 16w + l/4 + 8 (k % 2) + 64h, columns 8 (k / 2) + 2 (l % 4)
+// (+0, +1) of the 16: exactly one register of matrix k of an m8n8.x4 stmatrix.  sa: this lane's stmatrix row address for
+// rows 0-63 (rows 64-127 are 8 KB further); RES != 0 reads the residual pairs from the same place with ldmatrix first.
+// sb: column bias at the lane's column 2 (l % 4); rb: row bias of the lane's rows l/4 + {0, 8, 64, 72}.
+template <int ACT, int RES>
+__device__ __forceinline__ void epi_fragments(const float (&v)[16], uint32_t sa, const float* sb, const float (&rb)[4],
+                                              float alpha, float beta) {
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    uint32_t r[4];
+    if (RES != 0) ldmatrix_x4(r, sa + 8192u * h);
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const float2 b = *reinterpret_cast<const float2*>(sb + 8 * (k >> 1));
+      const float rbias = rb[2 * h + (k & 1)];
+      float2 rf = make_float2(0.f, 0.f);
+      if (RES != 0) rf = __half22float2(*reinterpret_cast<const __half2*>(&r[k]));
+      r[k] = pack_half2(epi_value<ACT, RES>(v[8 * h + 2 * k], b.x, rbias, rf.x, alpha, beta),
+                        epi_value<ACT, RES>(v[8 * h + 2 * k + 1], b.y, rbias, rf.y, alpha, beta));
+    }
+    stmatrix_x4(sa + 8192u * h, r);
+  }
+}
+
+// mode_act = 3 * ACT + RES, warp-uniform: dispatched once per 16 columns to straight-line code
+__device__ __forceinline__ void epi_fragments_dispatch(int mode_act, const float (&v)[16], uint32_t sa, const float* sb,
+                                                       const float (&rb)[4], float alpha, float beta) {
+  switch (mode_act) {
+    case 0: epi_fragments<0, 0>(v, sa, sb, rb, alpha, beta); break;
+    case 1: epi_fragments<0, 1>(v, sa, sb, rb, alpha, beta); break;
+    case 2: epi_fragments<0, 2>(v, sa, sb, rb, alpha, beta); break;
+    case 3: epi_fragments<1, 0>(v, sa, sb, rb, alpha, beta); break;
+    case 4: epi_fragments<1, 1>(v, sa, sb, rb, alpha, beta); break;
+    case 5: epi_fragments<1, 2>(v, sa, sb, rb, alpha, beta); break;
+    case 6: epi_fragments<2, 0>(v, sa, sb, rb, alpha, beta); break;
+    case 7: epi_fragments<2, 1>(v, sa, sb, rb, alpha, beta); break;
+    default: epi_fragments<2, 2>(v, sa, sb, rb, alpha, beta); break;
+  }
+}
+
 template <bool XM>
 __global__ void __launch_bounds__(kPersistThreads, 1)
 conv_gemm_persist_kernel(const ConvParams P, const __grid_constant__ ConvMaps maps) {
@@ -372,6 +429,7 @@ conv_gemm_persist_kernel(const ConvParams P, const __grid_constant__ ConvMaps ma
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (kMaxStages + s); };
   auto order_bar = [&](int c) { return bar_base + 8u * (2 * kMaxStages + c); };   // consumer c may start its main loop
+  auto res_bar = [&](int c) { return bar_base + 8u * (2 * kMaxStages + 2 + c); }; // consumer c's residual tile has landed
   uint8_t* smem_gen = smem_raw + (smem_base - smem_u32(smem_raw));
 
   pdl_launch_dependents();
@@ -379,6 +437,7 @@ conv_gemm_persist_kernel(const ConvParams P, const __grid_constant__ ConvMaps ma
   const int wg = tid >> 7;
   const int nkb = P.k_pad / BK;
   const int a_mode = P.a_mode;
+  const bool has_res = (P.epi & (ICAF_EPI_ADD_RES | ICAF_EPI_SCALED_RES)) != 0;
   if (tid == 0) {
     for (int s = 0; s < kStages; ++s) {
       mbar_init(full_bar(s), 1);
@@ -386,12 +445,18 @@ conv_gemm_persist_kernel(const ConvParams P, const __grid_constant__ ConvMaps ma
     }
     mbar_init(order_bar(0), 4);
     mbar_init(order_bar(1), 4);
+    mbar_init(res_bar(0), 1);
+    mbar_init(res_bar(1), 1);
     fence_mbar_init();
   }
   if (tid == 32) {
     tma_prefetch_desc(&maps.w[0]);
     tma_prefetch_desc(&maps.a[0]);
     if (P.tiles > P.m_tiles * P.n_tiles) { tma_prefetch_desc(&maps.w[1]); tma_prefetch_desc(&maps.a[1]); }
+    if (!XM) {
+      tma_prefetch_desc(&maps.y[0]);
+      if (has_res) tma_prefetch_desc(&maps.res[0]);
+    }
   }
   __syncthreads();
   pdl_wait();   // prologue (barriers, descriptor prefetch) overlapped the previous kernel
@@ -423,42 +488,75 @@ conv_gemm_persist_kernel(const ConvParams P, const __grid_constant__ ConvMaps ma
   const int c = wg - 1;
   const int t = tid & 127, w = t >> 5, l = t & 31;
   const int bar_id = 2 + c;                                   // warpgroup-local named barrier
-  float* sacc = reinterpret_cast<float*>(smem_gen + kStages * L::kStageBytes + c * PL::kChunkBytes);
+  const uint32_t sout = smem_base + uint32_t(kStages * L::kStageBytes + c * PL::kOutBytes);   // this consumer's output tile
+  float* sacc = reinterpret_cast<float*>(smem_gen + kStages * L::kStageBytes + c * PL::kOutBytes);   // XM: staged chunk
   float* sbias = reinterpret_cast<float*>(smem_gen + bar_off + 256 + c * 128 * 4);
+  // output / residual box: 64 columns x 128 rows (2-D) or 64 columns x tw x th pixels (4-D)
+  const uint32_t half_bytes = a_mode == A_TMA2D ? uint32_t(PL::kHalfBytes) : uint32_t(P.tw * P.th) * 128u;
   for (int tile = blockIdx.x + c * gridDim.x; tile < P.tiles; tile += 2 * gridDim.x) {
     const int j = (tile - int(blockIdx.x)) / int(gridDim.x);  // ordinal of the tile among this CTA's tiles
     const PersistTile pt = persist_tile(P, tile);
     const ConvProblem pr = pick_problem(P, pt.z);
     const int n0 = pt.n0;
     const TileOrigin& o = pt.o;
+    const int halves = n0 + 64 < P.N ? 2 : 1;                 // 64-column halves of the tile inside the output
+    // tile row -> output row m; valid: inside the map (4-D: tw divides Wo; the last tile row of an image may hang over)
+    auto out_row = [&](int row, int& m, bool& valid) {
+      if (a_mode == A_TMA4D) {
+        const int ry = row / P.tw, rx = row - ry * P.tw;
+        m = (o.tb * P.Ho + o.oy0 + ry) * P.Wo + o.ox0 + rx;
+        valid = ry < P.th && o.oy0 + ry < P.Ho;
+      } else {
+        m = o.m0 + row;
+        valid = m < P.M;
+      }
+    };
     // Epilogue operands that do not depend on the main loop are fetched now so their DRAM latency hides behind it:
-    // bias slice and (alpha, beta) into registers, this thread's residual row into L2.
+    // bias slice and (alpha, beta) into registers; XM: this thread's residual row into L2; otherwise the residual tile.
     const float bias_r = (pr.bias && !(P.epi & ICAF_EPI_BIAS_ROW) && n0 + t < P.N) ? __ldg(pr.bias + n0 + t) : 0.f;
     float alpha = 0.f, beta = 1.f;
     if (P.epi & ICAF_EPI_SCALED_RES) { alpha = __ldg(pr.alpha); beta = __ldg(pr.beta); }
     const int row = t;
     int m;
     bool mvalid;
-    if (a_mode == A_TMA4D) {
-      const int ry = row / P.tw, rx = row - ry * P.tw;
-      m = (o.tb * P.Ho + o.oy0 + ry) * P.Wo + o.ox0 + rx;
-      mvalid = ry < P.th && o.oy0 + ry < P.Ho;    // tw divides Wo; the last tile row of an image may hang over
-    } else {
-      m = o.m0 + row;
-      mvalid = m < P.M;
-    }
+    out_row(row, m, mvalid);
     const float rbias = ((P.epi & ICAF_EPI_BIAS_ROW) && pr.bias && mvalid) ? __ldg(pr.bias + m) : 0.f;
     __half* yrow = pr.y + size_t(mvalid ? m : 0) * pr.y_ld;
     const __half* rrow = pr.res ? pr.res + size_t(mvalid ? m : 0) * pr.res_ld : nullptr;
-    const int mode = (P.epi & ICAF_EPI_SCALED_RES) ? 2 : (rrow ? 1 : 0);
-    if (rrow && mvalid) {
-      for (int cb = 0; cb < 128 && n0 + cb < P.N; cb += 64) prefetch_l2(rrow + n0 + cb);
-    }
+    const int mode = (P.epi & ICAF_EPI_SCALED_RES) ? 2 : (has_res ? 1 : 0);
     EpiRow ex;
     ex.sum = ex.sumsq = 0.f; ex.ln_a = 1.f; ex.ln_mu = 0.f; ex.ln_s = nullptr;
+    float rb[4] = {0.f, 0.f, 0.f, 0.f};      // !XM: row bias of this lane's accumulator rows l/4 + {0, 8, 64, 72}
     if (XM) {
+      if (rrow && mvalid) {
+        for (int cb = 0; cb < 128 && n0 + cb < P.N; cb += 64) prefetch_l2(rrow + n0 + cb);
+      }
       ex.ln_s = pr.ln_s ? pr.ln_s + n0 : nullptr;
       if (P.ln_parts > 0) epi_row_ln(ex, P, pr, m, mvalid);
+    } else {
+      if ((P.epi & ICAF_EPI_BIAS_ROW) && pr.bias) {
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+          int mq;
+          bool vq;
+          out_row(16 * w + (l >> 2) + 8 * (q & 1) + 64 * (q >> 1), mq, vq);
+          rb[q] = vq ? __ldg(pr.bias + mq) : 0.f;
+        }
+      }
+      if (t == 0) {
+        bulk_wait_group_read<0>();                            // the previous tile's TMA store has read the buffer
+        if (has_res) {
+          const CUtensorMap* mr = pt.z ? &maps.res[1] : &maps.res[0];
+          mbar_arrive_expect_tx(res_bar(c), uint32_t(halves) * half_bytes);
+          for (int hh = 0; hh < halves; ++hh) {
+            const uint32_t dst = sout + uint32_t(hh * PL::kHalfBytes);
+            if (a_mode == A_TMA2D) tma_load_2d(dst, mr, res_bar(c), n0 + 64 * hh, o.m0);
+            else tma_load_4d(dst, mr, res_bar(c), n0 + 64 * hh, o.ox0, o.oy0, o.tb);
+          }
+        }
+      }
+      sbias[t] = bias_r;
+      named_bar_sync(bar_id, 128);                            // bias slice complete, output tile free
     }
 
     // ---- main loop.  Tile j's K blocks are ring blocks j*nkb ... j*nkb + nkb - 1.  Waiting for the other consumer's
@@ -476,9 +574,49 @@ conv_gemm_persist_kernel(const ConvParams P, const __grid_constant__ ConvMaps ma
     wgmma_wait<0>();
     hand_back(s_last);
 
-    // ---- epilogue, 32 columns at a time
-    // XM: 9 / 10 = LayerNorm folded into this GEMM (no activation / GELU); 11 = scaled residual + statistics of the output rows
-    const int mode_act = XM ? (P.ln_parts > 0 ? (P.act == ICAF_ACT_GELU ? 10 : 9) : 11) : P.act * 3 + mode;
+    if constexpr (!XM) {
+      // ---- epilogue on the accumulator registers, 16 columns at a time, then the TMA store of the tile
+      if (has_res) mbar_wait_quiet(res_bar(c), uint32_t(j >> 1) & 1u);
+      const int mode_act = P.act * 3 + mode;
+      const uint32_t sa = sout + uint32_t(16 * w + (l & 7) + 8 * ((l >> 3) & 1)) * 128u;   // stmatrix row of this lane
+      const float* sb = sbias + 2 * (l & 3);
+#pragma unroll 1
+      for (int p = 0; p < 8; ++p) {
+        float v[16];
+        switch (p) {
+          case 0: take_cols16<0>(acc0, acc1, v); break;
+          case 1: take_cols16<1>(acc0, acc1, v); break;
+          case 2: take_cols16<2>(acc0, acc1, v); break;
+          case 3: take_cols16<3>(acc0, acc1, v); break;
+          case 4: take_cols16<4>(acc0, acc1, v); break;
+          case 5: take_cols16<5>(acc0, acc1, v); break;
+          case 6: take_cols16<6>(acc0, acc1, v); break;
+          default: take_cols16<7>(acc0, acc1, v); break;
+        }
+        // half p / 4 of the tile; 16-byte chunk 2 (p % 4) + l / 16 of the 128-byte row, 128B-swizzled by the row
+        const uint32_t a = sa + uint32_t(p >> 2) * uint32_t(PL::kHalfBytes) + (uint32_t((2 * (p & 3) + (l >> 4)) ^ (l & 7)) << 4);
+        epi_fragments_dispatch(mode_act, v, a, sb + 16 * p, rb, alpha, beta);
+      }
+      fence_proxy_async_smem();                             // the tile is visible to the TMA unit ...
+      named_bar_sync(bar_id, 128);                          // ... once every thread of the warpgroup has written its part
+      if (t == 0) {
+        const CUtensorMap* my = pt.z ? &maps.y[1] : &maps.y[0];
+        for (int hh = 0; hh < halves; ++hh) {
+          const uint32_t src = sout + uint32_t(hh * PL::kHalfBytes);
+          if (a_mode == A_TMA2D) tma_store_2d(my, src, n0 + 64 * hh, o.m0);
+          else tma_store_4d(my, src, n0 + 64 * hh, o.ox0, o.oy0, o.tb);
+        }
+        bulk_commit_group();
+        // this consumer's last tile: its writes complete before the grid does (dependent launches read them after
+        // griddepcontrol.wait).  Waiting inside the loop keeps the consumer's code one setmaxnreg region for ptxas.
+        if (tile + 2 * int(gridDim.x) >= P.tiles) bulk_wait_group<0>();
+      }
+      continue;
+    }
+
+    // ---- XM epilogue, 32 columns at a time
+    // 9 / 10 = LayerNorm folded into this GEMM (no activation / GELU); 11 = scaled residual + statistics of the output rows
+    const int mode_act = P.ln_parts > 0 ? (P.act == ICAF_ACT_GELU ? 10 : 9) : 11;
     const float* arow = sacc + size_t(row) * PL::kPitch;
 #pragma unroll 1
     for (int cc = 0; cc < 4; ++cc) {
@@ -505,7 +643,7 @@ conv_gemm_persist_kernel(const ConvParams P, const __grid_constant__ ConvMaps ma
         epi_dispatch<XM>(mode_act, acc, sb, rbias, alpha, beta, rp, yp, vec, ncols, ex, cb);
       }
     }
-    if (XM && mode_act == 11 && mvalid && n0 < P.N) epi_row_emit(ex, P, pr, m, n0, min(n0 + 128, P.N));
+    if (mode_act == 11 && mvalid && n0 < P.N) epi_row_emit(ex, P, pr, m, n0, min(n0 + 128, P.N));
   }
 }
 
@@ -683,8 +821,12 @@ static int plan_persist(ConvParams& P, ConvPlan& pl) {
   return ICAF_OK;
 }
 
+// out_maps: the output (and residual) maps of the persistent kernel's TMA-store epilogue, 64-column boxes of the tile's rows
+// (2-D: 128 rows of [M][N]; 4-D: the tw x th patch of the (N, Wo, Ho, B) view).  They span N columns, so a tile never
+// writes the channels next to a slice of a wider buffer.
 template <int BN>
-static int encode_maps(const ConvParams& P, const __half* const (&w)[2], const icaf_conv_geom* g, int n_io, ConvMaps& maps) {
+static int encode_maps(const ConvParams& P, const __half* const (&w)[2], const icaf_conv_geom* g, int n_io, bool out_maps,
+                       ConvMaps& maps) {
   memset(&maps, 0, sizeof(maps));
   for (int i = 0; i < n_io; ++i) {
     int rc = encode_tmap_2d(&maps.w[i], w[i], (uint64_t)P.k_pad, (uint64_t)g->w_rows, (uint64_t)P.k_pad * 2, BK, BN);
@@ -696,13 +838,22 @@ static int encode_maps(const ConvParams& P, const __half* const (&w)[2], const i
       rc = encode_tmap_nhwc(&maps.a[i], pr.x, P.Cin, P.Wi, P.Hi, P.B, pr.x_ld, BK, P.tw * P.stride, P.th * P.stride, P.stride,
                             P.stride);
     if (rc) return rc;
+    if (out_maps) {
+      auto out_map = [&](CUtensorMap* m, const __half* base, long long ld) {
+        return P.a_mode == A_TMA2D ? encode_tmap_2d(m, base, (uint64_t)P.N, (uint64_t)P.M, (uint64_t)ld * 2, 64, BM)
+                                   : encode_tmap_nhwc(m, base, P.N, P.Wo, P.Ho, P.B, ld, 64, P.tw, P.th, 1, 1);
+      };
+      if ((rc = out_map(&maps.y[i], pr.y, pr.y_ld))) return rc;
+      if (pr.res && (rc = out_map(&maps.res[i], pr.res, pr.res_ld))) return rc;
+    }
   }
-  if (n_io == 1) { maps.w[1] = maps.w[0]; maps.a[1] = maps.a[0]; }
+  if (n_io == 1) { maps.w[1] = maps.w[0]; maps.a[1] = maps.a[0]; maps.y[1] = maps.y[0]; maps.res[1] = maps.res[0]; }
   return ICAF_OK;
 }
 
 // Launch a planned conv on the kernel the plan picked (XM: the LayerNorm-fold / row-statistics instantiation).  Its
-// shared-memory limit is raised once per device; the filter maps are encoded for the plan's tile width.
+// shared-memory limit is raised once per device; the filter maps are encoded for the plan's tile width, and the output
+// maps for the persistent kernel's TMA-store epilogue.
 template <int BN>
 static int launch_conv(const ConvParams& P, const ConvPlan& pl, const __half* const (&w)[2], const icaf_conv_geom* g, int n_io,
                        cudaStream_t st) {
@@ -712,7 +863,7 @@ static int launch_conv(const ConvParams& P, const ConvPlan& pl, const __half* co
   static bool configured[2][2][kMaxDevices] = {};
   if (int rc = configure_smem(kernel, 227 * 1024, configured[pl.persist][xm], "conv2d: cudaFuncSetAttribute")) return rc;
   ConvMaps maps;
-  if (int rc = encode_maps<BN>(P, w, g, n_io, maps)) return rc;
+  if (int rc = encode_maps<BN>(P, w, g, n_io, pl.persist && !xm, maps)) return rc;
   // the one-tile kernel takes the tile grid (split-K: in clusters along x); the persistent one `ctas` CTAs
   const dim3 grid = pl.persist ? dim3(unsigned(pl.ctas)) : dim3(pl.grid_x, pl.grid_y, pl.grid_z);
   launch_kc(kernel, grid, dim3(pl.persist ? kPersistThreads : kThreads), (size_t)pl.smem, st, pl.cluster, P, maps);
@@ -722,7 +873,8 @@ static int launch_conv(const ConvParams& P, const ConvPlan& pl, const __half* co
 // ---------------------------------------------------------------------------------------------------
 // The dispatcher, host only: staging mode, tile shape and tile width for one layer geometry.  No CUDA call.
 // (`pair_mode` of icaf_conv2d_plan selects CTA-pair kernels on architectures that have them; sm_90a has none.)
-static int plan_conv(const icaf_conv_geom* g, int n_io, int sms, ConvParams& P, ConvPlan& pl) {
+// persist_ok = false keeps an eligible launch on the one-tile kernel (its output cannot be written by TMA stores).
+static int plan_conv(const icaf_conv_geom* g, int n_io, int sms, ConvParams& P, ConvPlan& pl, bool persist_ok = true) {
   memset(&pl, 0, sizeof(pl));
   pl.sms = sms;
   if (sms < 1) return set_error(ICAF_ERR_BAD_ARG, "conv2d: SM count must be positive");
@@ -737,7 +889,7 @@ static int plan_conv(const icaf_conv_geom* g, int n_io, int sms, ConvParams& P, 
   switch (bn) {
     case 128: {
       if (int rc = plan_tc<128>(P, n_io, pl)) return rc;
-      return (P.a_mode != A_GATHER && P.splits == 1 && pl.tiles > sms) ? plan_persist(P, pl) : ICAF_OK;
+      return (persist_ok && P.a_mode != A_GATHER && P.splits == 1 && pl.tiles > sms) ? plan_persist(P, pl) : ICAF_OK;
     }
     case 64: return plan_tc<64>(P, n_io, pl);
     default: return plan_tc<32>(P, n_io, pl);
@@ -771,8 +923,17 @@ extern "C" int icaf_conv2d_fwd(const icaf_conv_geom* g, const icaf_conv_io* io, 
   const __half* w[2];
   int rc = fill_params(g, io, n_io, P, w);
   if (rc) return rc;
+  // The persistent kernel writes its outputs (and reads residuals) by TMA: 16-byte aligned base and row pitch.  The
+  // LayerNorm-fold / row-statistics epilogue (XM) stores rows directly and takes any layout.
+  bool tma_out = true;
+  for (int i = 0; i < n_io; ++i) {
+    const ConvProblem& pr = P.p[i];
+    tma_out = tma_out && (reinterpret_cast<uintptr_t>(pr.y) & 15) == 0 && pr.y_ld % 8 == 0 &&
+              (!pr.res || ((reinterpret_cast<uintptr_t>(pr.res) & 15) == 0 && pr.res_ld % 8 == 0));
+  }
+  const bool xm = (P.epi & (ICAF_EPI_LN_FOLD | ICAF_EPI_EMIT_STATS)) != 0;
   ConvPlan pl;
-  rc = plan_conv(g, n_io, sm_count_cached(), P, pl);
+  rc = plan_conv(g, n_io, sm_count_cached(), P, pl, xm || tma_out);
   if (rc) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   switch (pl.bn) {

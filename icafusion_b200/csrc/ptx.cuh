@@ -116,6 +116,35 @@ __device__ __forceinline__ void tma_load_4d(uint32_t dst, const void* tmap, uint
       : "memory");
 }
 
+// TMA stores (shared -> global, bulk-group completion): the box is clipped to the tensor's bounds.  The issuing thread
+// commits its stores as one group; wait_group_read<N> returns once all but N groups have finished reading shared memory
+// (the source may be rewritten), wait_group<N> once their writes are complete.
+__device__ __forceinline__ void tma_store_2d(const void* tmap, uint32_t src, int c0, int c1) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
+               ::"l"(tmap), "r"(src), "r"(c0), "r"(c1) : "memory");
+}
+__device__ __forceinline__ void tma_store_4d(const void* tmap, uint32_t src, int c0, int c1, int c2, int c3) {
+  asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];"
+               ::"l"(tmap), "r"(src), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
+}
+__device__ __forceinline__ void bulk_commit_group() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void bulk_wait_group_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
+template <int N>
+__device__ __forceinline__ void bulk_wait_group() { asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory"); }
+
+// ------------------------------------------------------------------ ldmatrix / stmatrix (four 8x8 b16 matrices)
+// Lane l gives the shared address of row l % 8 of matrix l / 8; register k holds, in every lane, the pair (row l / 4,
+// columns 2 (l % 4), +1) of matrix k -- the pair layout of the wgmma accumulator (see below).
+__device__ __forceinline__ void ldmatrix_x4(uint32_t (&r)[4], uint32_t addr) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr) : "memory");
+}
+__device__ __forceinline__ void stmatrix_x4(uint32_t addr, const uint32_t (&r)[4]) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};"
+               ::"r"(addr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]) : "memory");
+}
+
 // ------------------------------------------------------------------ wgmma (4th-gen tensor cores, sm_90a)
 // Shared-memory matrix descriptor.  [0,14) start >> 4 | [16,30) LBO >> 4 | [32,46) SBO >> 4 | [62,64) layout:
 // 1 = SWIZZLE_128B, 2 = SWIZZLE_64B, 3 = SWIZZLE_32B (CUTLASS' GmmaDescriptor).  Swizzled tiles keep their 1024-byte
