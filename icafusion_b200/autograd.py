@@ -386,9 +386,23 @@ def _layernorm(ln: nn.LayerNorm, x):
     return LayerNormFn.apply(x, ln.weight, ln.bias, ln.eps)
 
 
+# Head dims icaf_cross_attention_bwd is built for.  The forward runs every multiple of 8 up to 128, so a model can run in
+# eval() with a head dim (yolov5m: 24 / 48 / 96) that it cannot train with.
+ATTN_BWD_HEAD_DIMS = (8, 16, 32, 64, 128)
+
+
+def require_attention_backward(m):
+    """Raise NotImplementedError if the CrossAttention module `m` has a head dim without a backward kernel."""
+    d = m.d_model // m.h
+    if d not in ATTN_BWD_HEAD_DIMS:
+        raise NotImplementedError(f"training: cross-attention head dim {d} (d_model {m.d_model}, {m.h} heads) has no backward "
+                                  f"kernel; head dims {'/'.join(map(str, ATTN_BWD_HEAD_DIMS))} train")
+
+
 def cross_attention(m, r2, i2, B: int, N: int, n_pad: int):
     """common.py:641-687 on (B*n_pad, C) token matrices: LN -> one [q|k|v] GEMM per modality -> attention with dropout on the
     probabilities -> output projection -> dropout."""
+    require_attention_backward(m)
     C = m.d_model
     outs = []
     qkv = []
@@ -446,6 +460,10 @@ def detect(m, xs: Sequence[torch.Tensor]) -> List[torch.Tensor]:
 def model_forward(model, rgb_img: torch.Tensor, ir_img: torch.Tensor, taps: list = None):
     """The layer walk of Model.forward_once (yolo_test.py:136-163) over the training-mode nodes.  `taps` (diagnostics): receives
     every layer's NHWC output."""
+    from .common import CrossAttention
+    for mod in model.modules():          # refuse before the backbone launches anything
+        if isinstance(mod, CrossAttention):
+            require_attention_backward(mod)
     _STATE["defer_bn"], _STATE["bn"] = True, []
     try:
         return _walk(model, rgb_img, ir_img, taps)

@@ -57,9 +57,14 @@ def transfusion_kaist_cfg(size: str = "s", nc: int = 1) -> Dict:
             "anchors": copy.deepcopy(KAIST_ANCHORS), "backbone": rgb + ir + fusion, "head": head}
 
 
+# Stock dataset suffixes and their class counts: the reference's FLIR YAMLs differ from the KAIST ones only in nc.
+_DATASET_NC = {"_Transfusion_kaist": 1, "_Transfusion_FLIR": 3}
+
+
 def load_cfg(cfg: Union[str, Dict]) -> Dict:
     """Accepts a config dict, a YAML path in the reference's row format, or a stock name
-    ('yolov5s_Transfusion_kaist', 'yolov5l_Transfusion_kaist', with or without '.yaml')."""
+    ('yolov5{n,s,m,l,x}_Transfusion_kaist' or '..._Transfusion_FLIR', with or without '.yaml').  Other datasets' YAMLs
+    load by path; ``Model(cfg, nc=...)`` overrides the class count of any of them."""
     if isinstance(cfg, dict):
         out = copy.deepcopy(cfg)
     else:
@@ -70,8 +75,8 @@ def load_cfg(cfg: Union[str, Dict]) -> Dict:
             import yaml
             with open(cfg) as f:
                 out = yaml.safe_load(f)
-        elif stem.startswith("yolov5") and stem.endswith("_Transfusion_kaist") and stem[6] in _MULT:
-            out = transfusion_kaist_cfg(stem[6])
+        elif stem.startswith("yolov5") and len(stem) > 6 and stem[6] in _MULT and stem[7:] in _DATASET_NC:
+            out = transfusion_kaist_cfg(stem[6], nc=_DATASET_NC[stem[7:]])
         else:
             raise FileNotFoundError(cfg)
     # resolve the two symbolic Detect args like parse_model's eval() does (yolo_test.py:225-229)

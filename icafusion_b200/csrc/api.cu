@@ -95,6 +95,27 @@ int encode_tmap_2d(CUtensorMap* out, const void* base, uint64_t inner, uint64_t 
   return ICAF_OK;
 }
 
+int encode_tmap_3d(CUtensorMap* out, const void* base, const uint64_t (&dims)[3], uint64_t pitch1_bytes, uint64_t pitch2_bytes,
+                   const uint32_t (&box)[3]) {
+  EncodeTiledFn fn = encode_fn();
+  if (!fn) return set_error(ICAF_ERR_CUDA, "cuTensorMapEncodeTiled entry point not available");
+  cuuint64_t gdims[3] = {dims[0], dims[1], dims[2]};
+  cuuint64_t strides[2] = {pitch1_bytes, pitch2_bytes};
+  cuuint32_t gbox[3] = {box[0], box[1], box[2]};
+  cuuint32_t estr[3] = {1, 1, 1};
+  const CUtensorMapSwizzle swz = box[0] >= 64 ? CU_TENSOR_MAP_SWIZZLE_128B : (box[0] == 32 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B);
+  CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, const_cast<void*>(base), gdims, strides, gbox, estr,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, swz, l2_promotion(dims[0] * 2, pitch1_bytes), CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) {
+    char msg[200];
+    snprintf(msg, sizeof(msg), "cuTensorMapEncodeTiled(3d dims=%llu,%llu,%llu pitch=%llu,%llu box=%u,%u,%u) failed: %d",
+             (unsigned long long)dims[0], (unsigned long long)dims[1], (unsigned long long)dims[2], (unsigned long long)pitch1_bytes,
+             (unsigned long long)pitch2_bytes, box[0], box[1], box[2], int(r));
+    return set_error(ICAF_ERR_CUDA, msg);
+  }
+  return ICAF_OK;
+}
+
 int encode_tmap_nhwc(CUtensorMap* out, const void* base, int C, int W, int H, int B, int64_t ld, uint32_t box_c,
                      uint32_t box_w, uint32_t box_h, uint32_t sw, uint32_t sh) {
   EncodeTiledFn fn = encode_fn();

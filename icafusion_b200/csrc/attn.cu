@@ -39,6 +39,13 @@ struct AttnParams {
 //   V^T tiles  : two boxes (64 keys x D feature rows) of the (C, B*Npad) matrix -> K-major SW128 (keys are the K dim of PV)
 //   V tiles    : (VF, fused [q|k|v] rows) boxes like K's at column 2C + head*D -> rows = keys, i.e. an MN-major B operand
 // Rows / keys past the tensor are zero-filled by the TMA unit; keys in [N, ...) are masked in the softmax.
+//
+// PAD: head dims d = 8 / 24 / 40 ... 120 (multiples of 8 that are not a power of two >= 16) run the kernel of the next width
+// D = 16 / 32 / 64 / 128 over 3-D maps that give every head its own extent, so columns d .. D-1 of a tile are out of
+// bounds and zero-filled instead of reading the next head:
+//   Q / K / V tiles: (d, k*heads, B*Npad) view of the projection matrix (k = 2 split, 3 fused), box (min(D,64), 1, rows)
+//   V^T tiles      : (B*Npad, d, heads) view of the (C, B*Npad) matrix, box (64, D, 1)
+// The zero columns add exactly 0 to S = Q K^T and produce zero columns of O = P V, which are not stored.
 struct AttnMaps {
   CUtensorMap qk[2];   // [0] = vis, [1] = ir : (B*Npad rows, 2C | 3C cols), box (min(D,64), 128) -- Q tiles
   CUtensorMap kv[2];   // same matrices, box (min(D,64), KV) -- K tiles (and V tiles in the fused form)
@@ -46,9 +53,10 @@ struct AttnMaps {
 };
 
 // KV = keys per tile (N of S, K of PV).  Head dims 16 / 32 run 64-key tiles (less masked work at the DMFF token counts).
-template <int D>
+// The padded dropout kernel at D = 128 takes 64-key tiles too: with 128 it would spill, like the unpadded one does.
+template <int D, bool TRAIN = false, bool PAD = false>
 struct AttnCfg {
-  static constexpr int kKV = D <= 32 ? 64 : 128;
+  static constexpr int kKV = D <= 32 || (TRAIN && PAD && D == 128) ? 64 : 128;
 };
 
 template <int D, int KV>
@@ -74,9 +82,10 @@ __device__ __forceinline__ float fast_exp2_t(float x) {
 
 // TRAIN: dropout on the attention probabilities (the row sum still runs over the un-dropped values, like
 // `att = softmax(..); att = attn_drop(att)`); its own instantiation, so the inference kernels keep their size.
-template <int D, bool VF, bool TRAIN = false>
+// PAD: the head dim C / heads is below D (see AttnMaps); its own instantiation too.
+template <int D, bool VF, bool TRAIN = false, bool PAD = false>
 __global__ void __launch_bounds__(288, 1) cross_attn_tma_kernel(const AttnParams P, const __grid_constant__ AttnMaps M) {
-  constexpr int kKV = AttnCfg<D>::kKV;
+  constexpr int kKV = AttnCfg<D, TRAIN, PAD>::kKV;
   using L = AttnSmemT<D, kKV>;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -189,21 +198,23 @@ __global__ void __launch_bounds__(288, 1) cross_attn_tma_kernel(const AttnParams
       wgmma_wait<0>();
       if (l == 0) mbar_arrive(kv_empty(buf));
     }
-    // ---- normalise and store (heads merged: column head*D) ; zero the pad rows ----
+    // ---- normalise and store (heads merged: column head*d) ; zero the pad rows ----
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       l_run[h] += __shfl_xor_sync(0xffffffffu, l_run[h], 1);
       l_run[h] += __shfl_xor_sync(0xffffffffu, l_run[h], 2);
     }
+    const int d = PAD ? C / P.heads : D;      // true head dim: columns d .. D-1 of o are the zero padding
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const int qn = h ? qn1 : qn0;
       if (qn < n_pad) {
         const float inv = qn < N ? 1.f / l_run[h] : 0.f;
-        __half* op = (dir == 0 ? P.out[0] : P.out[1]) + (size_t(b) * n_pad + qn) * C + head * D + 2 * (l & 3);
+        __half* op = (dir == 0 ? P.out[0] : P.out[1]) + (size_t(b) * n_pad + qn) * C + head * d + 2 * (l & 3);
 #pragma unroll
         for (int i = 2 * h; i < D / 2; i += 4)
-          *reinterpret_cast<uint32_t*>(op + 8 * (i >> 2)) = pack_half2(o[i] * inv, o[i + 1] * inv);
+          if (!PAD || 8 * (i >> 2) < d)
+            *reinterpret_cast<uint32_t*>(op + 8 * (i >> 2)) = pack_half2(o[i] * inv, o[i + 1] * inv);
       }
     }
   } else if (lane_id() == 0) {
@@ -213,25 +224,32 @@ __global__ void __launch_bounds__(288, 1) cross_attn_tma_kernel(const AttnParams
     const CUtensorMap* mv = dir == 0 ? &M.vt[0] : &M.vt[1];
     (void)mv;
     const int row_b = b * n_pad;
-    mbar_arrive_expect_tx(q_full, L::kQBytes);
+    // a tile = (column block kb of projection k's head `head`, rows r0 ..): 2-D coordinates, or 3-D ones over the padded view
+    auto load_tile = [&](uint32_t dst, const CUtensorMap* m, uint32_t bar, int k, int kb, int r0) {
+      if (PAD) tma_load_3d(dst, m, bar, kb * 64, k * P.heads + head, r0);
+      else tma_load_2d(dst, m, bar, k * C + head * D + kb * 64, r0);
+    };
+    mbar_arrive_expect_tx(q_full, L::kQBytes);      // overhanging boxes count in full: the zero fill arrives as bytes too
 #pragma unroll
     for (int kb = 0; kb < L::kKB; ++kb)
-      tma_load_2d(sbase + L::kQOff + kb * (kQT * 128), mq, q_full, head * D + kb * 64, row_b + q0);
+      load_tile(sbase + L::kQOff + kb * (kQT * 128), mq, q_full, 0, kb, row_b + q0);
     for (int j = 0; j < nkv; ++j) {
       const int buf = j & 1;
       if (j >= 2) mbar_wait(kv_empty(buf), ((j >> 1) & 1) ^ 1);     // PV(j-2) has drained this buffer
       mbar_arrive_expect_tx(kv_full(buf), L::kKBytes + L::kVBytes);
 #pragma unroll
       for (int kb = 0; kb < L::kKB; ++kb)
-        tma_load_2d(sbase + L::kKOff + buf * L::kKBytes + kb * (kKV * 128), mk, kv_full(buf), C + head * D + kb * 64, row_b + j * kKV);
+        load_tile(sbase + L::kKOff + buf * L::kKBytes + kb * (kKV * 128), mk, kv_full(buf), 1, kb, row_b + j * kKV);
       if (VF) {
 #pragma unroll
         for (int kb = 0; kb < L::kKB; ++kb)
-          tma_load_2d(sbase + L::kVOff + buf * L::kVBytes + kb * (kKV * 128), mk, kv_full(buf), 2 * C + head * D + kb * 64, row_b + j * kKV);
+          load_tile(sbase + L::kVOff + buf * L::kVBytes + kb * (kKV * 128), mk, kv_full(buf), 2, kb, row_b + j * kKV);
       } else {
 #pragma unroll
-        for (int kb = 0; kb < kKV / 64; ++kb)
-          tma_load_2d(sbase + L::kVOff + buf * L::kVBytes + kb * (D * 128), mv, kv_full(buf), row_b + j * kKV + kb * 64, head * D);
+        for (int kb = 0; kb < kKV / 64; ++kb) {
+          if (PAD) tma_load_3d(sbase + L::kVOff + buf * L::kVBytes + kb * (D * 128), mv, kv_full(buf), row_b + j * kKV + kb * 64, 0, head);
+          else tma_load_2d(sbase + L::kVOff + buf * L::kVBytes + kb * (D * 128), mv, kv_full(buf), row_b + j * kKV + kb * 64, head * D);
+        }
       }
     }
   }
@@ -289,7 +307,7 @@ static int fill_attn(const void* qk_vis, const void* qk_ir, const void* vt_vis, 
   if (!qk_vis || !qk_ir || (!vt_vis != !vt_ir) || !out_vis || !out_ir) return set_error(ICAF_ERR_BAD_ARG, "cross_attention: null pointer");
   if (B < 1 || N < 1 || n_pad < N || n_pad % 8 || heads < 1 || C % heads) return set_error(ICAF_ERR_BAD_ARG, "cross_attention: bad shape");
   int d = C / heads;
-  if (d != 16 && d != 32 && d != 64 && d != 128) return set_error(ICAF_ERR_UNSUPPORTED, "cross_attention: head dim must be 16/32/64/128");
+  if (d % 8 || d < 8 || d > 128) return set_error(ICAF_ERR_UNSUPPORTED, "cross_attention: head dim must be a multiple of 8 in [8, 128]");
   P.qk[0] = (const __half*)qk_vis; P.qk[1] = (const __half*)qk_ir;
   P.vt[0] = (const __half*)vt_vis; P.vt[1] = (const __half*)vt_ir;
   P.out[0] = (__half*)out_vis; P.out[1] = (__half*)out_ir;
@@ -300,19 +318,33 @@ static int fill_attn(const void* qk_vis, const void* qk_ir, const void* vt_vis, 
   return ICAF_OK;
 }
 
-template <int D, bool VF, bool TRAIN = false>
+template <int D, bool VF, bool TRAIN = false, bool PAD = false>
 static int launch_attn_tma(const AttnParams& P, cudaStream_t st) {
-  constexpr int kKV = AttnCfg<D>::kKV;
+  constexpr int kKV = AttnCfg<D, TRAIN, PAD>::kKV;
   using L = AttnSmemT<D, kKV>;
   static bool configured[kMaxDevices] = {false};
-  if (int rc = configure_smem(cross_attn_tma_kernel<D, VF, TRAIN>, L::kTotal, configured, "cross_attention: cudaFuncSetAttribute")) return rc;
+  if (int rc = configure_smem(cross_attn_tma_kernel<D, VF, TRAIN, PAD>, L::kTotal, configured, "cross_attention: cudaFuncSetAttribute")) return rc;
   AttnMaps maps;
   memset(&maps, 0, sizeof(maps));
   const uint64_t rows = uint64_t(P.B) * P.n_pad;
+  const uint64_t d = uint64_t(P.C / P.heads);
+  const uint32_t bw = D < 64 ? D : 64;
   for (int i = 0; i < 2; ++i) {
-    int rc = encode_tmap_2d(&maps.qk[i], P.qk[i], uint64_t(P.ld), rows, uint64_t(P.ld) * 2, D < 64 ? D : 64, kQT);
+    int rc;
+    if (PAD) {
+      const uint64_t dims[3] = {d, uint64_t(P.ld / d), rows};       // (head column, projection * heads + head, token)
+      rc = encode_tmap_3d(&maps.qk[i], P.qk[i], dims, d * 2, uint64_t(P.ld) * 2, {bw, 1u, uint32_t(kQT)});
+      if (!rc) rc = encode_tmap_3d(&maps.kv[i], P.qk[i], dims, d * 2, uint64_t(P.ld) * 2, {bw, 1u, uint32_t(kKV)});
+      if (!rc && !VF) {
+        const uint64_t vdims[3] = {rows, d, uint64_t(P.heads)};       // (token, head row, head)
+        rc = encode_tmap_3d(&maps.vt[i], P.vt[i], vdims, rows * 2, rows * 2 * d, {64u, uint32_t(D), 1u});
+      }
+      if (rc) return rc;
+      continue;
+    }
+    rc = encode_tmap_2d(&maps.qk[i], P.qk[i], uint64_t(P.ld), rows, uint64_t(P.ld) * 2, bw, kQT);
     if (rc) return rc;
-    rc = encode_tmap_2d(&maps.kv[i], P.qk[i], uint64_t(P.ld), rows, uint64_t(P.ld) * 2, D < 64 ? D : 64, kKV);
+    rc = encode_tmap_2d(&maps.kv[i], P.qk[i], uint64_t(P.ld), rows, uint64_t(P.ld) * 2, bw, kKV);
     if (rc) return rc;
     if (!VF) {
       rc = encode_tmap_2d(&maps.vt[i], P.vt[i], rows, uint64_t(P.C), rows * 2, 64, D);
@@ -320,18 +352,24 @@ static int launch_attn_tma(const AttnParams& P, cudaStream_t st) {
     }
   }
   dim3 grid((P.n_pad + kQT - 1) / kQT, P.B * P.heads, 2);
-  launch_k(cross_attn_tma_kernel<D, VF, TRAIN>, dim3(grid), dim3(288), L::kTotal, st, P, maps);
+  launch_k(cross_attn_tma_kernel<D, VF, TRAIN, PAD>, dim3(grid), dim3(288), L::kTotal, st, P, maps);
   return check_launch("cross_attention");
 }
 
-template <bool VF>
+// Head dims 16 / 32 / 64 / 128 run their own width; every other multiple of 8 runs the next one up, padded.
+template <bool VF, bool TRAIN = false>
 static int dispatch_attn(const AttnParams& P, cudaStream_t st) {
-  switch (P.C / P.heads) {
-    case 16: return launch_attn_tma<16, VF>(P, st);
-    case 32: return launch_attn_tma<32, VF>(P, st);
-    case 64: return launch_attn_tma<64, VF>(P, st);
-    default: return launch_attn_tma<128, VF>(P, st);
+  const int d = P.C / P.heads;
+  switch (d) {
+    case 16: return launch_attn_tma<16, VF, TRAIN>(P, st);
+    case 32: return launch_attn_tma<32, VF, TRAIN>(P, st);
+    case 64: return launch_attn_tma<64, VF, TRAIN>(P, st);
+    case 128: return launch_attn_tma<128, VF, TRAIN>(P, st);
   }
+  if (d < 16) return launch_attn_tma<16, VF, TRAIN, true>(P, st);
+  if (d < 32) return launch_attn_tma<32, VF, TRAIN, true>(P, st);
+  if (d < 64) return launch_attn_tma<64, VF, TRAIN, true>(P, st);
+  return launch_attn_tma<128, VF, TRAIN, true>(P, st);
 }
 
 }  // namespace icaf
@@ -360,13 +398,7 @@ extern "C" int icaf_cross_attention_train(const void* qkv_vis, const void* qkv_i
     return set_error(ICAF_ERR_BAD_ARG, "cross_attention_train: TMA needs 16-byte aligned tensors and row pitches");
   P.p_drop = p_drop; P.seed = seed; P.seed_off = seed_offset_ptr();
   cudaStream_t st = (cudaStream_t)stream;
-  if (p_drop == 0.f) return dispatch_attn<true>(P, st);
-  switch (C / heads) {
-    case 16: return launch_attn_tma<16, true, true>(P, st);
-    case 32: return launch_attn_tma<32, true, true>(P, st);
-    case 64: return launch_attn_tma<64, true, true>(P, st);
-    default: return launch_attn_tma<128, true, true>(P, st);
-  }
+  return p_drop == 0.f ? dispatch_attn<true>(P, st) : dispatch_attn<true, true>(P, st);
 }
 
 extern "C" int icaf_cross_attention_simt(const void* qk_vis, const void* qk_ir, const void* vt_vis, const void* vt_ir,

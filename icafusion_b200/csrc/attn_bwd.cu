@@ -457,10 +457,11 @@ extern "C" int icaf_cross_attention_bwd(const void* qkv_vis, const void* qkv_ir,
   P.scale = 1.0f / sqrtf(float(d)); P.scale_log2 = 1.4426950408889634f * P.scale; P.p_drop = p_drop; P.seed = seed; P.seed_off = seed_offset_ptr();
   cudaStream_t st = (cudaStream_t)stream;
   switch (d) {
+    case 8: return launch_attn_bwd_reg<8>(P, st);        // yolov5n's P3 block
     case 16: return launch_attn_bwd_reg<16>(P, st);
     case 32: return launch_attn_bwd_reg<32>(P, st);
     case 64: return launch_attn_bwd_reg<64>(P, st);
     case 128: return launch_attn_bwd<128>(P, st);
-    default: return set_error(ICAF_ERR_UNSUPPORTED, "cross_attention_bwd: head dim must be 16/32/64/128");
+    default: return set_error(ICAF_ERR_UNSUPPORTED, "cross_attention_bwd: head dim must be 8/16/32/64/128");
   }
 }

@@ -67,6 +67,10 @@ inline int configure_smem(K kernel, int bytes, bool (&done)[kMaxDevices], const 
 // 2D: [rows][inner] with a row pitch in bytes; box = box_rows x box_inner (box_inner = 64 / 32 / 16 halfs -> 128B / 64B / 32B swizzle).
 int encode_tmap_2d(CUtensorMap* out, const void* base, uint64_t inner, uint64_t rows, uint64_t row_pitch_bytes,
                    uint32_t box_inner, uint32_t box_rows);
+// 3D: dims (d0, d1, d2) with d1 / d2 pitches in bytes; box = (box0, box1, box2), box0 = 64 / 32 / 16 halfs as in 2D.  Boxes may
+// overhang any dimension (the attention kernel reads a head of d columns as a padded box of up to 2d: the rest is zero-filled).
+int encode_tmap_3d(CUtensorMap* out, const void* base, const uint64_t (&dims)[3], uint64_t pitch1_bytes, uint64_t pitch2_bytes,
+                   const uint32_t (&box)[3]);
 // 4D NHWC activation view (C, W, H, B) with pixel pitch `ld` elements; box = (box_c, box_w, box_h, 1) *input* elements,
 // traversal strides (1, sw, sh, 1): loads ceil(box_w/sw) x ceil(box_h/sh) pixels per box.
 int encode_tmap_nhwc(CUtensorMap* out, const void* base, int C, int W, int H, int B, int64_t ld, uint32_t box_c,

@@ -442,7 +442,7 @@ def cross_attention(qk_vis, qk_ir, vt_vis, vt_ir, B: int, N: int, n_pad: int, Cc
         raise ValueError(f"cross_attention: projection tensors must be {want}, got {tuple(qk_vis.shape)}")
     _call("icaf_cross_attention_simt" if simt else "icaf_cross_attention", fn,
           (_ptr(qk_vis), _ptr(qk_ir), _ptr(vt_vis), _ptr(vt_ir), _ptr(out_v), _ptr(out_i), B, N, n_pad, Cc, heads),
-          {"flops": 8.0 * B * N * N * Cc, "bytes": 2.0 * 2 * (3 * B * n_pad * Cc + B * n_pad * Cc)})
+          {"flops": 8.0 * B * N * N * Cc, "bytes": 2.0 * 2 * (3 * B * n_pad * Cc + B * n_pad * Cc), "N": N, "d": Cc // heads})
     return out_v, out_i
 
 
