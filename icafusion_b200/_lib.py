@@ -40,6 +40,16 @@ class LossHyp(C.Structure):
                [("balance", C.c_float * 5)]
 
 
+class AugTile(C.Structure):
+    _fields_ = [("rgb", C.c_void_p), ("ir", C.c_void_p)] + \
+               [(n, C.c_int) for n in ("H0", "W0", "h", "w", "x1a", "y1a", "x2a", "y2a", "x1b", "y1b", "xtab", "ytab")]
+
+
+class AugSample(C.Structure):
+    _fields_ = [("tile", AugTile * 4)] + [(n, C.c_int) for n in ("ntiles", "canvas", "warp", "flipud", "fliplr", "reserved")] + \
+               [("lut", C.c_uint8 * (2 * 3 * 256))]
+
+
 KERNEL_TC = 0
 
 _vp, _i, _i64, _f = C.c_void_p, C.c_int, C.c_int64, C.c_float
@@ -94,6 +104,8 @@ SIGNATURES = {
     "icaf_cross_attention_bwd": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _f, C.c_uint32, _vp, C.c_size_t, _vp],
     "icaf_axpby": [_vp, _vp, _vp, _vp, _vp, _i64, _vp],
     "icaf_detect_decode": [_vp, _i64, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _f, C.POINTER(C.c_float), _vp],
+    "icaf_augment_params_bytes": [_i, _i, _i],
+    "icaf_augment": [_vp, C.c_size_t, _i, _i, _i, _vp, _vp, _vp],
 }
 
 _lib = None
@@ -117,7 +129,8 @@ def lib() -> C.CDLL:
             fn.restype = {"icaf_last_error": C.c_char_p, "icaf_kernel_launches": C.c_longlong,
                           "icaf_nms_workspace_bytes": C.c_size_t, "icaf_loss_workspace_bytes": C.c_size_t,
                           "icaf_conv2d_wgrad_workspace_bytes": C.c_size_t, "icaf_train_workspace_bytes": C.c_size_t,
-                          "icaf_cross_attention_bwd_workspace_bytes": C.c_size_t}.get(name, C.c_int)
+                          "icaf_cross_attention_bwd_workspace_bytes": C.c_size_t,
+                          "icaf_augment_params_bytes": C.c_size_t}.get(name, C.c_int)
         _lib = L
     return _lib
 

@@ -348,6 +348,45 @@ int icaf_cross_attention_bwd(const void* qkv_vis, const void* qkv_ir, const void
  * LearnableCoefficient.forward / LearnableWeights.forward called stand-alone (models/common.py:569-587). */
 int icaf_axpby(const void* x, const void* y, const float* a, const float* b, void* out, int64_t n, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Training augmentation of RGB/IR pairs: LoadMultiModalImagesAndLabels.__getitem__ (utils/datasets.py:948-1024) with
+ * augment=True -- mosaic (load_mosaic_RGB_IR :1208-1309, resize of load_image_rgb_ir :1097-1125), affine warp
+ * (random_perspective_rgb_ir :1535-1630, perspective = 0), HSV jitter (augment_hsv :1129-1141), flipud / fliplr and
+ * BGR->RGB + HWC->CHW -- for a batch, one launch, bit-exact against the cv2 pipeline.  The random draws, the warp tables
+ * and the LUTs are the host's (icafusion_b200/augment.py); the canvas is never materialised: every output pixel is
+ * evaluated through warp -> canvas tile -> cv2.resize taps of the decoded frame -> HSV LUTs.
+ * ------------------------------------------------------------------------------------------- */
+typedef struct {
+  const void* rgb; const void* ir;  /* device uint8 (H0, W0, 3) BGR frames of this tile's image                       */
+  int H0, W0;                       /* decoded size                                                                    */
+  int h, w;                         /* load_image size (int(h0 r), int(w0 r)); == (H0, W0): no resize                  */
+  int x1a, y1a, x2a, y2a;           /* canvas rectangle [x1a, x2a) x [y1a, y2a) ...                                     */
+  int x1b, y1b;                     /* ... filled from the resized image starting at (x1b, y1b)                         */
+  int xtab, ytab;                   /* first row (int4 units) of the cv2.resize taps in the taps region: [w] / [h] rows */
+} icaf_aug_tile;
+
+typedef struct {
+  icaf_aug_tile tile[4];
+  int ntiles;                       /* 1..4; a later tile covers an earlier one where they overlap (placement order)   */
+  int canvas;                       /* side of the square canvas: 2s with the mosaic, s without                         */
+  int warp;                         /* 1: output = warpAffine(canvas) via the sample's tables; 0: output = canvas      */
+  int flipud, fliplr;
+  int reserved;
+  unsigned char lut[2][3][256];     /* augment_hsv LUTs: [rgb, ir][hue, sat, val]                                        */
+} icaf_aug_sample;
+
+/* Bytes of the parameter block for B samples at output size s with n_taps resize-tap rows.  Layout (16-byte aligned regions):
+ *   icaf_aug_sample [B]                       at 0
+ *   int32 warp [B][4][s]                      at align16(B * sizeof(icaf_aug_sample)): per sample adelta[x], bdelta[x]
+ *                                             (cvRound(M'0 x 1024), cvRound(M'3 x 1024)) and X0[y], Y0[y]
+ *                                             (cvRound((M'1 y + M'2) 1024) + 16, likewise) of the inverted matrix M'
+ *   int32 taps [n_taps][4]                    after the warp tables: {i0, i1, w0, w1} rows as for icaf_letterbox
+ * 0 for a bad argument. */
+size_t icaf_augment_params_bytes(int B, int s, int n_taps);
+
+/* params: device block laid out as above (16-byte aligned); rgb_out / ir_out: uint8 (B, 3, s, s) RGB planar. */
+int icaf_augment(const void* params, size_t params_bytes, int B, int s, int n_taps, void* rgb_out, void* ir_out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
