@@ -1,5 +1,5 @@
 // Shared pieces of the implicit-GEMM conv kernels (conv_gemm.cu): problem descriptors, TMA descriptor bundle, tile origin,
-// and the epilogue (staged-row load, chunk dispatch).
+// and the epilogues (staged rows: load, chunk dispatch; accumulator registers: fragments into a TMA-stored output tile).
 #pragma once
 #include "icaf_internal.cuh"
 
@@ -32,11 +32,12 @@ struct ConvParams {
   int ln_parts;                           // LN fold: partials per input row (0 = no fold)
   float ln_eps, ln_inv_k;                 // LN fold: epsilon, 1 / (normalised features = K)
   int m_tiles, n_tiles, tiles;            // persistent kernel: tile grid (m, n, problem) and its product
+  int tma_epi;                            // one-tile kernel: register epilogue + TMA-stored output tile (else staged rows)
 };
 struct ConvMaps {          // TMA descriptors, passed by value as a __grid_constant__ kernel parameter
   CUtensorMap w[2];
   CUtensorMap a[2];
-  CUtensorMap y[2];        // persistent kernel, fragment epilogue: output (and residual) tiles, 64-column boxes
+  CUtensorMap y[2];        // register epilogue (both kernels): output (and residual) tiles, 64-column boxes
   CUtensorMap res[2];
 };
 
@@ -65,6 +66,18 @@ __device__ __forceinline__ void tile_origin(const ConvParams& P, int mtile, int&
     const int t = mtile - tb * per_img;
     oy0 = (t / P.tiles_x) * P.th;
     ox0 = (t % P.tiles_x) * P.tw;
+  }
+}
+
+// Tile row -> output row m; valid: inside the output (4-D: tw divides Wo; the last tile row of an image may hang over).
+__device__ __forceinline__ void tile_row(const ConvParams& P, const TileOrigin& o, int row, int& m, bool& valid) {
+  if (P.a_mode == A_TMA4D) {
+    const int ry = row / P.tw, rx = row - ry * P.tw;
+    m = (o.tb * P.Ho + o.oy0 + ry) * P.Wo + o.ox0 + rx;
+    valid = ry < P.th && o.oy0 + ry < P.Ho;
+  } else {
+    m = o.m0 + row;
+    valid = m < P.M;
   }
 }
 
@@ -199,6 +212,88 @@ __device__ __forceinline__ void epi_dispatch(int mode_act, const uint32_t (&acc)
       case 7: epi_chunk<2, 1>(acc, sb, rbias, alpha, beta, rp, yp, vec, ncols, ex, cb); break;
       default: epi_chunk<2, 2>(acc, sb, rbias, alpha, beta, rp, yp, vec, ncols, ex, cb); break;
     }
+  }
+}
+
+// ---------------------------------------------------------------------------------------------------
+// Epilogue on the accumulator registers of a consumer warpgroup (tile rows 0-63 in acc0, 64-127 in acc1, NA = BN / 2 each),
+// written as fp16 into an output tile of 64-column halves: 128 rows of 128 bytes each, 128B-swizzled (the layout of a TMA
+// box of 64 columns x 128 rows, or of tw x th pixels), the halves kOutHalfBytes apart.  One thread then stores each half
+// with a TMA store, which clips the rows and columns outside the output.
+constexpr int kOutHalfBytes = BM * 64 * 2;
+
+// columns [16 PP, 16 PP + 16) of the warpgroup's accumulators: v[0..7] from rows 0-63 (acc0), v[8..15] from rows 64-127
+template <int PP, int NA>
+__device__ __forceinline__ void take_cols16(const float (&acc0)[NA], const float (&acc1)[NA], float (&v)[16]) {
+  constexpr int Q = PP < NA / 8 ? PP : NA / 8 - 1;   // the groups past a narrow tile are never taken
+#pragma unroll
+  for (int e = 0; e < 8; ++e) { v[e] = acc0[8 * Q + e]; v[8 + e] = acc1[8 * Q + e]; }
+}
+
+// Epilogue of 16 columns (take_cols16) on the accumulator registers: epi_value per element, fp16 pairs into the output
+// tile with stmatrix.  Register pair k of v[8h ...] is tile row 16w + l/4 + 8 (k % 2) + 64h, columns 8 (k / 2) + 2 (l % 4)
+// (+0, +1) of the 16: exactly one register of matrix k of an m8n8.x4 stmatrix.  sa: this lane's stmatrix row address for
+// rows 0-63 (rows 64-127 are 8 KB further); RES != 0 reads the residual pairs from the same place with ldmatrix first.
+// sb: column bias at the lane's column 2 (l % 4); rb: row bias of the lane's rows l/4 + {0, 8, 64, 72}.
+template <int ACT, int RES>
+__device__ __forceinline__ void epi_fragments(const float (&v)[16], uint32_t sa, const float* sb, const float (&rb)[4],
+                                              float alpha, float beta) {
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    uint32_t r[4];
+    if (RES != 0) ldmatrix_x4(r, sa + 8192u * h);
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const float2 b = *reinterpret_cast<const float2*>(sb + 8 * (k >> 1));
+      const float rbias = rb[2 * h + (k & 1)];
+      float2 rf = make_float2(0.f, 0.f);
+      if (RES != 0) rf = __half22float2(*reinterpret_cast<const __half2*>(&r[k]));
+      r[k] = pack_half2(epi_value<ACT, RES>(v[8 * h + 2 * k], b.x, rbias, rf.x, alpha, beta),
+                        epi_value<ACT, RES>(v[8 * h + 2 * k + 1], b.y, rbias, rf.y, alpha, beta));
+    }
+    stmatrix_x4(sa + 8192u * h, r);
+  }
+}
+
+// mode_act = 3 * ACT + RES, warp-uniform: dispatched once per 16 columns to straight-line code
+__device__ __forceinline__ void epi_fragments_dispatch(int mode_act, const float (&v)[16], uint32_t sa, const float* sb,
+                                                       const float (&rb)[4], float alpha, float beta) {
+  switch (mode_act) {
+    case 0: epi_fragments<0, 0>(v, sa, sb, rb, alpha, beta); break;
+    case 1: epi_fragments<0, 1>(v, sa, sb, rb, alpha, beta); break;
+    case 2: epi_fragments<0, 2>(v, sa, sb, rb, alpha, beta); break;
+    case 3: epi_fragments<1, 0>(v, sa, sb, rb, alpha, beta); break;
+    case 4: epi_fragments<1, 1>(v, sa, sb, rb, alpha, beta); break;
+    case 5: epi_fragments<1, 2>(v, sa, sb, rb, alpha, beta); break;
+    case 6: epi_fragments<2, 0>(v, sa, sb, rb, alpha, beta); break;
+    case 7: epi_fragments<2, 1>(v, sa, sb, rb, alpha, beta); break;
+    default: epi_fragments<2, 2>(v, sa, sb, rb, alpha, beta); break;
+  }
+}
+
+// The whole tile, 16 columns at a time: sout = the output tile (1024-byte aligned), sbias = the tile's column bias,
+// w / l = warp of the warpgroup / lane.
+template <int NA>
+__device__ __forceinline__ void epi_tile_fragments(int mode_act, const float (&acc0)[NA], const float (&acc1)[NA], uint32_t sout,
+                                                   const float* sbias, const float (&rb)[4], float alpha, float beta, int w, int l) {
+  const uint32_t sa = sout + uint32_t(16 * w + (l & 7) + 8 * ((l >> 3) & 1)) * 128u;   // stmatrix row of this lane
+  const float* sb = sbias + 2 * (l & 3);
+#pragma unroll 1
+  for (int p = 0; p < NA / 8; ++p) {
+    float v[16];
+    switch (p) {
+      case 0: take_cols16<0>(acc0, acc1, v); break;
+      case 1: take_cols16<1>(acc0, acc1, v); break;
+      case 2: take_cols16<2>(acc0, acc1, v); break;
+      case 3: take_cols16<3>(acc0, acc1, v); break;
+      case 4: take_cols16<4>(acc0, acc1, v); break;
+      case 5: take_cols16<5>(acc0, acc1, v); break;
+      case 6: take_cols16<6>(acc0, acc1, v); break;
+      default: take_cols16<7>(acc0, acc1, v); break;
+    }
+    // half p / 4 of the tile; 16-byte chunk 2 (p % 4) + l / 16 of the 128-byte row, 128B-swizzled by the row
+    const uint32_t a = sa + uint32_t(p >> 2) * uint32_t(kOutHalfBytes) + (uint32_t((2 * (p & 3) + (l >> 4)) ^ (l & 7)) << 4);
+    epi_fragments_dispatch(mode_act, v, a, sb + 16 * p, rb, alpha, beta);
   }
 }
 

@@ -12,18 +12,21 @@
 //              with cp.async (zero-fill), 4 rows x 128 B per warp instruction.
 // The filter tile (BN rows x 64 K) always arrives by 2-D TMA.
 // conv_gemm_tc_kernel: CTA = one 128 x BN output tile (BN = 32 / 64 / 128), 288 threads:
-//   warps 0-3 : A_GATHER producers, then the epilogue (thread t owns output row t)
-//   warps 4-7 : one consumer warpgroup: two m64nBNk16 wgmma per 16 K (rows 0-63, 64-127), accumulators in registers,
-//               written to shared memory (the idle ring) once the K loop is done
-//   warp  8   : TMA producer (one elected thread)
+//   warps 0-3 : A_GATHER producers, then (staged-row epilogue) the epilogue: thread t owns output row t
+//   warps 4-7 : one consumer warpgroup: two m64nBNk16 wgmma per 16 K (rows 0-63, 64-127), accumulators in registers;
+//               then either the register epilogue (as in the persistent kernel) into an idle ring stage and a TMA store,
+//               or the accumulators as fp32 rows into the idle ring for warps 0-3
+//   warp  8   : TMA producer (one elected thread); with the register epilogue also the residual tile's TMA load
 // Pipelines: smem ring full[]/empty[] (producers <-> consumer), named barrier (staged accumulator -> epilogue).  Small
 // tiles (BN <= 64) let two CTAs share an SM so that one CTA's epilogue overlaps the other's main loop.  Split-K: the
 // CTAs of a cluster take a K range each; the leader adds the others' staged tiles through distributed shared memory.
+// The register epilogue serves BN >= 64 launches that are not XM or split-K and whose output TMA can write; the others
+// keep the staged rows.
 // conv_gemm_persist_kernel: BN = 128 grids of more than one wave with TMA-staged A -- one persistent CTA per SM, a TMA
 // producer warpgroup and two consumer warpgroups that take turns on the main loop; each consumer runs the epilogue on its
 // accumulator registers and writes the tile with TMA stores (see its own comment below).
-// The two kernels share the TMA producer stage (load_stage), the main loop (mma_loop), the tile origin and the
-// per-element epilogue expression (epi_value), so they compute bit-identical tiles.
+// The two kernels share the TMA producer stage (load_stage), the main loop (mma_loop), the tile origin, the register
+// epilogue (epi_tile_fragments) and the per-element epilogue expression (epi_value), so they compute bit-identical tiles.
 #include <cstdlib>
 #include <cstring>
 
@@ -70,14 +73,15 @@ __device__ __forceinline__ void load_stage(const ConvParams& P, int a_mode, uint
 // Consumer warpgroup main loop over the tile's nkb K blocks, from ring stage s0 at phase ph0: per stage, wait for it to
 // fill, issue two m64nBNk16 wgmma per 16 K (tile rows 0-63 into acc0, 64-127 into acc1), then hand back the previous
 // stage, whose MMAs are done once this stage's are the only ones in flight.  Returns the last stage, which is still in
-// use until the caller's final wgmma_wait.  kQuiet: wait without the printf report (see mbar_wait_quiet).
-template <int BN, bool kQuiet, class FullBar, class HandBack>
+// use until the caller's final wgmma_wait.  It waits without the printf report (see mbar_wait_quiet), and so do the
+// producers of both kernels: a printf reachable anywhere in the kernel makes ptxas serialise every wgmma (warning C7510).
+template <int BN, class FullBar, class HandBack>
 __device__ __forceinline__ int mma_loop(float (&acc0)[BN / 2], float (&acc1)[BN / 2], uint32_t smem_base, int kStages, int nkb,
                                         int s0, uint32_t ph0, FullBar full_bar, HandBack hand_back) {
   int s = s0, s_prev = s0;
   uint32_t ph = ph0;
   for (int kb = 0; kb < nkb; ++kb) {
-    if (kQuiet) mbar_wait_quiet(full_bar(s), ph); else mbar_wait(full_bar(s), ph);
+    mbar_wait_quiet(full_bar(s), ph);
     const uint32_t sa = smem_base + s * SmemLayout<BN>::kStageBytes;
     wgmma_fence();
 #pragma unroll
@@ -94,6 +98,15 @@ __device__ __forceinline__ int mma_loop(float (&acc0)[BN / 2], float (&acc1)[BN 
   }
   return s_prev;
 }
+
+// Register budget of the BN <= 64 instantiations (two CTAs per SM: 96 registers per thread at launch).  Warps 0-3 give
+// some to the consumer warpgroup, whose epilogue runs on its accumulators; warp 8 (not a whole warpgroup) keeps the launch
+// count, so the CTA's total stays 288 x 96.  BN = 64 XM keeps 96 everywhere: its consumer only stages rows, and the row
+// epilogue of warps 0-3 needs them.  (ptxas -v: no spills in any instantiation with this split.)
+constexpr int kRegsLow = 80, kRegsHigh = 112;
+static_assert(128 * kRegsLow + 128 * kRegsHigh + 32 * 96 <= kThreads * 96, "register rebalance exceeds the launch budget");
+template <int BN, bool XM>
+__host__ __device__ constexpr bool rebalance_regs() { return BN == 32 || (BN == 64 && !XM); }
 
 // XM: the LayerNorm-fold / row-statistics epilogues (DMFF linears) live in their own instantiation so that the epilogue
 // of every other layer stays small (the hot loops are instruction-cache sensitive).
@@ -127,6 +140,14 @@ conv_gemm_tc_kernel(const ConvParams P, const __grid_constant__ ConvMaps maps) {
   int m0, tb, oy0, ox0;
   tile_origin(P, mtile, m0, tb, oy0, ox0);
   const TileOrigin o{m0, tb, oy0, ox0};
+  // Register epilogue (host: not XM, no split-K, output writable by TMA, BN >= 64): the consumer warpgroup applies the
+  // epilogue to its accumulators and stores the tile by TMA from ring stage s_out -- the stage the K block after the last
+  // one would take.  It is free once block nkb - stages has been consumed, so a residual tile is TMA-loaded into it (on
+  // res_bar) while the last blocks of the main loop still run.
+  const bool tma_epi = !XM && BN >= 64 && P.tma_epi != 0;
+  const bool has_res = (P.epi & (ICAF_EPI_ADD_RES | ICAF_EPI_SCALED_RES)) != 0;
+  const int s_out = nkb % kStages;
+  const uint32_t res_bar = bar_base + 8u * (2 * kMaxStages);
 
   if (tid == 0) {
     const uint32_t nfull = a_mode == A_GATHER ? 129u : 1u;    // 128 gather threads + the TMA thread
@@ -134,11 +155,16 @@ conv_gemm_tc_kernel(const ConvParams P, const __grid_constant__ ConvMaps maps) {
       mbar_init(full_bar(s), nfull);
       mbar_init(empty_bar(s), 4);                             // one arrival per consumer warp
     }
+    mbar_init(res_bar, 1);
     fence_mbar_init();
   }
   if (warp == 8 && lane_id() == 0) {
     tma_prefetch_desc(bz ? &maps.w[1] : &maps.w[0]);
     if (a_mode != A_GATHER) tma_prefetch_desc(bz ? &maps.a[1] : &maps.a[0]);
+    if (tma_epi) {
+      tma_prefetch_desc(bz ? &maps.y[1] : &maps.y[0]);
+      if (has_res) tma_prefetch_desc(bz ? &maps.res[1] : &maps.res[0]);
+    }
   }
   float* sbias = reinterpret_cast<float*>(smem_gen + bar_off + 256);
   float* sacc = reinterpret_cast<float*>(smem_gen);           // staged accumulator [BM][kPitch], reuses the idle ring
@@ -146,16 +172,17 @@ conv_gemm_tc_kernel(const ConvParams P, const __grid_constant__ ConvMaps maps) {
   pdl_wait();   // prologue (barriers, descriptor prefetch) overlapped the previous kernel
 
   if (warp < 4) {
+    if constexpr (rebalance_regs<BN, XM>()) setmaxnreg_dec<kRegsLow>();
     // Epilogue operands that do not depend on the main loop are fetched now so their DRAM latency hides behind it:
     // bias slice and (alpha, beta) into registers, this thread's residual row into L2.
     float bias_r[(BN + 127) / 128];
 #pragma unroll
     for (int i = 0; i < (BN + 127) / 128; ++i) {
       const int col = tid + 128 * i;
-      bias_r[i] = (col < BN && pr.bias && !(P.epi & ICAF_EPI_BIAS_ROW) && n0 + col < P.N) ? __ldg(pr.bias + n0 + col) : 0.f;
+      bias_r[i] = (!tma_epi && col < BN && pr.bias && !(P.epi & ICAF_EPI_BIAS_ROW) && n0 + col < P.N) ? __ldg(pr.bias + n0 + col) : 0.f;
     }
     float alpha = 0.f, beta = 1.f;
-    if (P.epi & ICAF_EPI_SCALED_RES) { alpha = __ldg(pr.alpha); beta = __ldg(pr.beta); }
+    if (!tma_epi && (P.epi & ICAF_EPI_SCALED_RES)) { alpha = __ldg(pr.alpha); beta = __ldg(pr.beta); }
     if (a_mode == A_GATHER) {
       // ---------------------------------------------------------------- cp.async gather producers
       // A stage is handed over once this thread's copies of it have landed and been made visible to the async proxy
@@ -183,7 +210,7 @@ conv_gemm_tc_kernel(const ConvParams P, const __grid_constant__ ConvMaps maps) {
       int s = 0, s_done = 0;
       uint32_t ph = 0;
       for (int kb = 0; kb < nkb; ++kb) {
-        mbar_wait(empty_bar(s), ph ^ 1);
+        mbar_wait_quiet(empty_bar(s), ph ^ 1);
         const uint32_t sa = smem_base + s * L::kStageBytes;
         const int k0 = (kb_begin + kb) * BK + c * 8;
         const bool kvalid = k0 < P.K;
@@ -214,6 +241,7 @@ conv_gemm_tc_kernel(const ConvParams P, const __grid_constant__ ConvMaps maps) {
         if (++s_done == kStages) s_done = 0;
       }
     }
+    if (tma_epi) return;                   // the consumer warpgroup runs the epilogue
 
     // ------------------------------------------------------------------ epilogue
     const int row = tid;                   // staged accumulator row == tile row
@@ -283,14 +311,55 @@ conv_gemm_tc_kernel(const ConvParams P, const __grid_constant__ ConvMaps maps) {
     if (splits > 1) { cluster_arrive(); cluster_wait(); }   // the peers' staged tiles stay alive until the leader has read them
   } else if (warp < 8) {
     // ------------------------------------------------------------------ consumer warpgroup (wgmma)
+    if constexpr (rebalance_regs<BN, XM>()) setmaxnreg_inc<kRegsHigh>();
+    const int t = tid - 128, w = t >> 5, l = t & 31;
+    float alpha = 0.f, beta = 1.f;
+    float rb[4] = {0.f, 0.f, 0.f, 0.f};      // tma_epi: row bias of this lane's accumulator rows l/4 + {0, 8, 64, 72}
+    if (tma_epi) {
+      // epilogue operands that do not depend on the main loop: bias slice, (alpha, beta), row bias
+      if (t < BN) sbias[t] = (pr.bias && !(P.epi & ICAF_EPI_BIAS_ROW) && n0 + t < P.N) ? __ldg(pr.bias + n0 + t) : 0.f;
+      if (P.epi & ICAF_EPI_SCALED_RES) { alpha = __ldg(pr.alpha); beta = __ldg(pr.beta); }
+      if ((P.epi & ICAF_EPI_BIAS_ROW) && pr.bias) {
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+          int mq;
+          bool vq;
+          tile_row(P, o, 16 * w + (l >> 2) + 8 * (q & 1) + 64 * (q >> 1), mq, vq);
+          rb[q] = vq ? __ldg(pr.bias + mq) : 0.f;
+        }
+      }
+      named_bar_sync(2, 128);                                 // bias slice complete
+    }
     float acc0[BN / 2], acc1[BN / 2];
 #pragma unroll
     for (int i = 0; i < BN / 2; ++i) { acc0[i] = 0.f; acc1[i] = 0.f; }
-    mma_loop<BN, false>(acc0, acc1, smem_base, kStages, nkb, 0, 0u, full_bar,
-                        [&](int s) { if (lane_id() == 0) mbar_arrive(empty_bar(s)); });   // one arrival per consumer warp
+    mma_loop<BN>(acc0, acc1, smem_base, kStages, nkb, 0, 0u, full_bar,
+                 [&](int s) { if (lane_id() == 0) mbar_arrive(empty_bar(s)); });   // one arrival per consumer warp
     wgmma_wait<0>();
+    if constexpr (!XM && BN >= 64) {
+      if (tma_epi) {
+        // ---- epilogue on the accumulator registers into ring stage s_out (every stage is consumed now), TMA store
+        const uint32_t sout = smem_base + uint32_t(s_out) * L::kStageBytes;
+        if (has_res) mbar_wait_quiet(res_bar, 0);
+        const int mode = (P.epi & ICAF_EPI_SCALED_RES) ? 2 : (has_res ? 1 : 0);
+        epi_tile_fragments<BN / 2>(P.act * 3 + mode, acc0, acc1, sout, sbias, rb, alpha, beta, w, l);
+        fence_proxy_async_smem();                             // the tile is visible to the TMA unit ...
+        named_bar_sync(2, 128);                               // ... once every thread of the warpgroup has written its part
+        if (t == 0) {
+          const CUtensorMap* my = bz ? &maps.y[1] : &maps.y[0];
+          const int halves = (BN == 128 && n0 + 64 < P.N) ? 2 : 1;
+          for (int hh = 0; hh < halves; ++hh) {
+            const uint32_t src = sout + uint32_t(hh * kOutHalfBytes);
+            if (a_mode == A_TMA4D) tma_store_4d(my, src, n0 + 64 * hh, o.ox0, o.oy0, o.tb);
+            else tma_store_2d(my, src, n0 + 64 * hh, o.m0);
+          }
+          bulk_commit_group();
+          bulk_wait_group<0>();                               // complete before the grid is (PDL dependents read it)
+        }
+        return;
+      }
+    }
     // the ring is idle now (every stage consumed): stage the accumulator tile as rows for the epilogue warps
-    const int t = tid - 128, w = t >> 5, l = t & 31;
 #pragma unroll
     for (int i = 0; i < BN / 2; i += 2) {
       const int r = 16 * w + (l >> 2) + 8 * ((i >> 1) & 1), col = 8 * (i >> 2) + 2 * (l & 3);
@@ -308,9 +377,23 @@ conv_gemm_tc_kernel(const ConvParams P, const __grid_constant__ ConvMaps maps) {
       int s = 0;
       uint32_t ph = 0;
       for (int kb = 0; kb < nkb; ++kb) {
-        mbar_wait(empty_bar(s), ph ^ 1);
+        mbar_wait_quiet(empty_bar(s), ph ^ 1);
         load_stage<BN, false>(P, a_mode, smem_base + s * L::kStageBytes, full_bar(s), bytes, mw, ma, kb_begin + kb, n0, o);
         if (++s == kStages) { s = 0; ph ^= 1; }
+      }
+      if (tma_epi && has_res) {
+        // the residual tile into stage s_out (== s) once block nkb - stages has left it: 64-column boxes of 128 rows (2-D)
+        // or tw x th pixels (4-D)
+        mbar_wait_quiet(empty_bar(s), ph ^ 1);
+        const CUtensorMap* mr = bz ? &maps.res[1] : &maps.res[0];
+        const int halves = (BN == 128 && n0 + 64 < P.N) ? 2 : 1;
+        const uint32_t half_bytes = a_mode == A_TMA4D ? uint32_t(P.tw * P.th) * 128u : uint32_t(kOutHalfBytes);
+        mbar_arrive_expect_tx(res_bar, uint32_t(halves) * half_bytes);
+        for (int hh = 0; hh < halves; ++hh) {
+          const uint32_t dst = smem_base + uint32_t(s) * L::kStageBytes + uint32_t(hh * kOutHalfBytes);
+          if (a_mode == A_TMA4D) tma_load_4d(dst, mr, res_bar, n0 + 64 * hh, o.ox0, o.oy0, o.tb);
+          else tma_load_2d(dst, mr, res_bar, n0 + 64 * hh, o.m0);
+        }
       }
     }
     __syncwarp();
@@ -335,7 +418,7 @@ conv_gemm_tc_kernel(const ConvParams P, const __grid_constant__ ConvMaps maps) {
 constexpr int kPersistThreads = 384;
 struct PersistLayout {
   static constexpr int kStageBytes = SmemLayout<128>::kStageBytes;
-  static constexpr int kHalfBytes = BM * 64 * 2;               // one 64-column half of the output tile
+  static constexpr int kHalfBytes = kOutHalfBytes;             // one 64-column half of the output tile
   static constexpr int kOutBytes = 2 * kHalfBytes;             // per consumer, 1024-byte aligned (TMA 128B swizzle)
   static constexpr int kPitch = 32 + 4;                        // XM: floats per staged row of a 32-column chunk
   static constexpr int kChunkBytes = BM * kPitch * 4;
@@ -365,54 +448,6 @@ __device__ __forceinline__ void stage_chunk(const float (&acc0)[64], const float
     const int r = 16 * w + (l >> 2) + 8 * ((i >> 1) & 1), col = 8 * (i >> 2) - 32 * CC + 2 * (l & 3);
     *reinterpret_cast<float2*>(sacc + r * PersistLayout::kPitch + col) = make_float2(acc0[i], acc0[i + 1]);
     *reinterpret_cast<float2*>(sacc + (r + 64) * PersistLayout::kPitch + col) = make_float2(acc1[i], acc1[i + 1]);
-  }
-}
-
-// columns [16 PP, 16 PP + 16) of the warpgroup's accumulators: v[0..7] from rows 0-63 (acc0), v[8..15] from rows 64-127
-template <int PP>
-__device__ __forceinline__ void take_cols16(const float (&acc0)[64], const float (&acc1)[64], float (&v)[16]) {
-#pragma unroll
-  for (int e = 0; e < 8; ++e) { v[e] = acc0[8 * PP + e]; v[8 + e] = acc1[8 * PP + e]; }
-}
-
-// Epilogue of 16 columns (take_cols16) on the accumulator registers: epi_value per element, fp16 pairs into the output
-// tile with stmatrix.  Register pair k of v[8h ...] is tile row 16w + l/4 + 8 (k % 2) + 64h, columns 8 (k / 2) + 2 (l % 4)
-// (+0, +1) of the 16: exactly one register of matrix k of an m8n8.x4 stmatrix.  sa: this lane's stmatrix row address for
-// rows 0-63 (rows 64-127 are 8 KB further); RES != 0 reads the residual pairs from the same place with ldmatrix first.
-// sb: column bias at the lane's column 2 (l % 4); rb: row bias of the lane's rows l/4 + {0, 8, 64, 72}.
-template <int ACT, int RES>
-__device__ __forceinline__ void epi_fragments(const float (&v)[16], uint32_t sa, const float* sb, const float (&rb)[4],
-                                              float alpha, float beta) {
-#pragma unroll
-  for (int h = 0; h < 2; ++h) {
-    uint32_t r[4];
-    if (RES != 0) ldmatrix_x4(r, sa + 8192u * h);
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      const float2 b = *reinterpret_cast<const float2*>(sb + 8 * (k >> 1));
-      const float rbias = rb[2 * h + (k & 1)];
-      float2 rf = make_float2(0.f, 0.f);
-      if (RES != 0) rf = __half22float2(*reinterpret_cast<const __half2*>(&r[k]));
-      r[k] = pack_half2(epi_value<ACT, RES>(v[8 * h + 2 * k], b.x, rbias, rf.x, alpha, beta),
-                        epi_value<ACT, RES>(v[8 * h + 2 * k + 1], b.y, rbias, rf.y, alpha, beta));
-    }
-    stmatrix_x4(sa + 8192u * h, r);
-  }
-}
-
-// mode_act = 3 * ACT + RES, warp-uniform: dispatched once per 16 columns to straight-line code
-__device__ __forceinline__ void epi_fragments_dispatch(int mode_act, const float (&v)[16], uint32_t sa, const float* sb,
-                                                       const float (&rb)[4], float alpha, float beta) {
-  switch (mode_act) {
-    case 0: epi_fragments<0, 0>(v, sa, sb, rb, alpha, beta); break;
-    case 1: epi_fragments<0, 1>(v, sa, sb, rb, alpha, beta); break;
-    case 2: epi_fragments<0, 2>(v, sa, sb, rb, alpha, beta); break;
-    case 3: epi_fragments<1, 0>(v, sa, sb, rb, alpha, beta); break;
-    case 4: epi_fragments<1, 1>(v, sa, sb, rb, alpha, beta); break;
-    case 5: epi_fragments<1, 2>(v, sa, sb, rb, alpha, beta); break;
-    case 6: epi_fragments<2, 0>(v, sa, sb, rb, alpha, beta); break;
-    case 7: epi_fragments<2, 1>(v, sa, sb, rb, alpha, beta); break;
-    default: epi_fragments<2, 2>(v, sa, sb, rb, alpha, beta); break;
   }
 }
 
@@ -500,17 +535,6 @@ conv_gemm_persist_kernel(const ConvParams P, const __grid_constant__ ConvMaps ma
     const int n0 = pt.n0;
     const TileOrigin& o = pt.o;
     const int halves = n0 + 64 < P.N ? 2 : 1;                 // 64-column halves of the tile inside the output
-    // tile row -> output row m; valid: inside the map (4-D: tw divides Wo; the last tile row of an image may hang over)
-    auto out_row = [&](int row, int& m, bool& valid) {
-      if (a_mode == A_TMA4D) {
-        const int ry = row / P.tw, rx = row - ry * P.tw;
-        m = (o.tb * P.Ho + o.oy0 + ry) * P.Wo + o.ox0 + rx;
-        valid = ry < P.th && o.oy0 + ry < P.Ho;
-      } else {
-        m = o.m0 + row;
-        valid = m < P.M;
-      }
-    };
     // Epilogue operands that do not depend on the main loop are fetched now so their DRAM latency hides behind it:
     // bias slice and (alpha, beta) into registers; XM: this thread's residual row into L2; otherwise the residual tile.
     const float bias_r = (pr.bias && !(P.epi & ICAF_EPI_BIAS_ROW) && n0 + t < P.N) ? __ldg(pr.bias + n0 + t) : 0.f;
@@ -519,7 +543,7 @@ conv_gemm_persist_kernel(const ConvParams P, const __grid_constant__ ConvMaps ma
     const int row = t;
     int m;
     bool mvalid;
-    out_row(row, m, mvalid);
+    tile_row(P, o, row, m, mvalid);
     const float rbias = ((P.epi & ICAF_EPI_BIAS_ROW) && pr.bias && mvalid) ? __ldg(pr.bias + m) : 0.f;
     __half* yrow = pr.y + size_t(mvalid ? m : 0) * pr.y_ld;
     const __half* rrow = pr.res ? pr.res + size_t(mvalid ? m : 0) * pr.res_ld : nullptr;
@@ -539,7 +563,7 @@ conv_gemm_persist_kernel(const ConvParams P, const __grid_constant__ ConvMaps ma
         for (int q = 0; q < 4; ++q) {
           int mq;
           bool vq;
-          out_row(16 * w + (l >> 2) + 8 * (q & 1) + 64 * (q >> 1), mq, vq);
+          tile_row(P, o, 16 * w + (l >> 2) + 8 * (q & 1) + 64 * (q >> 1), mq, vq);
           rb[q] = vq ? __ldg(pr.bias + mq) : 0.f;
         }
       }
@@ -569,7 +593,7 @@ conv_gemm_persist_kernel(const ConvParams P, const __grid_constant__ ConvMaps ma
     const int s0 = g0 % kStages;
     const uint32_t ph0 = uint32_t(g0 / kStages) & 1u;
     if (j > 0) mbar_wait_quiet(order_bar(c), uint32_t((j >> 1) - (1 - c)) & 1u);
-    const int s_last = mma_loop<128, true>(acc0, acc1, smem_base, kStages, nkb, s0, ph0, full_bar, hand_back);
+    const int s_last = mma_loop<128>(acc0, acc1, smem_base, kStages, nkb, s0, ph0, full_bar, hand_back);
     if (l == 0) mbar_arrive(order_bar(c ^ 1));          // every MMA of this tile is issued: the other consumer's turn
     wgmma_wait<0>();
     hand_back(s_last);
@@ -577,26 +601,7 @@ conv_gemm_persist_kernel(const ConvParams P, const __grid_constant__ ConvMaps ma
     if constexpr (!XM) {
       // ---- epilogue on the accumulator registers, 16 columns at a time, then the TMA store of the tile
       if (has_res) mbar_wait_quiet(res_bar(c), uint32_t(j >> 1) & 1u);
-      const int mode_act = P.act * 3 + mode;
-      const uint32_t sa = sout + uint32_t(16 * w + (l & 7) + 8 * ((l >> 3) & 1)) * 128u;   // stmatrix row of this lane
-      const float* sb = sbias + 2 * (l & 3);
-#pragma unroll 1
-      for (int p = 0; p < 8; ++p) {
-        float v[16];
-        switch (p) {
-          case 0: take_cols16<0>(acc0, acc1, v); break;
-          case 1: take_cols16<1>(acc0, acc1, v); break;
-          case 2: take_cols16<2>(acc0, acc1, v); break;
-          case 3: take_cols16<3>(acc0, acc1, v); break;
-          case 4: take_cols16<4>(acc0, acc1, v); break;
-          case 5: take_cols16<5>(acc0, acc1, v); break;
-          case 6: take_cols16<6>(acc0, acc1, v); break;
-          default: take_cols16<7>(acc0, acc1, v); break;
-        }
-        // half p / 4 of the tile; 16-byte chunk 2 (p % 4) + l / 16 of the 128-byte row, 128B-swizzled by the row
-        const uint32_t a = sa + uint32_t(p >> 2) * uint32_t(PL::kHalfBytes) + (uint32_t((2 * (p & 3) + (l >> 4)) ^ (l & 7)) << 4);
-        epi_fragments_dispatch(mode_act, v, a, sb + 16 * p, rb, alpha, beta);
-      }
+      epi_tile_fragments<64>(P.act * 3 + mode, acc0, acc1, sout, sbias, rb, alpha, beta, w, l);
       fence_proxy_async_smem();                             // the tile is visible to the TMA unit ...
       named_bar_sync(bar_id, 128);                          // ... once every thread of the warpgroup has written its part
       if (t == 0) {
@@ -704,6 +709,7 @@ static int fill_geom(const icaf_conv_geom* g, int n_io, ConvParams& P) {
   P.a_mode = A_GATHER; P.tw = P.th = P.tiles_x = P.tiles_y = 0; P.stages = 2; P.splits = 1; P.cblk = 64;
   P.ln_parts = 0; P.ln_eps = 0.f; P.ln_inv_k = 0.f;
   P.m_tiles = P.n_tiles = P.tiles = 0;
+  P.tma_epi = 0;
   memset(P.p, 0, sizeof(P.p));
   return ICAF_OK;
 }
@@ -821,9 +827,9 @@ static int plan_persist(ConvParams& P, ConvPlan& pl) {
   return ICAF_OK;
 }
 
-// out_maps: the output (and residual) maps of the persistent kernel's TMA-store epilogue, 64-column boxes of the tile's rows
-// (2-D: 128 rows of [M][N]; 4-D: the tw x th patch of the (N, Wo, Ho, B) view).  They span N columns, so a tile never
-// writes the channels next to a slice of a wider buffer.
+// out_maps: the output (and residual) maps of the register epilogue's TMA stores, 64-column boxes of the tile's rows
+// (2-D: 128 rows of [M][N], for A_TMA2D and A_GATHER; 4-D: the tw x th patch of the (N, Wo, Ho, B) view).  They span N
+// columns, so a tile never writes the channels next to a slice of a wider buffer.
 template <int BN>
 static int encode_maps(const ConvParams& P, const __half* const (&w)[2], const icaf_conv_geom* g, int n_io, bool out_maps,
                        ConvMaps& maps) {
@@ -840,7 +846,7 @@ static int encode_maps(const ConvParams& P, const __half* const (&w)[2], const i
     if (rc) return rc;
     if (out_maps) {
       auto out_map = [&](CUtensorMap* m, const __half* base, long long ld) {
-        return P.a_mode == A_TMA2D ? encode_tmap_2d(m, base, (uint64_t)P.N, (uint64_t)P.M, (uint64_t)ld * 2, 64, BM)
+        return P.a_mode != A_TMA4D ? encode_tmap_2d(m, base, (uint64_t)P.N, (uint64_t)P.M, (uint64_t)ld * 2, 64, BM)
                                    : encode_tmap_nhwc(m, base, P.N, P.Wo, P.Ho, P.B, ld, 64, P.tw, P.th, 1, 1);
       };
       if ((rc = out_map(&maps.y[i], pr.y, pr.y_ld))) return rc;
@@ -853,7 +859,7 @@ static int encode_maps(const ConvParams& P, const __half* const (&w)[2], const i
 
 // Launch a planned conv on the kernel the plan picked (XM: the LayerNorm-fold / row-statistics instantiation).  Its
 // shared-memory limit is raised once per device; the filter maps are encoded for the plan's tile width, and the output
-// maps for the persistent kernel's TMA-store epilogue.
+// maps for the TMA-store epilogue of either kernel.
 template <int BN>
 static int launch_conv(const ConvParams& P, const ConvPlan& pl, const __half* const (&w)[2], const icaf_conv_geom* g, int n_io,
                        cudaStream_t st) {
@@ -863,7 +869,7 @@ static int launch_conv(const ConvParams& P, const ConvPlan& pl, const __half* co
   static bool configured[2][2][kMaxDevices] = {};
   if (int rc = configure_smem(kernel, 227 * 1024, configured[pl.persist][xm], "conv2d: cudaFuncSetAttribute")) return rc;
   ConvMaps maps;
-  if (int rc = encode_maps<BN>(P, w, g, n_io, pl.persist && !xm, maps)) return rc;
+  if (int rc = encode_maps<BN>(P, w, g, n_io, (pl.persist && !xm) || P.tma_epi, maps)) return rc;
   // the one-tile kernel takes the tile grid (split-K: in clusters along x); the persistent one `ctas` CTAs
   const dim3 grid = pl.persist ? dim3(unsigned(pl.ctas)) : dim3(pl.grid_x, pl.grid_y, pl.grid_z);
   launch_kc(kernel, grid, dim3(pl.persist ? kPersistThreads : kThreads), (size_t)pl.smem, st, pl.cluster, P, maps);
@@ -935,6 +941,9 @@ extern "C" int icaf_conv2d_fwd(const icaf_conv_geom* g, const icaf_conv_io* io, 
   ConvPlan pl;
   rc = plan_conv(g, n_io, sm_count_cached(), P, pl, xm || tma_out);
   if (rc) return rc;
+  // The one-tile kernel runs the same register epilogue with TMA stores where it can; split-K (the leader reduces the
+  // staged rows of the cluster), XM and BN = 32 launches keep the staged-row epilogue.
+  P.tma_epi = (!pl.persist && !xm && tma_out && P.splits == 1 && pl.bn >= 64) ? 1 : 0;
   cudaStream_t st = (cudaStream_t)stream;
   switch (pl.bn) {
     case 128: return launch_conv<128>(P, pl, w, g, n_io, st);
