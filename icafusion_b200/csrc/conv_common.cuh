@@ -1,5 +1,6 @@
 // Shared pieces of the implicit-GEMM conv kernels (conv_gemm.cu): problem descriptors, TMA descriptor bundle, tile origin,
-// and the epilogues (staged rows: load, chunk dispatch; accumulator registers: fragments into a TMA-stored output tile).
+// and the epilogues (staged rows: row set-up, load, chunk dispatch; accumulator registers: row bias, fragments into an
+// output tile, its TMA store and the residual tile's TMA load).
 #pragma once
 #include "icaf_internal.cuh"
 
@@ -32,7 +33,7 @@ struct ConvParams {
   int ln_parts;                           // LN fold: partials per input row (0 = no fold)
   float ln_eps, ln_inv_k;                 // LN fold: epsilon, 1 / (normalised features = K)
   int m_tiles, n_tiles, tiles;            // persistent kernel: tile grid (m, n, problem) and its product
-  int tma_epi;                            // one-tile kernel: register epilogue + TMA-stored output tile (else staged rows)
+  int tma_epi;                            // register epilogue + TMA-stored output tile (else staged rows), set by plan_conv
 };
 struct ConvMaps {          // TMA descriptors, passed by value as a __grid_constant__ kernel parameter
   CUtensorMap w[2];
@@ -100,6 +101,34 @@ __device__ __forceinline__ void epi_row_ln(EpiRow& ex, const ConvParams& P, cons
   ex.ln_mu = mu;
   ex.ln_a = rsqrtf(fmaxf(sq * P.ln_inv_k - mu * mu, 0.f) + P.ln_eps);
 }
+
+// The output row of an epilogue thread that owns tile row `row` (staged-row epilogue): output row m (mvalid: inside the
+// output), its row bias (ICAF_EPI_BIAS_ROW), output and residual row pointers, and the XM extras.  Everything here is
+// independent of the main loop, so it is set up (and the residual row prefetched into L2) while the main loop still runs.
+struct StagedRow {
+  int m;
+  bool mvalid;
+  float rbias;
+  __half* yrow;
+  const __half* rrow;
+  EpiRow ex;
+};
+template <int BN, bool XM>
+__device__ __forceinline__ void staged_row(StagedRow& r, const ConvParams& P, const ConvProblem& pr, const TileOrigin& o, int row, int n0) {
+  tile_row(P, o, row, r.m, r.mvalid);
+  r.rbias = ((P.epi & ICAF_EPI_BIAS_ROW) && pr.bias && r.mvalid) ? __ldg(pr.bias + r.m) : 0.f;
+  r.yrow = pr.y + size_t(r.mvalid ? r.m : 0) * pr.y_ld;
+  r.rrow = pr.res ? pr.res + size_t(r.mvalid ? r.m : 0) * pr.res_ld : nullptr;
+  if (r.rrow && r.mvalid) {
+    for (int cb = 0; cb < BN && n0 + cb < P.N; cb += 64) prefetch_l2(r.rrow + n0 + cb);   // 128-byte lines of the residual row
+  }
+  r.ex.sum = r.ex.sumsq = 0.f; r.ex.ln_a = 1.f; r.ex.ln_mu = 0.f; r.ex.ln_s = nullptr;
+  if (XM) {
+    r.ex.ln_s = pr.ln_s ? pr.ln_s + n0 : nullptr;
+    if (P.ln_parts > 0) epi_row_ln(r.ex, P, pr, r.m, r.mvalid);   // row statistics
+  }
+}
+
 // slots [n_begin/32, n_end/32) of this row's partials: the first one carries the sums, the others zero
 __device__ __forceinline__ void epi_row_emit(const EpiRow& ex, const ConvParams& P, const ConvProblem& pr, int m, int n_begin, int n_end) {
   const int slots = (P.N + 31) >> 5;
@@ -215,6 +244,26 @@ __device__ __forceinline__ void epi_dispatch(int mode_act, const uint32_t (&acc)
   }
 }
 
+// The launch's mode_act (see epi_dispatch) for both epilogues: 3 * ACT + RES (has_res: the launch adds a residual), or
+// the XM modes.
+template <bool XM>
+__device__ __forceinline__ int epi_mode_act(const ConvParams& P, bool has_res) {
+  if (XM) return P.ln_parts > 0 ? (P.act == ICAF_ACT_GELU ? 10 : 9) : 11;
+  return P.act * 3 + ((P.epi & ICAF_EPI_SCALED_RES) ? 2 : (has_res ? 1 : 0));
+}
+
+// Staged-row epilogue of tile columns [cb, cb + 32) of row r, output columns from nb = n0 + cb < N: the 32 staged
+// accumulators acc, sbias = the tile's column bias.  16-byte vectors when all 32 columns are inside the output and aligned.
+template <bool XM>
+__device__ __forceinline__ void epi_staged_chunk(int mode_act, const uint32_t (&acc)[32], StagedRow& r, const float* sbias,
+                                                 float alpha, float beta, int cb, int nb, int N) {
+  const int ncols = min(32, N - nb);
+  const bool vec = ncols == 32 && ((reinterpret_cast<uintptr_t>(r.yrow + nb) & 15) == 0) &&
+                   (!r.rrow || (reinterpret_cast<uintptr_t>(r.rrow + nb) & 15) == 0);
+  epi_dispatch<XM>(mode_act, acc, sbias + cb, r.rbias, alpha, beta, r.rrow ? r.rrow + nb : nullptr, r.yrow + nb, vec, ncols,
+                   r.ex, cb);
+}
+
 // ---------------------------------------------------------------------------------------------------
 // Epilogue on the accumulator registers of a consumer warpgroup (tile rows 0-63 in acc0, 64-127 in acc1, NA = BN / 2 each),
 // written as fp16 into an output tile of 64-column halves: 128 rows of 128 bytes each, 128B-swizzled (the layout of a TMA
@@ -297,6 +346,48 @@ __device__ __forceinline__ void epi_tile_fragments(int mode_act, const float (&a
   }
 }
 
+// rb of epi_tile_fragments (zero-initialised by the caller): the row bias (ICAF_EPI_BIAS_ROW) of this lane's accumulator
+// rows l/4 + {0, 8, 64, 72} of warp w
+__device__ __forceinline__ void fragment_row_bias(float (&rb)[4], const ConvParams& P, const ConvProblem& pr, const TileOrigin& o,
+                                                  int w, int l) {
+  if ((P.epi & ICAF_EPI_BIAS_ROW) && pr.bias) {
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      int mq;
+      bool vq;
+      tile_row(P, o, 16 * w + (l >> 2) + 8 * (q & 1) + 64 * (q >> 1), mq, vq);
+      rb[q] = vq ? __ldg(pr.bias + mq) : 0.f;
+    }
+  }
+}
+
+// The 64-column halves of a BN-wide tile from column n0 that lie inside the output, each one TMA box of the output or
+// residual map: 128 rows from m0 (2-D map: A_TMA2D and A_GATHER launches) or the tw x th patch (4-D map: A_TMA4D).  In
+// shared memory the halves are kOutHalfBytes apart from `s`.  The store commits one bulk group; the load completes on `bar`.
+template <int BN>
+__device__ __forceinline__ void tma_store_tile(const ConvParams& P, const CUtensorMap* map, uint32_t s, int n0, const TileOrigin& o) {
+  const int halves = (BN == 128 && n0 + 64 < P.N) ? 2 : 1;
+  for (int hh = 0; hh < halves; ++hh) {
+    const uint32_t src = s + uint32_t(hh * kOutHalfBytes);
+    if (P.a_mode == A_TMA4D) tma_store_4d(map, src, n0 + 64 * hh, o.ox0, o.oy0, o.tb);
+    else tma_store_2d(map, src, n0 + 64 * hh, o.m0);
+  }
+  bulk_commit_group();
+}
+
+template <int BN>
+__device__ __forceinline__ void tma_load_tile(const ConvParams& P, const CUtensorMap* map, uint32_t s, uint32_t bar, int n0,
+                                              const TileOrigin& o) {
+  const int halves = (BN == 128 && n0 + 64 < P.N) ? 2 : 1;
+  const uint32_t half_bytes = P.a_mode == A_TMA4D ? uint32_t(P.tw * P.th) * 128u : uint32_t(kOutHalfBytes);
+  mbar_arrive_expect_tx(bar, uint32_t(halves) * half_bytes);
+  for (int hh = 0; hh < halves; ++hh) {
+    const uint32_t dst = s + uint32_t(hh * kOutHalfBytes);
+    if (P.a_mode == A_TMA4D) tma_load_4d(dst, map, bar, n0 + 64 * hh, o.ox0, o.oy0, o.tb);
+    else tma_load_2d(dst, map, bar, n0 + 64 * hh, o.m0);
+  }
+}
+
 // Host-side launch plan: everything the dispatcher decides before it touches CUDA.  icaf_conv2d_plan (host only, no
 // device needed) exposes it so that a CPU test can walk every layer geometry through the dispatcher's invariants.
 struct ConvPlan {
@@ -307,6 +398,7 @@ struct ConvPlan {
   int tiles, m_tiles, n_tiles;    // output tiles of the launch (icaf_conv_plan.work_items) = m_tiles * n_tiles * problems
   int sms;                        // SM count the plan was made for
   bool persist;                   // conv_gemm_persist_kernel: `ctas` CTAs walk the grid_x * grid_y * grid_z tiles
+  bool xm;                        // LayerNorm-fold / row-statistics epilogue: the XM instantiation of either kernel
   int ctas;                       // CTAs the launch starts
 };
 

@@ -21,12 +21,14 @@
 // tiles (BN <= 64) let two CTAs share an SM so that one CTA's epilogue overlaps the other's main loop.  Split-K: the
 // CTAs of a cluster take a K range each; the leader adds the others' staged tiles through distributed shared memory.
 // The register epilogue serves BN >= 64 launches that are not XM or split-K and whose output TMA can write; the others
-// keep the staged rows.
+// keep the staged rows.  plan_conv makes that choice for both kernels (ConvParams::tma_epi).
 // conv_gemm_persist_kernel: BN = 128 grids of more than one wave with TMA-staged A -- one persistent CTA per SM, a TMA
 // producer warpgroup and two consumer warpgroups that take turns on the main loop; each consumer runs the epilogue on its
 // accumulator registers and writes the tile with TMA stores (see its own comment below).
-// The two kernels share the TMA producer stage (load_stage), the main loop (mma_loop), the tile origin, the register
-// epilogue (epi_tile_fragments) and the per-element epilogue expression (epi_value), so they compute bit-identical tiles.
+// The two kernels share the TMA producer stage (load_stage), the main loop (mma_loop), the tile origin, the per-element
+// epilogue expression (epi_value), so they compute bit-identical tiles, and every other epilogue piece (conv_common.cuh):
+// register epilogue (fragment_row_bias, epi_tile_fragments, tma_store_tile, tma_load_tile), staged rows (staged_row,
+// epi_staged_chunk) and the mode selection (epi_mode_act).
 #include <cstdlib>
 #include <cstring>
 
@@ -140,10 +142,10 @@ conv_gemm_tc_kernel(const ConvParams P, const __grid_constant__ ConvMaps maps) {
   int m0, tb, oy0, ox0;
   tile_origin(P, mtile, m0, tb, oy0, ox0);
   const TileOrigin o{m0, tb, oy0, ox0};
-  // Register epilogue (host: not XM, no split-K, output writable by TMA, BN >= 64): the consumer warpgroup applies the
-  // epilogue to its accumulators and stores the tile by TMA from ring stage s_out -- the stage the K block after the last
-  // one would take.  It is free once block nkb - stages has been consumed, so a residual tile is TMA-loaded into it (on
-  // res_bar) while the last blocks of the main loop still run.
+  // Register epilogue (P.tma_epi, see plan_conv; the XM and BN = 32 instantiations leave its code out): the consumer
+  // warpgroup applies the epilogue to its accumulators and stores the tile by TMA from ring stage s_out -- the stage the K
+  // block after the last one would take.  It is free once block nkb - stages has been consumed, so a residual tile is
+  // TMA-loaded into it (on res_bar) while the last blocks of the main loop still run.
   const bool tma_epi = !XM && BN >= 64 && P.tma_epi != 0;
   const bool has_res = (P.epi & (ICAF_EPI_ADD_RES | ICAF_EPI_SCALED_RES)) != 0;
   const int s_out = nkb % kStages;
@@ -245,36 +247,14 @@ conv_gemm_tc_kernel(const ConvParams P, const __grid_constant__ ConvMaps maps) {
 
     // ------------------------------------------------------------------ epilogue
     const int row = tid;                   // staged accumulator row == tile row
-    int m;
-    bool mvalid;
-    if (a_mode == A_TMA4D) {
-      const int ry = row / P.tw, rx = row - ry * P.tw;
-      m = (tb * P.Ho + oy0 + ry) * P.Wo + ox0 + rx;
-      mvalid = ry < P.th && oy0 + ry < P.Ho;      // tw divides Wo; the last tile row of an image may hang over
-    } else {
-      m = m0 + row;
-      mvalid = m < P.M;
-    }
-    const float rbias = ((P.epi & ICAF_EPI_BIAS_ROW) && pr.bias && mvalid) ? __ldg(pr.bias + m) : 0.f;
-    __half* yrow = pr.y + size_t(mvalid ? m : 0) * pr.y_ld;
-    const __half* rrow = pr.res ? pr.res + size_t(mvalid ? m : 0) * pr.res_ld : nullptr;
-    const int mode = (P.epi & ICAF_EPI_SCALED_RES) ? 2 : (rrow ? 1 : 0);
-    if (rrow && mvalid) {
-      for (int cb = 0; cb < BN && n0 + cb < P.N; cb += 64) prefetch_l2(rrow + n0 + cb);   // 128-byte lines of the residual row
-    }
+    StagedRow sr;
+    staged_row<BN, XM>(sr, P, pr, o, row, n0);
 #pragma unroll
     for (int i = 0; i < (BN + 127) / 128; ++i)
       if (tid + 128 * i < BN) sbias[tid + 128 * i] = bias_r[i];
-    EpiRow ex;
-    ex.sum = ex.sumsq = 0.f; ex.ln_a = 1.f; ex.ln_mu = 0.f; ex.ln_s = nullptr;
-    if (XM) {
-      ex.ln_s = pr.ln_s ? pr.ln_s + n0 : nullptr;
-      if (P.ln_parts > 0) epi_row_ln(ex, P, pr, m, mvalid);   // row statistics: fetched while the main loop still runs
-    }
     // the staged accumulators (of every CTA of the cluster) and the bias tile are complete
     if (splits > 1) { cluster_arrive(); cluster_wait(); } else { named_bar_sync(1, 256); }
-    // XM: 9 / 10 = LayerNorm folded into this GEMM (no activation / GELU); 11 = scaled residual + statistics of the output rows
-    const int mode_act = XM ? (P.ln_parts > 0 ? (P.act == ICAF_ACT_GELU ? 10 : 9) : 11) : P.act * 3 + mode;
+    const int mode_act = epi_mode_act<XM>(P, sr.rrow != nullptr);
     if (crank == 0) {
       const float* arow = sacc + size_t(row) * L::kPitch;
       const uint32_t arow_s = smem_u32(arow);
@@ -295,18 +275,9 @@ conv_gemm_tc_kernel(const ConvParams P, const __grid_constant__ ConvMaps maps) {
             acc[4 * q + 3] = __float_as_uint(__uint_as_float(acc[4 * q + 3]) + v.w);
           }
         }
-        const int nb = n0 + cb;
-        if (mvalid && nb < P.N) {
-          const int ncols = min(32, P.N - nb);
-          const bool vec = ncols == 32 && ((reinterpret_cast<uintptr_t>(yrow + nb) & 15) == 0) &&
-                           (!rrow || (reinterpret_cast<uintptr_t>(rrow + nb) & 15) == 0);
-          const float* sb = sbias + cb;
-          const __half* rp = rrow ? rrow + nb : nullptr;
-          __half* yp = yrow + nb;
-          epi_dispatch<XM>(mode_act, acc, sb, rbias, alpha, beta, rp, yp, vec, ncols, ex, cb);
-        }
+        if (sr.mvalid && n0 + cb < P.N) epi_staged_chunk<XM>(mode_act, acc, sr, sbias, alpha, beta, cb, n0 + cb, P.N);
       }
-      if (XM && mode_act == 11 && mvalid && n0 < P.N) epi_row_emit(ex, P, pr, m, n0, min(n0 + BN, P.N));
+      if (XM && mode_act == 11 && sr.mvalid && n0 < P.N) epi_row_emit(sr.ex, P, pr, sr.m, n0, min(n0 + BN, P.N));
     }
     if (splits > 1) { cluster_arrive(); cluster_wait(); }   // the peers' staged tiles stay alive until the leader has read them
   } else if (warp < 8) {
@@ -314,20 +285,12 @@ conv_gemm_tc_kernel(const ConvParams P, const __grid_constant__ ConvMaps maps) {
     if constexpr (rebalance_regs<BN, XM>()) setmaxnreg_inc<kRegsHigh>();
     const int t = tid - 128, w = t >> 5, l = t & 31;
     float alpha = 0.f, beta = 1.f;
-    float rb[4] = {0.f, 0.f, 0.f, 0.f};      // tma_epi: row bias of this lane's accumulator rows l/4 + {0, 8, 64, 72}
+    float rb[4] = {0.f, 0.f, 0.f, 0.f};      // tma_epi: row bias of the accumulator fragments
     if (tma_epi) {
       // epilogue operands that do not depend on the main loop: bias slice, (alpha, beta), row bias
       if (t < BN) sbias[t] = (pr.bias && !(P.epi & ICAF_EPI_BIAS_ROW) && n0 + t < P.N) ? __ldg(pr.bias + n0 + t) : 0.f;
       if (P.epi & ICAF_EPI_SCALED_RES) { alpha = __ldg(pr.alpha); beta = __ldg(pr.beta); }
-      if ((P.epi & ICAF_EPI_BIAS_ROW) && pr.bias) {
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          int mq;
-          bool vq;
-          tile_row(P, o, 16 * w + (l >> 2) + 8 * (q & 1) + 64 * (q >> 1), mq, vq);
-          rb[q] = vq ? __ldg(pr.bias + mq) : 0.f;
-        }
-      }
+      fragment_row_bias(rb, P, pr, o, w, l);
       named_bar_sync(2, 128);                                 // bias slice complete
     }
     float acc0[BN / 2], acc1[BN / 2];
@@ -341,19 +304,11 @@ conv_gemm_tc_kernel(const ConvParams P, const __grid_constant__ ConvMaps maps) {
         // ---- epilogue on the accumulator registers into ring stage s_out (every stage is consumed now), TMA store
         const uint32_t sout = smem_base + uint32_t(s_out) * L::kStageBytes;
         if (has_res) mbar_wait_quiet(res_bar, 0);
-        const int mode = (P.epi & ICAF_EPI_SCALED_RES) ? 2 : (has_res ? 1 : 0);
-        epi_tile_fragments<BN / 2>(P.act * 3 + mode, acc0, acc1, sout, sbias, rb, alpha, beta, w, l);
+        epi_tile_fragments<BN / 2>(epi_mode_act<false>(P, has_res), acc0, acc1, sout, sbias, rb, alpha, beta, w, l);
         fence_proxy_async_smem();                             // the tile is visible to the TMA unit ...
         named_bar_sync(2, 128);                               // ... once every thread of the warpgroup has written its part
         if (t == 0) {
-          const CUtensorMap* my = bz ? &maps.y[1] : &maps.y[0];
-          const int halves = (BN == 128 && n0 + 64 < P.N) ? 2 : 1;
-          for (int hh = 0; hh < halves; ++hh) {
-            const uint32_t src = sout + uint32_t(hh * kOutHalfBytes);
-            if (a_mode == A_TMA4D) tma_store_4d(my, src, n0 + 64 * hh, o.ox0, o.oy0, o.tb);
-            else tma_store_2d(my, src, n0 + 64 * hh, o.m0);
-          }
-          bulk_commit_group();
+          tma_store_tile<BN>(P, bz ? &maps.y[1] : &maps.y[0], sout, n0, o);
           bulk_wait_group<0>();                               // complete before the grid is (PDL dependents read it)
         }
         return;
@@ -382,18 +337,9 @@ conv_gemm_tc_kernel(const ConvParams P, const __grid_constant__ ConvMaps maps) {
         if (++s == kStages) { s = 0; ph ^= 1; }
       }
       if (tma_epi && has_res) {
-        // the residual tile into stage s_out (== s) once block nkb - stages has left it: 64-column boxes of 128 rows (2-D)
-        // or tw x th pixels (4-D)
+        // the residual tile into stage s_out (== s) once block nkb - stages has left it
         mbar_wait_quiet(empty_bar(s), ph ^ 1);
-        const CUtensorMap* mr = bz ? &maps.res[1] : &maps.res[0];
-        const int halves = (BN == 128 && n0 + 64 < P.N) ? 2 : 1;
-        const uint32_t half_bytes = a_mode == A_TMA4D ? uint32_t(P.tw * P.th) * 128u : uint32_t(kOutHalfBytes);
-        mbar_arrive_expect_tx(res_bar, uint32_t(halves) * half_bytes);
-        for (int hh = 0; hh < halves; ++hh) {
-          const uint32_t dst = smem_base + uint32_t(s) * L::kStageBytes + uint32_t(hh * kOutHalfBytes);
-          if (a_mode == A_TMA4D) tma_load_4d(dst, mr, res_bar, n0 + 64 * hh, o.ox0, o.oy0, o.tb);
-          else tma_load_2d(dst, mr, res_bar, n0 + 64 * hh, o.m0);
-        }
+        tma_load_tile<BN>(P, bz ? &maps.res[1] : &maps.res[0], smem_base + uint32_t(s) * L::kStageBytes, res_bar, n0, o);
       }
     }
     __syncwarp();
@@ -418,8 +364,7 @@ conv_gemm_tc_kernel(const ConvParams P, const __grid_constant__ ConvMaps maps) {
 constexpr int kPersistThreads = 384;
 struct PersistLayout {
   static constexpr int kStageBytes = SmemLayout<128>::kStageBytes;
-  static constexpr int kHalfBytes = kOutHalfBytes;             // one 64-column half of the output tile
-  static constexpr int kOutBytes = 2 * kHalfBytes;             // per consumer, 1024-byte aligned (TMA 128B swizzle)
+  static constexpr int kOutBytes = 2 * kOutHalfBytes;          // per consumer, 1024-byte aligned (TMA 128B swizzle)
   static constexpr int kPitch = 32 + 4;                        // XM: floats per staged row of a 32-column chunk
   static constexpr int kChunkBytes = BM * kPitch * 4;
   static_assert(kChunkBytes <= kOutBytes, "the XM staged chunk lives in the output tile");
@@ -526,58 +471,27 @@ conv_gemm_persist_kernel(const ConvParams P, const __grid_constant__ ConvMaps ma
   const uint32_t sout = smem_base + uint32_t(kStages * L::kStageBytes + c * PL::kOutBytes);   // this consumer's output tile
   float* sacc = reinterpret_cast<float*>(smem_gen + kStages * L::kStageBytes + c * PL::kOutBytes);   // XM: staged chunk
   float* sbias = reinterpret_cast<float*>(smem_gen + bar_off + 256 + c * 128 * 4);
-  // output / residual box: 64 columns x 128 rows (2-D) or 64 columns x tw x th pixels (4-D)
-  const uint32_t half_bytes = a_mode == A_TMA2D ? uint32_t(PL::kHalfBytes) : uint32_t(P.tw * P.th) * 128u;
   for (int tile = blockIdx.x + c * gridDim.x; tile < P.tiles; tile += 2 * gridDim.x) {
     const int j = (tile - int(blockIdx.x)) / int(gridDim.x);  // ordinal of the tile among this CTA's tiles
     const PersistTile pt = persist_tile(P, tile);
     const ConvProblem pr = pick_problem(P, pt.z);
     const int n0 = pt.n0;
     const TileOrigin& o = pt.o;
-    const int halves = n0 + 64 < P.N ? 2 : 1;                 // 64-column halves of the tile inside the output
     // Epilogue operands that do not depend on the main loop are fetched now so their DRAM latency hides behind it:
-    // bias slice and (alpha, beta) into registers; XM: this thread's residual row into L2; otherwise the residual tile.
+    // bias slice and (alpha, beta) into registers; XM: this thread's output row (residual row into L2); otherwise the
+    // row bias of the accumulator fragments and the residual tile.
     const float bias_r = (pr.bias && !(P.epi & ICAF_EPI_BIAS_ROW) && n0 + t < P.N) ? __ldg(pr.bias + n0 + t) : 0.f;
     float alpha = 0.f, beta = 1.f;
     if (P.epi & ICAF_EPI_SCALED_RES) { alpha = __ldg(pr.alpha); beta = __ldg(pr.beta); }
-    const int row = t;
-    int m;
-    bool mvalid;
-    tile_row(P, o, row, m, mvalid);
-    const float rbias = ((P.epi & ICAF_EPI_BIAS_ROW) && pr.bias && mvalid) ? __ldg(pr.bias + m) : 0.f;
-    __half* yrow = pr.y + size_t(mvalid ? m : 0) * pr.y_ld;
-    const __half* rrow = pr.res ? pr.res + size_t(mvalid ? m : 0) * pr.res_ld : nullptr;
-    const int mode = (P.epi & ICAF_EPI_SCALED_RES) ? 2 : (has_res ? 1 : 0);
-    EpiRow ex;
-    ex.sum = ex.sumsq = 0.f; ex.ln_a = 1.f; ex.ln_mu = 0.f; ex.ln_s = nullptr;
-    float rb[4] = {0.f, 0.f, 0.f, 0.f};      // !XM: row bias of this lane's accumulator rows l/4 + {0, 8, 64, 72}
+    StagedRow sr;                                             // XM
+    float rb[4] = {0.f, 0.f, 0.f, 0.f};                       // !XM: row bias of the accumulator fragments
     if (XM) {
-      if (rrow && mvalid) {
-        for (int cb = 0; cb < 128 && n0 + cb < P.N; cb += 64) prefetch_l2(rrow + n0 + cb);
-      }
-      ex.ln_s = pr.ln_s ? pr.ln_s + n0 : nullptr;
-      if (P.ln_parts > 0) epi_row_ln(ex, P, pr, m, mvalid);
+      staged_row<128, XM>(sr, P, pr, o, t, n0);
     } else {
-      if ((P.epi & ICAF_EPI_BIAS_ROW) && pr.bias) {
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          int mq;
-          bool vq;
-          tile_row(P, o, 16 * w + (l >> 2) + 8 * (q & 1) + 64 * (q >> 1), mq, vq);
-          rb[q] = vq ? __ldg(pr.bias + mq) : 0.f;
-        }
-      }
+      fragment_row_bias(rb, P, pr, o, w, l);
       if (t == 0) {
         bulk_wait_group_read<0>();                            // the previous tile's TMA store has read the buffer
-        if (has_res) {
-          const CUtensorMap* mr = pt.z ? &maps.res[1] : &maps.res[0];
-          mbar_arrive_expect_tx(res_bar(c), uint32_t(halves) * half_bytes);
-          for (int hh = 0; hh < halves; ++hh) {
-            const uint32_t dst = sout + uint32_t(hh * PL::kHalfBytes);
-            if (a_mode == A_TMA2D) tma_load_2d(dst, mr, res_bar(c), n0 + 64 * hh, o.m0);
-            else tma_load_4d(dst, mr, res_bar(c), n0 + 64 * hh, o.ox0, o.oy0, o.tb);
-          }
-        }
+        if (has_res) tma_load_tile<128>(P, pt.z ? &maps.res[1] : &maps.res[0], sout, res_bar(c), n0, o);
       }
       sbias[t] = bias_r;
       named_bar_sync(bar_id, 128);                            // bias slice complete, output tile free
@@ -601,17 +515,11 @@ conv_gemm_persist_kernel(const ConvParams P, const __grid_constant__ ConvMaps ma
     if constexpr (!XM) {
       // ---- epilogue on the accumulator registers, 16 columns at a time, then the TMA store of the tile
       if (has_res) mbar_wait_quiet(res_bar(c), uint32_t(j >> 1) & 1u);
-      epi_tile_fragments<64>(P.act * 3 + mode, acc0, acc1, sout, sbias, rb, alpha, beta, w, l);
+      epi_tile_fragments<64>(epi_mode_act<false>(P, has_res), acc0, acc1, sout, sbias, rb, alpha, beta, w, l);
       fence_proxy_async_smem();                             // the tile is visible to the TMA unit ...
       named_bar_sync(bar_id, 128);                          // ... once every thread of the warpgroup has written its part
       if (t == 0) {
-        const CUtensorMap* my = pt.z ? &maps.y[1] : &maps.y[0];
-        for (int hh = 0; hh < halves; ++hh) {
-          const uint32_t src = sout + uint32_t(hh * PL::kHalfBytes);
-          if (a_mode == A_TMA2D) tma_store_2d(my, src, n0 + 64 * hh, o.m0);
-          else tma_store_4d(my, src, n0 + 64 * hh, o.ox0, o.oy0, o.tb);
-        }
-        bulk_commit_group();
+        tma_store_tile<128>(P, pt.z ? &maps.y[1] : &maps.y[0], sout, n0, o);
         // this consumer's last tile: its writes complete before the grid does (dependent launches read them after
         // griddepcontrol.wait).  Waiting inside the loop keeps the consumer's code one setmaxnreg region for ptxas.
         if (tile + 2 * int(gridDim.x) >= P.tiles) bulk_wait_group<0>();
@@ -620,9 +528,8 @@ conv_gemm_persist_kernel(const ConvParams P, const __grid_constant__ ConvMaps ma
     }
 
     // ---- XM epilogue, 32 columns at a time
-    // 9 / 10 = LayerNorm folded into this GEMM (no activation / GELU); 11 = scaled residual + statistics of the output rows
-    const int mode_act = P.ln_parts > 0 ? (P.act == ICAF_ACT_GELU ? 10 : 9) : 11;
-    const float* arow = sacc + size_t(row) * PL::kPitch;
+    const int mode_act = epi_mode_act<XM>(P, has_res);
+    const float* arow = sacc + size_t(t) * PL::kPitch;
 #pragma unroll 1
     for (int cc = 0; cc < 4; ++cc) {
       named_bar_sync(bar_id, 128);                      // the previous chunk (or tile) has been read out
@@ -635,20 +542,13 @@ conv_gemm_persist_kernel(const ConvParams P, const __grid_constant__ ConvMaps ma
       }
       named_bar_sync(bar_id, 128);
       const int cb = 32 * cc;
-      const int nb = n0 + cb;
-      if (mvalid && nb < P.N) {
+      if (sr.mvalid && n0 + cb < P.N) {
         uint32_t acc[32];
         load_staged(acc, arow);
-        const int ncols = min(32, P.N - nb);
-        const bool vec = ncols == 32 && ((reinterpret_cast<uintptr_t>(yrow + nb) & 15) == 0) &&
-                         (!rrow || (reinterpret_cast<uintptr_t>(rrow + nb) & 15) == 0);
-        const float* sb = sbias + cb;
-        const __half* rp = rrow ? rrow + nb : nullptr;
-        __half* yp = yrow + nb;
-        epi_dispatch<XM>(mode_act, acc, sb, rbias, alpha, beta, rp, yp, vec, ncols, ex, cb);
+        epi_staged_chunk<XM>(mode_act, acc, sr, sbias, alpha, beta, cb, n0 + cb, P.N);
       }
     }
-    if (mode_act == 11 && mvalid && n0 < P.N) epi_row_emit(ex, P, pr, m, n0, min(n0 + 128, P.N));
+    if (mode_act == 11 && sr.mvalid && n0 < P.N) epi_row_emit(sr.ex, P, pr, sr.m, n0, min(n0 + 128, P.N));
   }
 }
 
@@ -859,17 +759,16 @@ static int encode_maps(const ConvParams& P, const __half* const (&w)[2], const i
 
 // Launch a planned conv on the kernel the plan picked (XM: the LayerNorm-fold / row-statistics instantiation).  Its
 // shared-memory limit is raised once per device; the filter maps are encoded for the plan's tile width, and the output
-// maps for the TMA-store epilogue of either kernel.
+// maps when the launch stores its tiles by TMA (P.tma_epi).
 template <int BN>
 static int launch_conv(const ConvParams& P, const ConvPlan& pl, const __half* const (&w)[2], const icaf_conv_geom* g, int n_io,
                        cudaStream_t st) {
-  const int xm = (P.epi & (ICAF_EPI_LN_FOLD | ICAF_EPI_EMIT_STATS)) ? 1 : 0;
-  void (*kernel)(ConvParams, ConvMaps) = xm ? conv_gemm_tc_kernel<BN, true> : conv_gemm_tc_kernel<BN, false>;
-  if (pl.persist) kernel = xm ? conv_gemm_persist_kernel<true> : conv_gemm_persist_kernel<false>;
+  void (*kernel)(ConvParams, ConvMaps) = pl.xm ? conv_gemm_tc_kernel<BN, true> : conv_gemm_tc_kernel<BN, false>;
+  if (pl.persist) kernel = pl.xm ? conv_gemm_persist_kernel<true> : conv_gemm_persist_kernel<false>;
   static bool configured[2][2][kMaxDevices] = {};
-  if (int rc = configure_smem(kernel, 227 * 1024, configured[pl.persist][xm], "conv2d: cudaFuncSetAttribute")) return rc;
+  if (int rc = configure_smem(kernel, 227 * 1024, configured[pl.persist][pl.xm], "conv2d: cudaFuncSetAttribute")) return rc;
   ConvMaps maps;
-  if (int rc = encode_maps<BN>(P, w, g, n_io, (pl.persist && !xm) || P.tma_epi, maps)) return rc;
+  if (int rc = encode_maps<BN>(P, w, g, n_io, P.tma_epi != 0, maps)) return rc;
   // the one-tile kernel takes the tile grid (split-K: in clusters along x); the persistent one `ctas` CTAs
   const dim3 grid = pl.persist ? dim3(unsigned(pl.ctas)) : dim3(pl.grid_x, pl.grid_y, pl.grid_z);
   launch_kc(kernel, grid, dim3(pl.persist ? kPersistThreads : kThreads), (size_t)pl.smem, st, pl.cluster, P, maps);
@@ -879,11 +778,13 @@ static int launch_conv(const ConvParams& P, const ConvPlan& pl, const __half* co
 // ---------------------------------------------------------------------------------------------------
 // The dispatcher, host only: staging mode, tile shape and tile width for one layer geometry.  No CUDA call.
 // (`pair_mode` of icaf_conv2d_plan selects CTA-pair kernels on architectures that have them; sm_90a has none.)
-// persist_ok = false keeps an eligible launch on the one-tile kernel (its output cannot be written by TMA stores).
-static int plan_conv(const icaf_conv_geom* g, int n_io, int sms, ConvParams& P, ConvPlan& pl, bool persist_ok = true) {
+// It also picks the epilogue (P.tma_epi): tma_out says whether TMA can write the outputs and read the residuals
+// (16-byte aligned bases and row pitches).
+static int plan_conv(const icaf_conv_geom* g, int n_io, int sms, bool tma_out, ConvParams& P, ConvPlan& pl) {
   memset(&pl, 0, sizeof(pl));
   pl.sms = sms;
   if (sms < 1) return set_error(ICAF_ERR_BAD_ARG, "conv2d: SM count must be positive");
+  pl.xm = (P.epi & (ICAF_EPI_LN_FOLD | ICAF_EPI_EMIT_STATS)) != 0;
   plan_a_mode(g, P);
   // Tile width: the widest BN that still yields at least ~one CTA per SM; small problems take BN = 32 so that more SMs
   // share the K loop (and split it over clusters when even that leaves most SMs idle).
@@ -892,14 +793,21 @@ static int plan_conv(const icaf_conv_geom* g, int n_io, int sms, ConvParams& P, 
   int bn = 32;
   if (P.N > 64 && ctas(128) >= sms) bn = 128;
   else if (P.N > 32 && ctas(64) >= sms) bn = 64;
+  int rc;
   switch (bn) {
-    case 128: {
-      if (int rc = plan_tc<128>(P, n_io, pl)) return rc;
-      return (persist_ok && P.a_mode != A_GATHER && P.splits == 1 && pl.tiles > sms) ? plan_persist(P, pl) : ICAF_OK;
-    }
-    case 64: return plan_tc<64>(P, n_io, pl);
-    default: return plan_tc<32>(P, n_io, pl);
+    case 128:
+      rc = plan_tc<128>(P, n_io, pl);
+      // the persistent kernel stores its non-XM tiles by TMA; a launch whose outputs TMA cannot write stays one-tile
+      if (!rc && (pl.xm || tma_out) && P.a_mode != A_GATHER && P.splits == 1 && pl.tiles > sms) rc = plan_persist(P, pl);
+      break;
+    case 64: rc = plan_tc<64>(P, n_io, pl); break;
+    default: rc = plan_tc<32>(P, n_io, pl); break;
   }
+  if (rc) return rc;
+  // Register epilogue with TMA-stored output tiles: every persistent launch but XM; on the one-tile kernel also BN >= 64
+  // without split-K (the leader reduces the cluster's staged rows).  The others keep the staged-row epilogue.
+  P.tma_epi = !pl.xm && (pl.persist || (tma_out && P.splits == 1 && pl.bn >= 64)) ? 1 : 0;
+  return ICAF_OK;
 }
 
 }  // namespace icaf
@@ -914,7 +822,7 @@ extern "C" int icaf_conv2d_plan(const icaf_conv_geom* g, int n_io, int sm_count,
   if (rc) return rc;
   ConvPlan pl;
   (void)pair_mode;
-  rc = plan_conv(g, n_io, sm_count, P, pl);
+  rc = plan_conv(g, n_io, sm_count, true, P, pl);
   if (rc) return rc;
   out->kernel = pl.kernel; out->bn = pl.bn; out->a_mode = P.a_mode;
   out->tile_w = P.tw; out->tile_h = P.th; out->tiles_x = P.tiles_x; out->tiles_y = P.tiles_y;
@@ -929,21 +837,16 @@ extern "C" int icaf_conv2d_fwd(const icaf_conv_geom* g, const icaf_conv_io* io, 
   const __half* w[2];
   int rc = fill_params(g, io, n_io, P, w);
   if (rc) return rc;
-  // The persistent kernel writes its outputs (and reads residuals) by TMA: 16-byte aligned base and row pitch.  The
-  // LayerNorm-fold / row-statistics epilogue (XM) stores rows directly and takes any layout.
+  // TMA stores outputs (and loads residuals) from 16-byte aligned bases with 16-byte aligned row pitches
   bool tma_out = true;
   for (int i = 0; i < n_io; ++i) {
     const ConvProblem& pr = P.p[i];
     tma_out = tma_out && (reinterpret_cast<uintptr_t>(pr.y) & 15) == 0 && pr.y_ld % 8 == 0 &&
               (!pr.res || ((reinterpret_cast<uintptr_t>(pr.res) & 15) == 0 && pr.res_ld % 8 == 0));
   }
-  const bool xm = (P.epi & (ICAF_EPI_LN_FOLD | ICAF_EPI_EMIT_STATS)) != 0;
   ConvPlan pl;
-  rc = plan_conv(g, n_io, sm_count_cached(), P, pl, xm || tma_out);
+  rc = plan_conv(g, n_io, sm_count_cached(), tma_out, P, pl);
   if (rc) return rc;
-  // The one-tile kernel runs the same register epilogue with TMA stores where it can; split-K (the leader reduces the
-  // staged rows of the cluster), XM and BN = 32 launches keep the staged-row epilogue.
-  P.tma_epi = (!pl.persist && !xm && tma_out && P.splits == 1 && pl.bn >= 64) ? 1 : 0;
   cudaStream_t st = (cudaStream_t)stream;
   switch (pl.bn) {
     case 128: return launch_conv<128>(P, pl, w, g, n_io, st);

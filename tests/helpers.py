@@ -18,6 +18,23 @@ def nchw(x_nhwc: torch.Tensor) -> torch.Tensor:
     return x_nhwc.permute(0, 3, 1, 2).contiguous()
 
 
+def sm_count() -> int:
+    """SM count of the current CUDA device."""
+    return torch.cuda.get_device_properties(torch.cuda.current_device()).multi_processor_count
+
+
+def conv_plan(fn):
+    """The icaf_conv2d_plan of the one conv launch `fn` makes, on this device."""
+    import ctypes
+    from icafusion_b200 import _lib, ops
+    with ops.dry_run() as dr:
+        fn()
+    (_, _, work), = dr.records
+    pl = _lib.ConvPlan()
+    assert _lib.lib().icaf_conv2d_plan(ctypes.byref(work["geom"]), work["n_io"], sm_count(), 0, ctypes.byref(pl)) == 0
+    return pl
+
+
 def err(a, b) -> float:
     """max|a-b| / max|b|"""
     a = a.detach().float().cpu().numpy() if torch.is_tensor(a) else np.asarray(a, dtype=np.float32)

@@ -1,12 +1,10 @@
 """wgmma implicit-GEMM conv / linear kernel vs the CPU oracle (torch fp32 conv on the same fp16-rounded
 operands) and vs the on-device CUDA-core reference.  All calls go through the C ABI."""
-import ctypes
-
 import pytest
 import torch
 import torch.nn.functional as F
 
-from helpers import err, nchw, nhwc
+from helpers import conv_plan, err, nchw, nhwc
 
 pytestmark = pytest.mark.gpu
 
@@ -109,18 +107,6 @@ def test_grouped_residual_and_slices(cuda_device):
         assert float(xs[i][..., :C].abs().max()) == 0 and float(xs[i][..., 2 * C:].abs().max()) == 0   # neighbours untouched
 
 
-def _plan(xs, packs, outs, ress):
-    """The icaf_conv2d_plan of the launch ops.conv2d makes for these arguments on this device."""
-    from icafusion_b200 import _lib, ops
-    with ops.dry_run() as dr:
-        ops.conv2d(xs, packs, outs, ress)
-    (_, _, work), = dr.records
-    pl = _lib.ConvPlan()
-    sms = torch.cuda.get_device_properties(xs[0].device).multi_processor_count
-    assert _lib.lib().icaf_conv2d_plan(ctypes.byref(work["geom"]), work["n_io"], sms, 0, ctypes.byref(pl)) == 0
-    return pl
-
-
 def test_persistent_kernel_grouped_residual(cuda_device):
     """Wide-tile (BN = 128) launch with two problems (RGB / IR streams) and the fused Bottleneck residual: more tiles than
     SMs, so it runs on the persistent kernel."""
@@ -133,7 +119,7 @@ def test_persistent_kernel_grouped_residual(cuda_device):
         xs.append(nhwc(x).to(cuda_device)); ress.append(nhwc(res).to(cuda_device))
         packs.append(ops.pack_conv_weight(w.float(), b, 1, 1, 1, device=cuda_device))
         refs.append(_ref(x, w, b, 1, 1, 1) + res.float())
-    pl = _plan(xs, packs, None, ress)
+    pl = conv_plan(lambda: ops.conv2d(xs, packs, None, ress))
     assert pl.ctas < pl.grid_x * pl.grid_y * pl.grid_z, "expected a persistent launch"
     ys = ops.conv2d(xs, packs, None, ress)
     torch.cuda.synchronize()
@@ -169,7 +155,7 @@ def test_one_tile_kernel_grouped_residual(cuda_device):
         xin.append(nhwc(x).to(cuda_device)); ress.append(nhwc(res).to(cuda_device)); outs.append(wide[..., C:])
         packs.append(ops.pack_conv_weight(w.float(), b, 1, 1, 1, device=cuda_device))
         refs.append(_ref(x, w, b, 1, 1, 1) + res.float())
-    pl = _plan(xin, packs, outs, ress)
+    pl = conv_plan(lambda: ops.conv2d(xin, packs, outs, ress))
     assert pl.bn == 64 and pl.ctas == pl.grid_x * pl.grid_y * pl.grid_z, "expected a one-tile-per-CTA launch"
     ops.conv2d(xin, packs, outs, ress)
     torch.cuda.synchronize()

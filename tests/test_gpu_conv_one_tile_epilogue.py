@@ -3,35 +3,17 @@ tile in the ring stage after the last K block), vs the CPU oracle and the on-dev
 gather launches at BN = 64 and 128, ragged M tails, channel-slice outputs with a residual, and the launches that keep
 the staged-row epilogue (BN = 32, split-K, the row-statistics epilogue).  Every case asserts through icaf_conv2d_plan
 that it runs one tile per CTA."""
-import ctypes
-
 import pytest
 import torch
 
-from helpers import err, nchw, nhwc
+from helpers import conv_plan, err, nchw, nhwc, sm_count
 from test_gpu_conv import TOL, _mk, _ref
 
 pytestmark = pytest.mark.gpu
 
 
-def _plan(fn):
-    """The icaf_conv2d_plan of the one launch `fn` makes, on this device."""
-    from icafusion_b200 import _lib, ops
-    with ops.dry_run() as dr:
-        fn()
-    (_, _, work), = dr.records
-    pl = _lib.ConvPlan()
-    sms = torch.cuda.get_device_properties(torch.cuda.current_device()).multi_processor_count
-    assert _lib.lib().icaf_conv2d_plan(ctypes.byref(work["geom"]), work["n_io"], sms, 0, ctypes.byref(pl)) == 0
-    return pl
-
-
 def _one_tile(pl):
     return pl.ctas == pl.grid_x * pl.grid_y * pl.grid_z
-
-
-def _sms():
-    return torch.cuda.get_device_properties(torch.cuda.current_device()).multi_processor_count
 
 
 def _run(dev, B, Cin, H, W, Cout, k, s, p, act, resid, n_io, seed):
@@ -50,7 +32,7 @@ def _run(dev, B, Cin, H, W, Cout, k, s, p, act, resid, n_io, seed):
             ref = ref + r.float() if resid == "add" else 0.7 * r.float() + 1.25 * ref
         refs.append(ref)
     kw = dict(res=ress or None, scaled=[(coef[0:1], coef[1:2])] * n_io if resid == "scaled" else None)
-    pl = _plan(lambda: ops.conv2d(xs, packs, **kw))
+    pl = conv_plan(lambda: ops.conv2d(xs, packs, **kw))
     ys = ops.conv2d(xs, packs, **kw)
     ys_simt = ops.conv2d(xs, packs, simt=True, **kw)
     torch.cuda.synchronize()
@@ -90,7 +72,7 @@ def test_one_tile_epilogue(cuda_device, name):
 def test_one_tile_epilogue_bn128_single_wave(cuda_device, resid):
     """BN = 128 tiles that fit in one wave stay on the one-tile kernel: N = 192 (the last n-tile stores one 64-column half),
     a ragged M tail, both problems: m-tiles x 2 n-tiles x 2 problems = the SM count."""
-    mt = _sms() // 4
+    mt = sm_count() // 4
     ys, ys_simt, refs, pl = _run(cuda_device, 1, 64, 1, mt * 128 - 40, 192, 1, 1, 0, 1, resid, 2, seed=90)
     assert _one_tile(pl) and pl.bn == 128 and pl.cluster == 1, (pl.bn, pl.ctas, pl.cluster)
     _check(f"bn128_single_wave_{resid}", ys, ys_simt, refs)
@@ -114,7 +96,7 @@ def test_one_tile_epilogue_stem(cuda_device, H, W, n_io):
         packs.append(ops.pack_stem_weight(w.float(), b, 1, device=cuda_device))
         xs.append(ops.pack_image(x.to(cuda_device), s2d=True))
         refs.append(_ref(x, w, b, 2, 2, 1))
-    pl = _plan(lambda: ops.conv2d(xs, packs))
+    pl = conv_plan(lambda: ops.conv2d(xs, packs))
     assert _one_tile(pl) and pl.bn == 64 and pl.a_mode == 0 and pl.cluster == 1
     if (H, W) == (264, 264):
         assert pl.grid_x == 137
@@ -134,7 +116,7 @@ def test_one_tile_epilogue_channel_slice_residual(cuda_device):
     wide = torch.full((B, H, W, 3 * C), 7.0, dtype=torch.float16, device=cuda_device)
     pk = ops.pack_conv_weight(w.float(), b, 1, 1, 1, device=cuda_device)
     xd, rd, y = nhwc(x).to(cuda_device), nhwc(r).to(cuda_device), wide[..., C:2 * C]
-    pl = _plan(lambda: ops.conv2d([xd], [pk], [y], [rd]))
+    pl = conv_plan(lambda: ops.conv2d([xd], [pk], [y], [rd]))
     assert _one_tile(pl) and pl.bn == 64 and pl.a_mode == 2
     ops.conv2d([xd], [pk], [y], [rd])
     y_simt = ops.conv2d([xd], [pk], None, [rd], simt=True)[0]
@@ -158,12 +140,7 @@ def test_one_tile_epilogue_row_statistics(cuda_device):
                                      device=cuda_device))
     so = [torch.zeros(M, (N + 31) // 32, 2, device=cuda_device) for _ in range(n_io)]
     kw = dict(res=rs, scaled=[(al[0:1], al[1:2])] * n_io)
-    from icafusion_b200 import _lib
-    with ops.dry_run() as dr:
-        ops.linear(xs, packs, stats_out=so, **kw)
-    (_, _, work), = dr.records
-    pl = _lib.ConvPlan()
-    assert _lib.lib().icaf_conv2d_plan(ctypes.byref(work["geom"]), work["n_io"], _sms(), 0, ctypes.byref(pl)) == 0
+    pl = conv_plan(lambda: ops.linear(xs, packs, stats_out=so, **kw))
     assert _one_tile(pl) and pl.bn == 64
     ys = ops.linear(xs, packs, stats_out=so, **kw)
     ys_simt = ops.linear(xs, packs, simt=True, **kw)

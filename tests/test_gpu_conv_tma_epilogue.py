@@ -2,27 +2,13 @@
 tiles), vs the CPU oracle and the on-device CUDA-core reference: 2-D and 4-D output maps, stride 2, a partial last n-tile,
 channel-slice outputs, both residual forms, the per-row bias, every activation and grouped problems.  Every case asserts
 through icaf_conv2d_plan that it runs on the persistent kernel."""
-import ctypes
-
 import pytest
 import torch
 
-from helpers import err, nchw, nhwc
+from helpers import conv_plan, err, nchw, nhwc
 from test_gpu_conv import TOL, _mk, _ref
 
 pytestmark = pytest.mark.gpu
-
-
-def _plan(fn):
-    """The icaf_conv2d_plan of the one launch `fn` makes, on this device."""
-    from icafusion_b200 import _lib, ops
-    with ops.dry_run() as dr:
-        fn()
-    (_, _, work), = dr.records
-    pl = _lib.ConvPlan()
-    sms = torch.cuda.get_device_properties(torch.cuda.current_device()).multi_processor_count
-    assert _lib.lib().icaf_conv2d_plan(ctypes.byref(work["geom"]), work["n_io"], sms, 0, ctypes.byref(pl)) == 0
-    return pl
 
 
 def _persistent(pl):
@@ -61,7 +47,7 @@ def test_persistent_tma_epilogue(cuda_device, name):
             ref = ref + r.float() if resid == "add" else 0.7 * r.float() + 1.25 * ref
         refs.append(ref)
     kw = dict(res=ress or None, scaled=[(coef[0:1], coef[1:2])] * n_io if resid == "scaled" else None)
-    pl = _plan(lambda: ops.conv2d(xs, packs, **kw))
+    pl = conv_plan(lambda: ops.conv2d(xs, packs, **kw))
     assert _persistent(pl) and pl.a_mode == a_mode, f"expected a persistent launch with a_mode {a_mode}"
     ys = ops.conv2d(xs, packs, **kw)
     ys_simt = ops.conv2d(xs, packs, simt=True, **kw)
@@ -84,7 +70,7 @@ def test_persistent_tma_epilogue_channel_slice(cuda_device):
     out_wide = torch.zeros(B, H, W, 3 * C, dtype=torch.float16, device=cuda_device)
     pk = ops.pack_conv_weight(w.float(), b, 1, 0, 1, device=cuda_device)
     xin, y = wide_in[..., C:], out_wide[..., C:2 * C]
-    assert _persistent(_plan(lambda: ops.conv2d([xin], [pk], [y])))
+    assert _persistent(conv_plan(lambda: ops.conv2d([xin], [pk], [y])))
     ops.conv2d([xin], [pk], [y])
     y_simt = ops.conv2d([xin], [pk], simt=True)[0]
     torch.cuda.synchronize()
@@ -104,7 +90,7 @@ def test_persistent_tma_epilogue_bias_row(cuda_device):
     bv = torch.randn(C, generator=g)
     tok = ops.PackedConv(x.to(cuda_device), bv.to(cuda_device), K, rows, 1, 1, 1, 0, ops.ACT_NONE, is_weight=False)
     wd = wv.to(cuda_device)
-    assert _persistent(_plan(lambda: ops.linear([wd], [tok], bias_row=True)))
+    assert _persistent(conv_plan(lambda: ops.linear([wd], [tok], bias_row=True)))
     vt = ops.linear([wd], [tok], bias_row=True)[0]
     vt_simt = ops.linear([wd], [tok], bias_row=True, simt=True)[0]
     torch.cuda.synchronize()
@@ -122,7 +108,7 @@ def test_misaligned_output_pitch_takes_one_tile_kernel(cuda_device):
     out_wide = torch.zeros(B, H, W, N + 4, dtype=torch.float16, device=cuda_device)
     pk = ops.pack_conv_weight(w.float(), b, 1, 0, 1, device=cuda_device)
     xd, y = nhwc(x).to(cuda_device), out_wide[..., :N]
-    assert _persistent(_plan(lambda: ops.conv2d([xd], [pk], [y])))
+    assert _persistent(conv_plan(lambda: ops.conv2d([xd], [pk], [y])))
     ops.conv2d([xd], [pk], [y])
     torch.cuda.synchronize()
     assert err(nchw(y), _ref(x, w, b, 1, 0, 1)) < TOL
