@@ -35,6 +35,11 @@ class ConvPlan(C.Structure):
                                        "work_items", "ctas")]
 
 
+class BottleneckIO(C.Structure):
+    _fields_ = [("x", C.c_void_p), ("x_ld", C.c_int64), ("w1", C.c_void_p), ("b1", C.c_void_p), ("w3", C.c_void_p),
+                ("b2", C.c_void_p), ("y", C.c_void_p), ("y_ld", C.c_int64)]
+
+
 class LossHyp(C.Structure):
     _fields_ = [(n, C.c_float) for n in ("box", "obj", "cls", "cls_pw", "obj_pw", "anchor_t", "fl_gamma", "gr", "cp", "cn")] + \
                [("balance", C.c_float * 5)]
@@ -62,6 +67,7 @@ SIGNATURES = {
     "icaf_conv2d_fwd": [C.POINTER(ConvGeom), C.POINTER(ConvIO), _i, _vp],
     "icaf_conv2d_plan": [C.POINTER(ConvGeom), _i, _i, _i, C.POINTER(ConvPlan)],
     "icaf_conv2d_fwd_simt": [C.POINTER(ConvGeom), C.POINTER(ConvIO), _i, _vp],
+    "icaf_bottleneck_fwd": [_i, _i, _i, C.POINTER(BottleneckIO), _i, _vp],
     "icaf_pack_image": [_vp, _i, _f, _i, _i, _i, _vp, _vp],
     "icaf_pack_image_s2d": [_vp, _i, _f, _i, _i, _i, _vp, _vp],
     "icaf_letterbox": [_vp, _i, _i, _i, _vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _i, _vp],

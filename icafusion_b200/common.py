@@ -165,7 +165,30 @@ class Bottleneck(nn.Module):
         self.add = shortcut and c1 == c2
 
     @staticmethod
+    def fusable(mods, xs, outs=None) -> bool:
+        """The one-launch form (ops.bottleneck) applies: shortcut, 64 channels throughout, 16-byte aligned views, outputs
+        that share no storage with the inputs (its patches read x halos that neighbouring patches would overwrite), and
+        enough 4 x 32-pixel patches to give both consumer warpgroups of every SM of an H100 SXM (132 SMs) one."""
+        m0 = mods[0]
+        if not m0.add or m0.cv1.conv.in_channels != 64 or m0.cv1.conv.out_channels != 64 or m0.cv2.conv.kernel_size != (3, 3):
+            return False
+        B, H, W, _ = xs[0].shape
+        if len(xs) * B * ((H + 3) // 4) * ((W + 31) // 32) < 2 * 132:
+            return False
+        for m in mods:
+            _require_eval(m)
+        views = list(xs) + list(outs or [])
+        if any(t.shape[3] != 64 or t.stride(2) % 8 or (ops._addr(t) or 0) % 16 for t in views):
+            return False
+        stores = {t.untyped_storage()._cdata for t in xs}
+        return not any(t.untyped_storage()._cdata in stores for t in outs or [])
+
+    @staticmethod
     def run(mods, xs, outs=None):
+        if Bottleneck.fusable(mods, xs, outs):
+            p1s, p3s = [m.cv1.packed() for m in mods], [m.cv2.packed() for m in mods]
+            if all(p.act == ACT_SILU for p in p1s + p3s):
+                return ops.bottleneck(list(xs), p1s, p3s, outs)
         h = Conv.run([m.cv1 for m in mods], xs)
         return Conv.run([m.cv2 for m in mods], h, outs, list(xs) if mods[0].add else None)   # residual fused in the epilogue
 
@@ -215,7 +238,9 @@ class C3(nn.Module):
         a = left
         n = len(mods[0].m)
         for j in range(n):
-            # the last bottleneck writes back into the left half (its own residual read is element-wise, same thread)
+            # the last bottleneck writes back into the left half: with n = 1 that is its own input, which only the
+            # two-launch form allows (its residual read is element-wise, same thread); with n >= 2 it reads a scratch map
+            # and runs fused like the others
             a = Bottleneck.run([m.m[j] for m in mods], a, left if j == n - 1 else None)
         return Conv.run([m.cv3 for m in mods], cats, outs)
 

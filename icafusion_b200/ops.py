@@ -336,6 +336,40 @@ def linear(xs: Sequence[torch.Tensor], packs: Sequence[PackedConv], outs=None, r
     return [t[0, 0] for t in o]
 
 
+def bottleneck(xs: Sequence[torch.Tensor], p1s: Sequence[PackedConv], p3s: Sequence[PackedConv],
+               outs: Optional[Sequence[torch.Tensor]] = None) -> List[torch.Tensor]:
+    """Grouped (1 or 2 problems) Bottleneck with shortcut, 64 channels: y = x + cv2(cv1(x)) in one launch that keeps the
+    hidden map on chip (icaf_bottleneck_fwd).  p1s: the packed 1x1 SiLU cv1 filters, p3s: the packed 3x3 / pad 1 SiLU cv2
+    filters.  Outputs must not overlap the inputs."""
+    n = len(xs)
+    assert n in (1, 2) and len(p1s) == n and len(p3s) == n
+    B, H, W, Cx = xs[0].shape
+    for p1, p3 in zip(p1s, p3s):
+        if (p1.cin, p1.cout, p1.kh, p1.stride, p1.pad, p1.act, tuple(p1.w.shape)) != (64, 64, 1, 1, 0, ACT_SILU, (64, 64)) or \
+                (p3.cin, p3.cout, p3.kh, p3.kw, p3.stride, p3.pad, p3.act, tuple(p3.w.shape)) != (64, 64, 3, 3, 1, 1, ACT_SILU, (64, 576)) or \
+                p1.bias is None or p3.bias is None:
+            raise ValueError("bottleneck: needs a 64-channel 1x1 and a 3x3 / pad 1 filter, both with bias and SiLU")
+    if outs is None:
+        outs = [torch.empty(B, H, W, 64, dtype=torch.float16, device=xs[0].device) for _ in range(n)]
+    ios = (_lib.BottleneckIO * n)()
+    for i in range(n):
+        if tuple(xs[i].shape) != (B, H, W, 64) or tuple(outs[i].shape) != (B, H, W, 64):
+            raise ValueError(f"bottleneck: input {tuple(xs[i].shape)} / output {tuple(outs[i].shape)} must both be {(B, H, W, 64)}")
+        note_weight(p1s[i], "w")
+        note_weight(p3s[i], "w")
+        ios[i].x, ios[i].x_ld = _addr(xs[i]), _check_view(xs[i], "bottleneck input")
+        ios[i].y, ios[i].y_ld = _addr(outs[i]), _check_view(outs[i], "bottleneck output")
+        ios[i].w1, ios[i].b1 = _addr(p1s[i].w), _addr(p1s[i].bias)
+        ios[i].w3, ios[i].b2 = _addr(p3s[i].w), _addr(p3s[i].bias)
+    M = B * H * W
+    patches = B * ((H + 3) // 4) * ((W + 31) // 32)          # 4 x 32 output pixels each, cv1 recomputed on a 6 x 34 halo
+    work = {"tag": f"bottleneck M{M} C64 x{n}",
+            "flops": 2.0 * 64 * (6 * 34 * 64 + 128 * 9 * 64) * patches * n,
+            "bytes": 2.0 * n * (2 * M * 64 + 64 * 64 + 64 * 576)}
+    _call("icaf_bottleneck_fwd", _lib.lib().icaf_bottleneck_fwd, (B, H, W, ios, n), work)
+    return list(outs)
+
+
 def pack_stem_weight(weight: torch.Tensor, bias: Optional[torch.Tensor], act: int, device=None) -> "PackedConv":
     """(Cout,3,6,6) stride-2 pad-2 stem filter (BN folded) -> the equivalent 3x3 / stride 1 / pad 1 filter over the
     space-to-depth image (16 channels: (dy*2+dx)*4 + c), packed for the implicit-GEMM kernel.  ky = 2*ty+dy, kx = 2*tx+dx."""

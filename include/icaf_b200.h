@@ -120,6 +120,20 @@ int icaf_conv2d_plan(const icaf_conv_geom* g, int n_io, int sm_count, int pair_m
  * localise tensor-core bugs on the device.  Not called by the product path. */
 int icaf_conv2d_fwd_simt(const icaf_conv_geom* g, const icaf_conv_io* io, int n_io, void* stream);
 
+/* Fused Bottleneck with shortcut and 64 channels throughout (models/common.py:184-194, BN folded):
+ *   y = x + SiLU(conv3x3/p1(h) + b2),   h = SiLU(conv1x1(x) + b1)
+ * in one launch that keeps h on chip; the result equals icaf_conv2d_fwd of cv1 followed by that of cv2 with ADD_RES.
+ * `n_io` problems of identical geometry (B, H, W) per launch.  x and y are fp16 NHWC views of 64 channels (16-byte aligned,
+ * pitches multiples of 8); y must not overlap any x.  w1 / w3: the packed filters of icaf_conv2d_fwd (fp16 [64][64] and
+ * [64][576], K order (ky,kx,c)); b1 / b2: fp32 [64]. */
+typedef struct {
+  const void* x;     int64_t x_ld;
+  const void* w1;    const float* b1;
+  const void* w3;    const float* b2;
+  void* y;           int64_t y_ld;
+} icaf_bottleneck_io;
+int icaf_bottleneck_fwd(int B, int H, int W, const icaf_bottleneck_io* io, int n_io, void* stream);
+
 /* ---------------------------------------------------------------------------------------------
  * Input staging: (B,3,H,W) planar image -> fp16 NHWC with C padded to 4 (r,g,b,0).
  * Replaces the `.half()` / `/255` staging of detect_twostream.py:70-80 / train.py:295-297.

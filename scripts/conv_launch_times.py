@@ -4,13 +4,13 @@ Builds the detector the way bench.py does (seeded synthetic weights, BN folded, 
 on one stream with a CUDA event after every library launch (ops.profile).  Each pass is queued behind a spin kernel so the
 launches execute back to back; the L2 is flushed before each pass and every launch keeps its fastest of the passes.
 
-For every icaf_conv2d_fwd launch it prints the kernel the dispatcher picks (persist / one-tile), K, the tile count, the
+For every icaf_conv2d_fwd launch (and every fused Bottleneck launch, icaf_bottleneck_fwd) it prints the kernel the dispatcher picks (persist / one-tile), K, the tile count, the
 time, the achieved TFLOP/s and GB/s (algorithmic bytes: input + output + filter, + residual) and the roofline fraction:
 max(FLOPs / tensor peak, bytes / HBM peak) / time.  The launches are then summed per K class.  The peaks are the H100 SXM
 data-sheet figures (989 TFLOP/s dense FP16, 3.35 TB/s), which hold at 700 W; the card name and power limit are printed
 with the table.
 
-    python scripts/conv_launch_times.py [--batch 16] [--passes 3] [--csv out.csv]
+    python scripts/conv_launch_times.py [--batch 16] [--passes 3] [--csv out.csv] [--unfused]
 """
 from __future__ import annotations
 
@@ -52,6 +52,8 @@ def main():
     ap.add_argument("--batch", type=int, default=16)
     ap.add_argument("--passes", type=int, default=3)
     ap.add_argument("--csv", default=None, help="also write the per-launch table to this CSV file")
+    ap.add_argument("--unfused", action="store_true", help="run the 64-channel Bottlenecks as two conv launches each instead "
+                    "of the fused launch (icaf_bottleneck_fwd), to compare the two")
     args = ap.parse_args()
 
     import torch
@@ -60,6 +62,9 @@ def main():
     from icafusion_b200 import Model, _lib, ops, synth
     from icafusion_b200.synth import load_synth
 
+    if args.unfused:
+        from icafusion_b200 import common
+        common.Bottleneck.fusable = staticmethod(lambda mods, xs, outs=None: False)
     dev = torch.device("cuda:0")
     torch.cuda.set_device(dev)
     B, H, W = args.batch, 512, 640
@@ -89,18 +94,23 @@ def main():
     rows = []
     for i in range(per):
         name, work, _, _ = recs[i]
-        if name != "icaf_conv2d_fwd":
+        if name not in ("icaf_conv2d_fwd", "icaf_bottleneck_fwd"):
             continue
         ms = min(recs[r * per + i][2].elapsed_time(recs[r * per + i][3]) for r in range(args.passes))
+        fl, by = work["flops"], work["bytes"]
+        us = ms * 1e3
+        flop_us, hbm_us = fl / (PEAK_TFLOPS * 1e6), by / (PEAK_GBS * 1e3)
+        if name == "icaf_bottleneck_fwd":           # 1x1 (on the patch halo) + 3x3 + residual, 4 x 32-pixel patches
+            rows.append(dict(tag=work["tag"], kernel="fused", K=64 + 576, tiles=0, us=us, tflops=fl / (us * 1e-6) / 1e12,
+                             gbs=by / (us * 1e-6) / 1e9, frac=max(flop_us, hbm_us) / us, bound="flop" if flop_us >= hbm_us else "hbm",
+                             cls="fused bottleneck", flops=fl, bytes=by, bound_us=max(flop_us, hbm_us)))
+            continue
         pl = _lib.ConvPlan()
         if L.icaf_conv2d_plan(ctypes.byref(work["geom"]), work["n_io"], sms, 0, ctypes.byref(pl)) != 0:
             raise RuntimeError(L.icaf_last_error().decode())
         g = work["geom"]
         K = g.kh * g.kw * g.Cin
         persistent = pl.ctas < pl.grid_x * pl.grid_y * pl.grid_z
-        fl, by = work["flops"], work["bytes"]
-        us = ms * 1e3
-        flop_us, hbm_us = fl / (PEAK_TFLOPS * 1e6), by / (PEAK_GBS * 1e3)
         bound_us = max(flop_us, hbm_us)
         rows.append(dict(tag=work["tag"], kernel="persist" if persistent else "one-tile", K=K, tiles=pl.work_items, us=us,
                          tflops=fl / (us * 1e-6) / 1e12, gbs=by / (us * 1e-6) / 1e9, frac=bound_us / us,
@@ -117,7 +127,8 @@ def main():
               f"{r['gbs']:>7.0f} {r['bound']:>5} {r['frac']:>5.2f}")
     print()
     print(f"{'class':<20} {'launches':>8} {'GFLOP':>7} {'GB':>6} {'us':>8} {'bound us':>9} {'TFLOP/s':>8} {'GB/s':>6} {'frac':>5}")
-    classes = ["persist K <= 256", "persist K 257-1152", "persist K 1153-2047", "persist K >= 2048", "one-tile kernel", "all"]
+    classes = ["persist K <= 256", "persist K 257-1152", "persist K 1153-2047", "persist K >= 2048", "one-tile kernel",
+               "fused bottleneck", "all"]
     for c in classes:
         sel = [r for r in rows if c == "all" or r["cls"] == c]
         if not sel:
