@@ -25,6 +25,7 @@ struct AttnParams {
   const __half* vt[2];   // NULL in the fused-qkv form
   __half* out[2];
   int B, N, n_pad, C, heads;
+  int d;                 // head dim C / heads (the kernel runs width D >= d)
   int ld;                // row pitch of qk: 2C, or 3C in the fused-qkv form ([q | k | v])
   float p_drop;          // training forward only (TRAIN instantiation): dropout on the probabilities (common.py:677,680)
   uint32_t seed;
@@ -34,29 +35,28 @@ struct AttnParams {
 
 // ---------------------------------------------------------------------------------------------------
 // 288 threads: warps 0-7 two consumer warpgroups (queries 0-63 / 64-127 of the tile), warp 8 TMA producer.
-//   Q / K tiles: 2-D boxes (min(D,64) columns x 128 token rows) of the (B*Npad, 2C) projection matrix -> K-major rows of
-//                32 / 64 / 128 bytes with the matching swizzle (D = 128: two 64-column blocks)
-//   V^T tiles  : two boxes (64 keys x D feature rows) of the (C, B*Npad) matrix -> K-major SW128 (keys are the K dim of PV)
-//   V tiles    : (VF, fused [q|k|v] rows) boxes like K's at column 2C + head*D -> rows = keys, i.e. an MN-major B operand
-// Rows / keys past the tensor are zero-filled by the TMA unit; keys in [N, ...) are masked in the softmax.
-//
-// PAD: head dims d = 8 / 24 / 40 ... 120 (multiples of 8 that are not a power of two >= 16) run the kernel of the next width
-// D = 16 / 32 / 64 / 128 over 3-D maps that give every head its own extent, so columns d .. D-1 of a tile are out of
-// bounds and zero-filled instead of reading the next head:
-//   Q / K / V tiles: (d, k*heads, B*Npad) view of the projection matrix (k = 2 split, 3 fused), box (min(D,64), 1, rows)
-//   V^T tiles      : (B*Npad, d, heads) view of the (C, B*Npad) matrix, box (64, D, 1)
-// The zero columns add exactly 0 to S = Q K^T and produce zero columns of O = P V, which are not stored.
+// A head dim d (any multiple of 8 up to 128) runs the kernel of width D = 16 / 32 / 64 / 128, the smallest >= d.  Every
+// tile comes through a 3-D map that gives each head its own extent of d columns:
+//   Q / K tiles: (d, k*heads, B*Npad) view of the projection matrix (k = 2 split, 3 fused), box (min(D,64), 1, rows)
+//                -> K-major rows of 32 / 64 / 128 bytes with the matching swizzle (D = 128: two 64-column blocks)
+//   V tiles    : (VF, fused [q|k|v] rows) boxes like K's at projection 2 -> rows = keys, i.e. an MN-major B operand
+//   V^T tiles  : (B*Npad, d, heads) view of the (C, B*Npad) matrix, box (64, D, 1) -> K-major SW128 (keys are the K dim
+//                of PV)
+// Columns d .. D-1, rows past the tensor and keys past the tensor are zero-filled by the TMA unit; keys in [N, ...) are
+// masked in the softmax.  The zero columns add exactly 0 to S = Q K^T and produce zero columns of O = P V, which are not
+// stored.
 struct AttnMaps {
-  CUtensorMap qk[2];   // [0] = vis, [1] = ir : (B*Npad rows, 2C | 3C cols), box (min(D,64), 128) -- Q tiles
-  CUtensorMap kv[2];   // same matrices, box (min(D,64), KV) -- K tiles (and V tiles in the fused form)
-  CUtensorMap vt[2];   // split form: (C rows, B*Npad cols), box (64, D)
+  CUtensorMap qk[2];   // [0] = vis, [1] = ir : box (min(D,64), 1, 128) -- Q tiles
+  CUtensorMap kv[2];   // same views, box (min(D,64), 1, KV) -- K tiles (and V tiles in the fused form)
+  CUtensorMap vt[2];   // split form: V^T view, box (64, D, 1)
 };
 
-// KV = keys per tile (N of S, K of PV).  Head dims 16 / 32 run 64-key tiles (less masked work at the DMFF token counts).
-// The padded dropout kernel at D = 128 takes 64-key tiles too: with 128 it would spill, like the unpadded one does.
-template <int D, bool TRAIN = false, bool PAD = false>
+// KV = keys per tile (N of S, K of PV).  Head dims up to 32 run 64-key tiles (less masked work at the DMFF token counts).
+// The dropout kernel at D = 128 spills 48 bytes with 128-key tiles; 64-key tiles would change the rounding of yolov5l's
+// P5 training attention (d = 128).
+template <int D>
 struct AttnCfg {
-  static constexpr int kKV = D <= 32 || (TRAIN && PAD && D == 128) ? 64 : 128;
+  static constexpr int kKV = D <= 32 ? 64 : 128;
 };
 
 template <int D, int KV>
@@ -82,10 +82,9 @@ __device__ __forceinline__ float fast_exp2_t(float x) {
 
 // TRAIN: dropout on the attention probabilities (the row sum still runs over the un-dropped values, like
 // `att = softmax(..); att = attn_drop(att)`); its own instantiation, so the inference kernels keep their size.
-// PAD: the head dim C / heads is below D (see AttnMaps); its own instantiation too.
-template <int D, bool VF, bool TRAIN = false, bool PAD = false>
+template <int D, bool VF, bool TRAIN = false>
 __global__ void __launch_bounds__(288, 1) cross_attn_tma_kernel(const AttnParams P, const __grid_constant__ AttnMaps M) {
-  constexpr int kKV = AttnCfg<D, TRAIN, PAD>::kKV;
+  constexpr int kKV = AttnCfg<D>::kKV;
   using L = AttnSmemT<D, kKV>;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -204,7 +203,7 @@ __global__ void __launch_bounds__(288, 1) cross_attn_tma_kernel(const AttnParams
       l_run[h] += __shfl_xor_sync(0xffffffffu, l_run[h], 1);
       l_run[h] += __shfl_xor_sync(0xffffffffu, l_run[h], 2);
     }
-    const int d = PAD ? C / P.heads : D;      // true head dim: columns d .. D-1 of o are the zero padding
+    const int d = P.d;                        // true head dim: columns d .. D-1 of o are the zero padding
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const int qn = h ? qn1 : qn0;
@@ -213,7 +212,7 @@ __global__ void __launch_bounds__(288, 1) cross_attn_tma_kernel(const AttnParams
         __half* op = (dir == 0 ? P.out[0] : P.out[1]) + (size_t(b) * n_pad + qn) * C + head * d + 2 * (l & 3);
 #pragma unroll
         for (int i = 2 * h; i < D / 2; i += 4)
-          if (!PAD || 8 * (i >> 2) < d)
+          if (8 * (i >> 2) < d)
             *reinterpret_cast<uint32_t*>(op + 8 * (i >> 2)) = pack_half2(o[i] * inv, o[i + 1] * inv);
       }
     }
@@ -222,12 +221,10 @@ __global__ void __launch_bounds__(288, 1) cross_attn_tma_kernel(const AttnParams
     const CUtensorMap* mq = dir == 0 ? &M.qk[1] : &M.qk[0];
     const CUtensorMap* mk = dir == 0 ? &M.kv[0] : &M.kv[1];
     const CUtensorMap* mv = dir == 0 ? &M.vt[0] : &M.vt[1];
-    (void)mv;
     const int row_b = b * n_pad;
-    // a tile = (column block kb of projection k's head `head`, rows r0 ..): 2-D coordinates, or 3-D ones over the padded view
+    // a tile = (column block kb of projection k's head `head`, rows r0 ..)
     auto load_tile = [&](uint32_t dst, const CUtensorMap* m, uint32_t bar, int k, int kb, int r0) {
-      if (PAD) tma_load_3d(dst, m, bar, kb * 64, k * P.heads + head, r0);
-      else tma_load_2d(dst, m, bar, k * C + head * D + kb * 64, r0);
+      tma_load_3d(dst, m, bar, kb * 64, k * P.heads + head, r0);
     };
     mbar_arrive_expect_tx(q_full, L::kQBytes);      // overhanging boxes count in full: the zero fill arrives as bytes too
 #pragma unroll
@@ -246,10 +243,8 @@ __global__ void __launch_bounds__(288, 1) cross_attn_tma_kernel(const AttnParams
           load_tile(sbase + L::kVOff + buf * L::kVBytes + kb * (kKV * 128), mk, kv_full(buf), 2, kb, row_b + j * kKV);
       } else {
 #pragma unroll
-        for (int kb = 0; kb < kKV / 64; ++kb) {
-          if (PAD) tma_load_3d(sbase + L::kVOff + buf * L::kVBytes + kb * (D * 128), mv, kv_full(buf), row_b + j * kKV + kb * 64, 0, head);
-          else tma_load_2d(sbase + L::kVOff + buf * L::kVBytes + kb * (D * 128), mv, kv_full(buf), row_b + j * kKV + kb * 64, head * D);
-        }
+        for (int kb = 0; kb < kKV / 64; ++kb)
+          tma_load_3d(sbase + L::kVOff + buf * L::kVBytes + kb * (D * 128), mv, kv_full(buf), row_b + j * kKV + kb * 64, 0, head);
       }
     }
   }
@@ -311,65 +306,45 @@ static int fill_attn(const void* qk_vis, const void* qk_ir, const void* vt_vis, 
   P.qk[0] = (const __half*)qk_vis; P.qk[1] = (const __half*)qk_ir;
   P.vt[0] = (const __half*)vt_vis; P.vt[1] = (const __half*)vt_ir;
   P.out[0] = (__half*)out_vis; P.out[1] = (__half*)out_ir;
-  P.B = B; P.N = N; P.n_pad = n_pad; P.C = C; P.heads = heads;
+  P.B = B; P.N = N; P.n_pad = n_pad; P.C = C; P.heads = heads; P.d = d;
   P.ld = vt_vis ? 2 * C : 3 * C;
   P.p_drop = 0.f; P.seed = 0u; P.seed_off = nullptr;
   P.scale_log2 = 1.4426950408889634f / sqrtf(float(d));   // 1/sqrt(d_k), common.py:670
   return ICAF_OK;
 }
 
-template <int D, bool VF, bool TRAIN = false, bool PAD = false>
+template <int D, bool VF, bool TRAIN = false>
 static int launch_attn_tma(const AttnParams& P, cudaStream_t st) {
-  constexpr int kKV = AttnCfg<D, TRAIN, PAD>::kKV;
+  constexpr int kKV = AttnCfg<D>::kKV;
   using L = AttnSmemT<D, kKV>;
   static bool configured[kMaxDevices] = {false};
-  if (int rc = configure_smem(cross_attn_tma_kernel<D, VF, TRAIN, PAD>, L::kTotal, configured, "cross_attention: cudaFuncSetAttribute")) return rc;
+  if (int rc = configure_smem(cross_attn_tma_kernel<D, VF, TRAIN>, L::kTotal, configured, "cross_attention: cudaFuncSetAttribute")) return rc;
   AttnMaps maps;
   memset(&maps, 0, sizeof(maps));
   const uint64_t rows = uint64_t(P.B) * P.n_pad;
-  const uint64_t d = uint64_t(P.C / P.heads);
+  const uint64_t d = uint64_t(P.d);
   const uint32_t bw = D < 64 ? D : 64;
+  const uint64_t dims[3] = {d, uint64_t(P.ld / d), rows};       // (head column, projection * heads + head, token)
+  const uint64_t vdims[3] = {rows, d, uint64_t(P.heads)};       // (token, head row, head)
   for (int i = 0; i < 2; ++i) {
-    int rc;
-    if (PAD) {
-      const uint64_t dims[3] = {d, uint64_t(P.ld / d), rows};       // (head column, projection * heads + head, token)
-      rc = encode_tmap_3d(&maps.qk[i], P.qk[i], dims, d * 2, uint64_t(P.ld) * 2, {bw, 1u, uint32_t(kQT)});
-      if (!rc) rc = encode_tmap_3d(&maps.kv[i], P.qk[i], dims, d * 2, uint64_t(P.ld) * 2, {bw, 1u, uint32_t(kKV)});
-      if (!rc && !VF) {
-        const uint64_t vdims[3] = {rows, d, uint64_t(P.heads)};       // (token, head row, head)
-        rc = encode_tmap_3d(&maps.vt[i], P.vt[i], vdims, rows * 2, rows * 2 * d, {64u, uint32_t(D), 1u});
-      }
-      if (rc) return rc;
-      continue;
-    }
-    rc = encode_tmap_2d(&maps.qk[i], P.qk[i], uint64_t(P.ld), rows, uint64_t(P.ld) * 2, bw, kQT);
+    int rc = encode_tmap_3d(&maps.qk[i], P.qk[i], dims, d * 2, uint64_t(P.ld) * 2, {bw, 1u, uint32_t(kQT)});
+    if (!rc) rc = encode_tmap_3d(&maps.kv[i], P.qk[i], dims, d * 2, uint64_t(P.ld) * 2, {bw, 1u, uint32_t(kKV)});
+    if (!rc && !VF) rc = encode_tmap_3d(&maps.vt[i], P.vt[i], vdims, rows * 2, rows * 2 * d, {64u, uint32_t(D), 1u});
     if (rc) return rc;
-    rc = encode_tmap_2d(&maps.kv[i], P.qk[i], uint64_t(P.ld), rows, uint64_t(P.ld) * 2, bw, kKV);
-    if (rc) return rc;
-    if (!VF) {
-      rc = encode_tmap_2d(&maps.vt[i], P.vt[i], rows, uint64_t(P.C), rows * 2, 64, D);
-      if (rc) return rc;
-    }
   }
   dim3 grid((P.n_pad + kQT - 1) / kQT, P.B * P.heads, 2);
-  launch_k(cross_attn_tma_kernel<D, VF, TRAIN, PAD>, dim3(grid), dim3(288), L::kTotal, st, P, maps);
+  launch_k(cross_attn_tma_kernel<D, VF, TRAIN>, dim3(grid), dim3(288), L::kTotal, st, P, maps);
   return check_launch("cross_attention");
 }
 
-// Head dims 16 / 32 / 64 / 128 run their own width; every other multiple of 8 runs the next one up, padded.
+// A head dim d runs the kernel of the smallest width D >= d; columns d .. D-1 are zero-filled (see AttnMaps).
 template <bool VF, bool TRAIN = false>
 static int dispatch_attn(const AttnParams& P, cudaStream_t st) {
-  const int d = P.C / P.heads;
-  switch (d) {
-    case 16: return launch_attn_tma<16, VF, TRAIN>(P, st);
-    case 32: return launch_attn_tma<32, VF, TRAIN>(P, st);
-    case 64: return launch_attn_tma<64, VF, TRAIN>(P, st);
-    case 128: return launch_attn_tma<128, VF, TRAIN>(P, st);
-  }
-  if (d < 16) return launch_attn_tma<16, VF, TRAIN, true>(P, st);
-  if (d < 32) return launch_attn_tma<32, VF, TRAIN, true>(P, st);
-  if (d < 64) return launch_attn_tma<64, VF, TRAIN, true>(P, st);
-  return launch_attn_tma<128, VF, TRAIN, true>(P, st);
+  const int d = P.d;
+  if (d <= 16) return launch_attn_tma<16, VF, TRAIN>(P, st);
+  if (d <= 32) return launch_attn_tma<32, VF, TRAIN>(P, st);
+  if (d <= 64) return launch_attn_tma<64, VF, TRAIN>(P, st);
+  return launch_attn_tma<128, VF, TRAIN>(P, st);
 }
 
 }  // namespace icaf
