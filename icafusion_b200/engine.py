@@ -13,7 +13,7 @@ from typing import Iterable, Iterator, Optional, Tuple
 
 import torch
 
-from . import _lib, ops
+from . import ops
 from .yolo_test import Model
 
 
@@ -63,7 +63,7 @@ class GraphedDetector:
             if nms is not None:                         # static NMS buffers live outside the graph's private pool
                 z0 = self.model(self.rgb, self.ir)[0]
                 self.det, self.count = ops.nms(z0, **nms)
-                need = int(_lib.lib().icaf_nms_workspace_bytes(z0.shape[0], z0.shape[1]))
+                need = ops.nms_workspace_bytes(*z0.shape, nms.get("multi_label", False))
                 self._nms_ws = torch.empty((need + 7) // 8, dtype=torch.int64, device=self.device)
                 self.stream.synchronize()
             self.graph = torch.cuda.CUDAGraph()

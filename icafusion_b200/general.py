@@ -27,16 +27,13 @@ def xywh2xyxy(x: torch.Tensor) -> torch.Tensor:
 def non_max_suppression(prediction: torch.Tensor, conf_thres: float = 0.25, iou_thres: float = 0.45,
                         classes: Optional[Sequence[int]] = None, agnostic: bool = False, multi_label: bool = False,
                         labels=()) -> List[torch.Tensor]:
-    """reference: utils/general.py:518-607.  Returns a list with one (n,6) fp32 tensor [xyxy, conf, cls] per image."""
-    nc = prediction.shape[2] - 5
-    if multi_label and nc > 1:
-        raise NotImplementedError("non_max_suppression: the multi-label branch (nc > 1) is not built; the KAIST / LLVIP "
-                                  "configurations are single-class, where the reference switches it off itself (general.py:533)")
+    """reference: utils/general.py:518-607.  Returns a list with one (n,6) fp32 tensor [xyxy, conf, cls] per image.
+    `multi_label` (test.py:139) keeps every (box, class) pair above conf_thres; it is off when nc == 1, as in the reference."""
     if labels:
         raise NotImplementedError("non_max_suppression: autolabelling (labels=...) is outside the hot path built here")
     if not prediction.is_cuda:
         raise RuntimeError("icafusion_b200 runs on CUDA tensors only (no CPU fallback)")
     z = prediction if prediction.dtype == torch.float16 else prediction.to(torch.float16)
-    det, count = ops.nms(z.contiguous(), conf_thres, iou_thres, agnostic, classes)
+    det, count = ops.nms(z.contiguous(), conf_thres, iou_thres, agnostic, classes, multi_label=multi_label)
     counts = count.tolist()                       # the one host sync of the list-shaped API
     return [det[i, :n] for i, n in enumerate(counts)]

@@ -600,11 +600,20 @@ def axpby(x: torch.Tensor, a: torch.Tensor, y: Optional[torch.Tensor] = None, b:
     return out
 
 
+def nms_workspace_bytes(B: int, R: int, no: int, multi_label: bool = False) -> int:
+    """Device workspace :func:`nms` needs for a (B, R, no) prediction tensor (multi_label only counts when nc = no - 5 > 1)."""
+    if multi_label and no - 5 > 1:
+        return int(_lib.lib().icaf_nms_multi_label_workspace_bytes(B, R, no))
+    return int(_lib.lib().icaf_nms_workspace_bytes(B, R))
+
+
 def nms(z: torch.Tensor, conf_thres: float = 0.25, iou_thres: float = 0.45, agnostic: bool = False,
         classes: Optional[Sequence[int]] = None, max_det: int = 300, det: Optional[torch.Tensor] = None,
-        count: Optional[torch.Tensor] = None, workspace: Optional[torch.Tensor] = None):
-    """Batched NMS on the device (utils/general.py:518-607, best-class branch).  z: fp16 (B, R, nc+5) decoded predictions.
-    Returns (det fp32 (B, max_det, 6) rows [x1,y1,x2,y2,conf,cls] in confidence order, count int32 (B,)); no host sync."""
+        count: Optional[torch.Tensor] = None, workspace: Optional[torch.Tensor] = None, multi_label: bool = False):
+    """Batched NMS on the device (utils/general.py:518-607).  z: fp16 (B, R, nc+5) decoded predictions.  `multi_label`
+    (test.py's setting) keeps one candidate per (row, class) above the threshold; like the reference it only applies when
+    nc > 1.  Returns (det fp32 (B, max_det, 6) rows [x1,y1,x2,y2,conf,cls] in confidence order, count int32 (B,)); no host
+    sync.  `workspace` must hold :func:`nms_workspace_bytes` bytes."""
     if z.dim() != 3 or z.dtype != torch.float16 or not on_device(z) or not z.is_contiguous():
         raise ValueError(f"nms: expected a contiguous CUDA fp16 (B, R, nc+5) tensor, got {z.dtype} {tuple(z.shape)}")
     B, R, no = z.shape
@@ -620,12 +629,14 @@ def nms(z: torch.Tensor, conf_thres: float = 0.25, iou_thres: float = 0.45, agno
         det = torch.zeros(B, max_det, 6, dtype=torch.float32, device=z.device)
     if count is None:
         count = torch.zeros(B, dtype=torch.int32, device=z.device)
-    need = int(_lib.lib().icaf_nms_workspace_bytes(B, R))
+    multi_label = bool(multi_label) and no - 5 > 1
+    need = nms_workspace_bytes(B, R, no, multi_label)
     if workspace is None:
         workspace = torch.empty((need + 7) // 8, dtype=torch.int64, device=z.device)
     if tuple(det.shape) != (B, max_det, 6) or det.dtype != torch.float32 or tuple(count.shape) != (B,) or count.dtype != torch.int32:
         raise ValueError("nms: det must be fp32 (B, max_det, 6) and count int32 (B,)")
-    _call("icaf_nms", _lib.lib().icaf_nms,
+    name = "icaf_nms_multi_label" if multi_label else "icaf_nms"
+    _call(name, getattr(_lib.lib(), name),
           (_ptr(z), B, R, no, float(conf_thres), float(iou_thres), int(bool(agnostic)), C.c_uint64(mask), int(max_det), _ptr(det), _ptr(count),
            _ptr(workspace), C.c_size_t(workspace.numel() * workspace.element_size())), {"bytes": 2.0 * z.numel()})
     return det, count

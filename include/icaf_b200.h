@@ -233,6 +233,17 @@ size_t icaf_nms_workspace_bytes(int B, int R);
 int icaf_nms(const void* z, int B, int R, int no, float conf_thres, float iou_thres, int agnostic, uint64_t class_mask,
              int max_det, float* det, int* count, void* workspace, size_t workspace_bytes, void* stream);
 
+/* Multi-label branch of the same function (utils/general.py:566-568, what test.py:139 asks for): one candidate per
+ * (row, class j) with obj > conf_thres and cls_j * obj > conf_thres (class_mask applies per pair), sorted by descending
+ * confidence with ties in (row * nc + j) order, cut to the first max_nms = 30000, then the same suppression.  A box may be
+ * kept once per class (once in all unless `agnostic`).  det rows [x1, y1, x2, y2, cls_j * obj, j].  Same arguments as
+ * icaf_nms; workspace: icaf_nms_multi_label_workspace_bytes(B, R, no) bytes (16 per row and class), 8-byte aligned;
+ * R * (no - 5) must fit in int.  Returns 0 from the size query for a bad shape. */
+size_t icaf_nms_multi_label_workspace_bytes(int B, int R, int no);
+int icaf_nms_multi_label(const void* z, int B, int R, int no, float conf_thres, float iou_thres, int agnostic,
+                         uint64_t class_mask, int max_det, float* det, int* count, void* workspace, size_t workspace_bytes,
+                         void* stream);
+
 /* ---------------------------------------------------------------------------------------------
  * Detection loss, forward only (the validation loss test.py:132-133 accumulates; the training backward is not built):
  * utils/loss.py:325-463 ComputeLoss.__call__ + build_targets -- anchor-ratio matching with the four half-cell neighbour
