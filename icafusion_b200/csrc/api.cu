@@ -17,11 +17,6 @@ int set_cuda_error(cudaError_t e, const char* where) {
   snprintf(g_err, sizeof(g_err), "%s: %s (%s)", where, cudaGetErrorString(e), cudaGetErrorName(e));
   return ICAF_ERR_CUDA;
 }
-int check_launch(const char* where) {
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return set_cuda_error(e, where);
-  return ICAF_OK;
-}
 bool pdl_enabled() {
   static int v = -1;
   if (v < 0) {
@@ -73,69 +68,53 @@ static std::atomic<long long> g_launches{0};
 void count_launch() { g_launches.fetch_add(1, std::memory_order_relaxed); }
 long long launches_so_far() { return g_launches.load(std::memory_order_relaxed); }
 
-int encode_tmap_2d(CUtensorMap* out, const void* base, uint64_t inner, uint64_t rows, uint64_t row_pitch_bytes,
-                   uint32_t box_inner, uint32_t box_rows) {
+// The one cuTensorMapEncodeTiled call behind the encoders below: fp16, no interleave, zero fill out of bounds.  Staged rows
+// are box[0] halfs wide and the swizzle span equals the row (64 / 32 / 16 halfs -> 128 / 64 / 32 B); the L2 promotion
+// follows the innermost row and its pitch (strides[0]).
+static int encode_tmap(CUtensorMap* out, const void* base, cuuint32_t rank, const cuuint64_t* dims, const cuuint64_t* strides,
+                       const cuuint32_t* box, const cuuint32_t* estr) {
   EncodeTiledFn fn = encode_fn();
   if (!fn) return set_error(ICAF_ERR_CUDA, "cuTensorMapEncodeTiled entry point not available");
-  cuuint64_t dims[2] = {inner, rows};
-  cuuint64_t strides[1] = {row_pitch_bytes};
-  cuuint32_t box[2] = {box_inner, box_rows};
-  cuuint32_t estr[2] = {1, 1};
-  // staged rows are box_inner*2 bytes wide; the swizzle span equals the row (32 / 64 / 128 B)
-  const CUtensorMapSwizzle swz = box_inner >= 64 ? CU_TENSOR_MAP_SWIZZLE_128B : (box_inner == 32 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B);
-  CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(base), dims, strides, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, swz, l2_promotion(inner * 2, row_pitch_bytes),
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  const CUtensorMapSwizzle swz = box[0] >= 64 ? CU_TENSOR_MAP_SWIZZLE_128B : (box[0] == 32 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B);
+  CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, rank, const_cast<void*>(base), dims, strides, box, estr,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, swz, l2_promotion(dims[0] * 2, strides[0]), CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
-    char msg[160];
-    snprintf(msg, sizeof(msg), "cuTensorMapEncodeTiled(2d inner=%llu rows=%llu pitch=%llu box=%ux%u) failed: %d",
-             (unsigned long long)inner, (unsigned long long)rows, (unsigned long long)row_pitch_bytes, box_inner, box_rows, int(r));
+    char msg[512];      // room for four dimensions of 64-bit sizes and pitches
+    int n = snprintf(msg, sizeof(msg), "cuTensorMapEncodeTiled(%ud, size/pitch/box/step per dim:", rank);
+    for (cuuint32_t i = 0; i < rank; ++i)
+      n += snprintf(msg + n, sizeof(msg) - n, " %llu/%lluB/%u/%u", (unsigned long long)dims[i], i ? (unsigned long long)strides[i - 1] : 2ull,
+                    box[i], estr[i]);
+    snprintf(msg + n, sizeof(msg) - n, ") failed: %d", int(r));
     return set_error(ICAF_ERR_CUDA, msg);
   }
   return ICAF_OK;
+}
+
+int encode_tmap_2d(CUtensorMap* out, const void* base, uint64_t inner, uint64_t rows, uint64_t row_pitch_bytes,
+                   uint32_t box_inner, uint32_t box_rows) {
+  const cuuint64_t dims[2] = {inner, rows};
+  const cuuint64_t strides[1] = {row_pitch_bytes};
+  const cuuint32_t box[2] = {box_inner, box_rows};
+  const cuuint32_t estr[2] = {1, 1};
+  return encode_tmap(out, base, 2, dims, strides, box, estr);
 }
 
 int encode_tmap_3d(CUtensorMap* out, const void* base, const uint64_t (&dims)[3], uint64_t pitch1_bytes, uint64_t pitch2_bytes,
                    const uint32_t (&box)[3]) {
-  EncodeTiledFn fn = encode_fn();
-  if (!fn) return set_error(ICAF_ERR_CUDA, "cuTensorMapEncodeTiled entry point not available");
-  cuuint64_t gdims[3] = {dims[0], dims[1], dims[2]};
-  cuuint64_t strides[2] = {pitch1_bytes, pitch2_bytes};
-  cuuint32_t gbox[3] = {box[0], box[1], box[2]};
-  cuuint32_t estr[3] = {1, 1, 1};
-  const CUtensorMapSwizzle swz = box[0] >= 64 ? CU_TENSOR_MAP_SWIZZLE_128B : (box[0] == 32 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B);
-  CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, const_cast<void*>(base), gdims, strides, gbox, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, swz, l2_promotion(dims[0] * 2, pitch1_bytes), CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    char msg[200];
-    snprintf(msg, sizeof(msg), "cuTensorMapEncodeTiled(3d dims=%llu,%llu,%llu pitch=%llu,%llu box=%u,%u,%u) failed: %d",
-             (unsigned long long)dims[0], (unsigned long long)dims[1], (unsigned long long)dims[2], (unsigned long long)pitch1_bytes,
-             (unsigned long long)pitch2_bytes, box[0], box[1], box[2], int(r));
-    return set_error(ICAF_ERR_CUDA, msg);
-  }
-  return ICAF_OK;
+  const cuuint64_t gdims[3] = {dims[0], dims[1], dims[2]};
+  const cuuint64_t strides[2] = {pitch1_bytes, pitch2_bytes};
+  const cuuint32_t gbox[3] = {box[0], box[1], box[2]};
+  const cuuint32_t estr[3] = {1, 1, 1};
+  return encode_tmap(out, base, 3, gdims, strides, gbox, estr);
 }
 
 int encode_tmap_nhwc(CUtensorMap* out, const void* base, int C, int W, int H, int B, int64_t ld, uint32_t box_c,
                      uint32_t box_w, uint32_t box_h, uint32_t sw, uint32_t sh) {
-  EncodeTiledFn fn = encode_fn();
-  if (!fn) return set_error(ICAF_ERR_CUDA, "cuTensorMapEncodeTiled entry point not available");
-  cuuint64_t dims[4] = {cuuint64_t(C), cuuint64_t(W), cuuint64_t(H), cuuint64_t(B)};
-  cuuint64_t strides[3] = {cuuint64_t(ld) * 2, cuuint64_t(ld) * 2 * W, cuuint64_t(ld) * 2 * W * H};
-  cuuint32_t box[4] = {box_c, box_w, box_h, 1};
-  cuuint32_t estr[4] = {1, sw, sh, 1};
-  // rows of the staged tile are box_c*2 bytes wide; the swizzle span equals the row (32 / 64 / 128 B)
-  const CUtensorMapSwizzle swz = box_c >= 64 ? CU_TENSOR_MAP_SWIZZLE_128B : (box_c == 32 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B);
-  CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(base), dims, strides, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, swz, l2_promotion(uint64_t(C) * 2, uint64_t(ld) * 2),
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    char msg[200];
-    snprintf(msg, sizeof(msg), "cuTensorMapEncodeTiled(nhwc C=%d W=%d H=%d B=%d ld=%lld box=%u,%u,%u stride=%u,%u) failed: %d", C, W, H, B,
-             (long long)ld, box_c, box_w, box_h, sw, sh, int(r));
-    return set_error(ICAF_ERR_CUDA, msg);
-  }
-  return ICAF_OK;
+  const cuuint64_t dims[4] = {cuuint64_t(C), cuuint64_t(W), cuuint64_t(H), cuuint64_t(B)};
+  const cuuint64_t strides[3] = {cuuint64_t(ld) * 2, cuuint64_t(ld) * 2 * W, cuuint64_t(ld) * 2 * W * H};
+  const cuuint32_t box[4] = {box_c, box_w, box_h, 1};
+  const cuuint32_t estr[4] = {1, sw, sh, 1};
+  return encode_tmap(out, base, 4, dims, strides, box, estr);
 }
 
 }  // namespace icaf

@@ -332,9 +332,8 @@ static int launch_attn_tma(const AttnParams& P, cudaStream_t st) {
     if (!rc && !VF) rc = encode_tmap_3d(&maps.vt[i], P.vt[i], vdims, rows * 2, rows * 2 * d, {64u, uint32_t(D), 1u});
     if (rc) return rc;
   }
-  dim3 grid((P.n_pad + kQT - 1) / kQT, P.B * P.heads, 2);
-  launch_k(cross_attn_tma_kernel<D, VF, TRAIN>, dim3(grid), dim3(288), L::kTotal, st, P, maps);
-  return check_launch("cross_attention");
+  dim3 grid(blocks_for(P.n_pad, kQT), P.B * P.heads, 2);
+  return launch_k("cross_attention", cross_attn_tma_kernel<D, VF, TRAIN>, dim3(grid), dim3(288), L::kTotal, st, P, maps);
 }
 
 // A head dim d runs the kernel of the smallest width D >= d; columns d .. D-1 are zero-filled (see AttnMaps).
@@ -383,6 +382,5 @@ extern "C" int icaf_cross_attention_simt(const void* qk_vis, const void* qk_ir, 
   int rc = fill_attn(qk_vis, qk_ir, vt_vis, vt_ir, out_vis, out_ir, B, N, n_pad, C, heads, P);
   if (rc) return rc;
   long long total = 2LL * B * heads * n_pad;
-  launch_k(cross_attn_simt_kernel, dim3((unsigned)((total + 127) / 128)), dim3(128), 0, (cudaStream_t)stream, P);
-  return check_launch("cross_attention_simt");
+  return launch_k("cross_attention_simt", cross_attn_simt_kernel, dim3(blocks_for(total, 128)), dim3(128), 0, (cudaStream_t)stream, P);
 }

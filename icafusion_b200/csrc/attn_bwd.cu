@@ -200,12 +200,6 @@ __global__ void __launch_bounds__(kBT) attn_bwd_kv_kernel(const AttnBwdParams P)
 // so the inner loops are FMA-bound instead of shared-memory-load-bound (two LDS per FMA in the kernels above).
 constexpr int kT2 = 64;    // rows of the other side staged per tile
 
-__device__ __forceinline__ void cvt8(const uint4& u, float (&f)[8]) {
-  const __half2* h = reinterpret_cast<const __half2*>(&u);
-#pragma unroll
-  for (int i = 0; i < 4; ++i) { const float2 t = __half22float2(h[i]); f[2 * i] = t.x; f[2 * i + 1] = t.y; }
-}
-
 template <int D>
 __global__ void __launch_bounds__(kBT) attn_bwd_q_reg_kernel(const AttnBwdParams P) {
   pdl_launch_dependents();
@@ -228,9 +222,9 @@ __global__ void __launch_bounds__(kBT) attn_bwd_q_reg_kernel(const AttnBwdParams
   for (int c8 = 0; c8 < D / 8; ++c8) {
     float a[8], g[8], o[8];
     const uint4 z4 = make_uint4(0, 0, 0, 0);
-    cvt8(valid ? __ldg(reinterpret_cast<const uint4*>(qsrc + size_t(i) * ld) + c8) : z4, a);
-    cvt8(valid ? __ldg(reinterpret_cast<const uint4*>(dsrc + size_t(i) * P.C) + c8) : z4, g);
-    cvt8(valid ? __ldg(reinterpret_cast<const uint4*>(osrc + size_t(i) * P.C) + c8) : z4, o);
+    unpack8(valid ? __ldg(reinterpret_cast<const uint4*>(qsrc + size_t(i) * ld) + c8) : z4, a);
+    unpack8(valid ? __ldg(reinterpret_cast<const uint4*>(dsrc + size_t(i) * P.C) + c8) : z4, g);
+    unpack8(valid ? __ldg(reinterpret_cast<const uint4*>(osrc + size_t(i) * P.C) + c8) : z4, o);
 #pragma unroll
     for (int e = 0; e < 8; ++e) { q[c8 * 8 + e] = a[e] * P.scale_log2; d_o[c8 * 8 + e] = g[e]; dq[c8 * 8 + e] = 0.f; delta += g[e] * o[e]; }
   }
@@ -249,7 +243,7 @@ __global__ void __launch_bounds__(kBT) attn_bwd_q_reg_kernel(const AttnBwdParams
 #pragma unroll
       for (int c8 = 0; c8 < D / 8; ++c8) {
         float kf[8];
-        cvt8(reinterpret_cast<const uint4*>(kt + j * D)[c8], kf);
+        unpack8(reinterpret_cast<const uint4*>(kt + j * D)[c8], kf);
 #pragma unroll
         for (int e = 0; e < 8; ++e) s = fmaf(q[c8 * 8 + e], kf[e], s);
       }
@@ -281,8 +275,8 @@ __global__ void __launch_bounds__(kBT) attn_bwd_q_reg_kernel(const AttnBwdParams
 #pragma unroll
       for (int c8 = 0; c8 < D / 8; ++c8) {
         float kf[8], vf[8];
-        cvt8(reinterpret_cast<const uint4*>(kt + j * D)[c8], kf);
-        cvt8(reinterpret_cast<const uint4*>(vt + j * D)[c8], vf);
+        unpack8(reinterpret_cast<const uint4*>(kt + j * D)[c8], kf);
+        unpack8(reinterpret_cast<const uint4*>(vt + j * D)[c8], vf);
 #pragma unroll
         for (int e = 0; e < 8; ++e) { s = fmaf(q[c8 * 8 + e], kf[e], s); dp = fmaf(d_o[c8 * 8 + e], vf[e], dp); }
       }
@@ -292,7 +286,7 @@ __global__ void __launch_bounds__(kBT) attn_bwd_q_reg_kernel(const AttnBwdParams
 #pragma unroll
       for (int c8 = 0; c8 < D / 8; ++c8) {
         float kf[8];
-        cvt8(reinterpret_cast<const uint4*>(kt + j * D)[c8], kf);
+        unpack8(reinterpret_cast<const uint4*>(kt + j * D)[c8], kf);
 #pragma unroll
         for (int e = 0; e < 8; ++e) dq[c8 * 8 + e] = fmaf(ds, kf[e], dq[c8 * 8 + e]);
       }
@@ -361,8 +355,8 @@ __global__ void __launch_bounds__(kBT) attn_bwd_kv_reg_kernel(const AttnBwdParam
 #pragma unroll
       for (int c8 = 0; c8 < D / 8; ++c8) {
         float qf[8], gf[8];
-        cvt8(reinterpret_cast<const uint4*>(qt + i * D)[c8], qf);
-        cvt8(reinterpret_cast<const uint4*>(dt + i * D)[c8], gf);
+        unpack8(reinterpret_cast<const uint4*>(qt + i * D)[c8], qf);
+        unpack8(reinterpret_cast<const uint4*>(dt + i * D)[c8], gf);
 #pragma unroll
         for (int e = 0; e < 4; ++e) {
           const float2 k2 = __half22float2(kh[c8 * 4 + e]), v2 = __half22float2(vh[c8 * 4 + e]);
@@ -381,8 +375,8 @@ __global__ void __launch_bounds__(kBT) attn_bwd_kv_reg_kernel(const AttnBwdParam
 #pragma unroll
       for (int c8 = 0; c8 < D / 8; ++c8) {
         float qf[8], gf[8];
-        cvt8(reinterpret_cast<const uint4*>(qt + i * D)[c8], qf);
-        cvt8(reinterpret_cast<const uint4*>(dt + i * D)[c8], gf);
+        unpack8(reinterpret_cast<const uint4*>(qt + i * D)[c8], qf);
+        unpack8(reinterpret_cast<const uint4*>(dt + i * D)[c8], gf);
 #pragma unroll
         for (int e = 0; e < 8; ++e) { dk[c8 * 8 + e] = fmaf(ds, qf[e], dk[c8 * 8 + e]); dv[c8 * 8 + e] = fmaf(pd, gf[e], dv[c8 * 8 + e]); }
       }
@@ -403,18 +397,16 @@ template <int D>
 static int launch_attn_bwd_reg(const AttnBwdParams& P, cudaStream_t st) {
   const size_t smq = size_t(2 * kT2 * D) * sizeof(__half);
   const size_t smk = smq + kT2 * 3 * sizeof(float);
-  dim3 gridp((P.n_pad + kBT - 1) / kBT, P.B * P.heads, 2);     // also zeroes the pad rows of the gradient
-  launch_k(attn_bwd_q_reg_kernel<D>, gridp, dim3(kBT), smq, st, P);
-  if (int rc = check_launch("cross_attention_bwd(q)")) return rc;
+  dim3 gridp(blocks_for(P.n_pad, kBT), P.B * P.heads, 2);     // also zeroes the pad rows of the gradient
+  if (int rc = launch_k("cross_attention_bwd(q)", attn_bwd_q_reg_kernel<D>, gridp, dim3(kBT), smq, st, P)) return rc;
   if constexpr (D <= 32) {
-    launch_k(attn_bwd_kv_reg_kernel<D>, gridp, dim3(kBT), smk, st, P);
+    return launch_k("cross_attention_bwd(kv)", attn_bwd_kv_reg_kernel<D>, gridp, dim3(kBT), smk, st, P);
   } else {     // k, v, dk, dv of a 64-wide head do not fit the register file together: the shared-memory variant (64 channels per pass)
     const size_t smo = size_t(2 * D * kBT + 2 * kTT * D) * sizeof(__half) + kTT * 3 * sizeof(float);
     static bool configured[kMaxDevices] = {false};
     if (int rc = configure_smem(attn_bwd_kv_kernel<D>, (int)smo, configured, "cross_attention_bwd: cudaFuncSetAttribute")) return rc;
-    launch_k(attn_bwd_kv_kernel<D>, gridp, dim3(kBT), smo, st, P);
+    return launch_k("cross_attention_bwd(kv)", attn_bwd_kv_kernel<D>, gridp, dim3(kBT), smo, st, P);
   }
-  return check_launch("cross_attention_bwd(kv)");
 }
 
 template <int D>
@@ -425,13 +417,9 @@ static int launch_attn_bwd(const AttnBwdParams& P, cudaStream_t st) {
   if (int rc = configure_smem(attn_bwd_q_kernel<D>, (int)smq, configured, "cross_attention_bwd: cudaFuncSetAttribute")) return rc;
   static bool configured2[kMaxDevices] = {false};
   if (int rc = configure_smem(attn_bwd_kv_kernel<D>, (int)smk, configured2, "cross_attention_bwd: cudaFuncSetAttribute")) return rc;
-  dim3 grid((P.N + kBT - 1) / kBT, P.B * P.heads, 2);
-  dim3 gridp((P.n_pad + kBT - 1) / kBT, P.B * P.heads, 2);     // also zero the pad rows of the gradient
-  launch_k(attn_bwd_q_kernel<D>, gridp, dim3(kBT), smq, st, P);
-  if (int rc = check_launch("cross_attention_bwd(q)")) return rc;
-  launch_k(attn_bwd_kv_kernel<D>, gridp, dim3(kBT), smk, st, P);
-  (void)grid;
-  return check_launch("cross_attention_bwd(kv)");
+  dim3 gridp(blocks_for(P.n_pad, kBT), P.B * P.heads, 2);     // also zero the pad rows of the gradient
+  if (int rc = launch_k("cross_attention_bwd(q)", attn_bwd_q_kernel<D>, gridp, dim3(kBT), smq, st, P)) return rc;
+  return launch_k("cross_attention_bwd(kv)", attn_bwd_kv_kernel<D>, gridp, dim3(kBT), smk, st, P);
 }
 
 }  // namespace icaf

@@ -165,7 +165,6 @@ extern "C" int icaf_augment(const void* params, size_t params_bytes, int B, int 
   P.taps = reinterpret_cast<const int4*>(base + off_warp + (size_t)B * 4 * s * sizeof(int));
   P.rgb_out = static_cast<unsigned char*>(rgb_out); P.ir_out = static_cast<unsigned char*>(ir_out);
   P.s = s;
-  const dim3 grid((unsigned)(((long long)s * s + kAugThreads - 1) / kAugThreads), (unsigned)B);
-  launch_k(augment_kernel, grid, dim3(kAugThreads), 0, (cudaStream_t)stream, P);
-  return check_launch("augment");
+  const dim3 grid(blocks_for((long long)s * s, kAugThreads), (unsigned)B);
+  return launch_k("augment", augment_kernel, grid, dim3(kAugThreads), 0, (cudaStream_t)stream, P);
 }

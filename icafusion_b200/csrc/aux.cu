@@ -8,32 +8,6 @@
 
 namespace icaf {
 
-__device__ __forceinline__ uint4 ldg16(const __half* p) { return __ldg(reinterpret_cast<const uint4*>(p)); }
-__device__ __forceinline__ void unpack8(const uint4& v, float (&f)[8]) {
-  const __half2* h = reinterpret_cast<const __half2*>(&v);
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    float2 t = __half22float2(h[i]);
-    f[2 * i] = t.x;
-    f[2 * i + 1] = t.y;
-  }
-}
-__device__ __forceinline__ uint4 pack8(const float (&f)[8]) {
-  uint4 v;
-  v.x = pack_half2(f[0], f[1]); v.y = pack_half2(f[2], f[3]);
-  v.z = pack_half2(f[4], f[5]); v.w = pack_half2(f[6], f[7]);
-  return v;
-}
-__device__ __forceinline__ uint4 hmax8(const uint4& a, const uint4& b) {
-  uint4 r;
-  const __half2* x = reinterpret_cast<const __half2*>(&a);
-  const __half2* y = reinterpret_cast<const __half2*>(&b);
-  __half2* z = reinterpret_cast<__half2*>(&r);
-#pragma unroll
-  for (int i = 0; i < 4; ++i) z[i] = __hmax2(x[i], y[i]);
-  return r;
-}
-
 // ------------------------------------------------------------------------------------------------
 // (B,3,H,W) planar -> (B,H,W,4) fp16
 template <typename T>
@@ -782,8 +756,6 @@ __global__ void prefetch_l2_kernel(const char* __restrict__ p, size_t bytes) {
   pdl_wait();
 }
 
-static inline unsigned blocks_for(long long n, int bs) { return (unsigned)((n + bs - 1) / bs); }
-
 }  // namespace icaf
 
 using namespace icaf;
@@ -793,22 +765,26 @@ extern "C" int icaf_pack_image(const void* src, int src_dtype, float scale, int 
   long long hw = (long long)H * W, npix = hw * B;
   cudaStream_t st = (cudaStream_t)stream;
   unsigned g = blocks_for(npix, 256);
-  if (src_dtype == 0) launch_k(pack_image_kernel<__half>, dim3(g), dim3(256), 0, st, (const __half*)src, scale, npix, hw, (__half*)dst);
-  else if (src_dtype == 1) launch_k(pack_image_kernel<float>, dim3(g), dim3(256), 0, st, (const float*)src, scale, npix, hw, (__half*)dst);
-  else if (src_dtype == 2) launch_k(pack_image_kernel<uint8_t>, dim3(g), dim3(256), 0, st, (const uint8_t*)src, scale, npix, hw, (__half*)dst);
-  else return set_error(ICAF_ERR_BAD_ARG, "pack_image: src_dtype must be 0 (fp16), 1 (fp32) or 2 (uint8)");
-  return check_launch("pack_image");
+  if (src_dtype == 0) return launch_k("pack_image", pack_image_kernel<__half>, dim3(g), dim3(256), 0, st, (const __half*)src, scale, npix, hw,
+                                      (__half*)dst);
+  if (src_dtype == 1) return launch_k("pack_image", pack_image_kernel<float>, dim3(g), dim3(256), 0, st, (const float*)src, scale, npix, hw,
+                                      (__half*)dst);
+  if (src_dtype == 2) return launch_k("pack_image", pack_image_kernel<uint8_t>, dim3(g), dim3(256), 0, st, (const uint8_t*)src, scale, npix, hw,
+                                      (__half*)dst);
+  return set_error(ICAF_ERR_BAD_ARG, "pack_image: src_dtype must be 0 (fp16), 1 (fp32) or 2 (uint8)");
 }
 
 extern "C" int icaf_pack_image_s2d(const void* src, int src_dtype, float scale, int B, int H, int W, void* dst, void* stream) {
   if (!src || !dst || B < 1 || H < 2 || W < 2 || (H & 1) || (W & 1)) return set_error(ICAF_ERR_BAD_ARG, "pack_image_s2d: H and W must be even");
   cudaStream_t st = (cudaStream_t)stream;
   unsigned g = blocks_for((long long)B * (H / 2) * (W / 2), 256);
-  if (src_dtype == 0) launch_k(pack_image_s2d_kernel<__half>, dim3(g), dim3(256), 0, st, (const __half*)src, scale, B, H, W, (__half*)dst);
-  else if (src_dtype == 1) launch_k(pack_image_s2d_kernel<float>, dim3(g), dim3(256), 0, st, (const float*)src, scale, B, H, W, (__half*)dst);
-  else if (src_dtype == 2) launch_k(pack_image_s2d_kernel<uint8_t>, dim3(g), dim3(256), 0, st, (const uint8_t*)src, scale, B, H, W, (__half*)dst);
-  else return set_error(ICAF_ERR_BAD_ARG, "pack_image_s2d: src_dtype must be 0 (fp16), 1 (fp32) or 2 (uint8)");
-  return check_launch("pack_image_s2d");
+  if (src_dtype == 0) return launch_k("pack_image_s2d", pack_image_s2d_kernel<__half>, dim3(g), dim3(256), 0, st, (const __half*)src, scale, B, H, W,
+                                      (__half*)dst);
+  if (src_dtype == 1) return launch_k("pack_image_s2d", pack_image_s2d_kernel<float>, dim3(g), dim3(256), 0, st, (const float*)src, scale, B, H, W,
+                                      (__half*)dst);
+  if (src_dtype == 2) return launch_k("pack_image_s2d", pack_image_s2d_kernel<uint8_t>, dim3(g), dim3(256), 0, st, (const uint8_t*)src, scale, B, H,
+                                      W, (__half*)dst);
+  return set_error(ICAF_ERR_BAD_ARG, "pack_image_s2d: src_dtype must be 0 (fp16), 1 (fp32) or 2 (uint8)");
 }
 
 extern "C" int icaf_sppf_pool(const void* x, int64_t x_ld, void* y1, void* y2, void* y3, int64_t y_ld, int B, int H,
@@ -816,37 +792,32 @@ extern "C" int icaf_sppf_pool(const void* x, int64_t x_ld, void* y1, void* y2, v
   if (!x || !y1 || !y2 || !y3 || C % 8 || x_ld % 8 || y_ld % 8) return set_error(ICAF_ERR_BAD_ARG, "sppf_pool: bad argument");
   if (H * W <= 1024) {
     int threads = (H * W + 31) / 32 * 32;
-    launch_k(sppf_pool_smem_kernel, dim3(B * (C / 8)), dim3(threads), (size_t)(2 * H * W * sizeof(uint4)), (cudaStream_t)stream,
-             (const __half*)x, x_ld, (__half*)y1, (__half*)y2, (__half*)y3, y_ld, H, W, C / 8);
-    return check_launch("sppf_pool");
+    return launch_k("sppf_pool", sppf_pool_smem_kernel, dim3(B * (C / 8)), dim3(threads), (size_t)(2 * H * W * sizeof(uint4)), (cudaStream_t)stream,
+                    (const __half*)x, x_ld, (__half*)y1, (__half*)y2, (__half*)y3, y_ld, H, W, C / 8);
   }
   long long total = (long long)B * H * W * (C / 8);
-  launch_k(sppf_pool_kernel, dim3(blocks_for(total, 128)), dim3(128), 0, (cudaStream_t)stream, (const __half*)x, x_ld, (__half*)y1, (__half*)y2,
-                                                                            (__half*)y3, y_ld, B, H, W, C / 8);
-  return check_launch("sppf_pool");
+  return launch_k("sppf_pool", sppf_pool_kernel, dim3(blocks_for(total, 128)), dim3(128), 0, (cudaStream_t)stream, (const __half*)x, x_ld,
+                  (__half*)y1, (__half*)y2, (__half*)y3, y_ld, B, H, W, C / 8);
 }
 
 extern "C" int icaf_upsample2x(const void* x, int64_t x_ld, void* y, int64_t y_ld, int B, int H, int W, int C, void* stream) {
   if (!x || !y || C % 8 || x_ld % 8 || y_ld % 8) return set_error(ICAF_ERR_BAD_ARG, "upsample2x: bad argument");
   long long total = (long long)B * 4 * H * W * (C / 8);
-  launch_k(upsample2x_kernel, dim3(blocks_for(total, 256)), dim3(256), 0, (cudaStream_t)stream, (const __half*)x, x_ld, (__half*)y, y_ld, B, H, W, C / 8);
-  return check_launch("upsample2x");
+  return launch_k("upsample2x", upsample2x_kernel, dim3(blocks_for(total, 256)), dim3(256), 0, (cudaStream_t)stream, (const __half*)x, x_ld,
+                  (__half*)y, y_ld, B, H, W, C / 8);
 }
 
 extern "C" int icaf_prefetch_l2(const void* ptr, size_t bytes, void* stream) {
   if (!ptr || bytes == 0) return set_error(ICAF_ERR_BAD_ARG, "prefetch_l2: bad argument");
-  size_t lines = (bytes + 127) / 128;
-  unsigned blocks = (unsigned)((lines + 255) / 256);
+  unsigned blocks = blocks_for((bytes + 127) / 128, 256);
   if (blocks > 148u * 8u) blocks = 148u * 8u;
-  launch_k(prefetch_l2_kernel, dim3(blocks), dim3(256), 0, (cudaStream_t)stream, (const char*)ptr, bytes);
-  return check_launch("prefetch_l2");
+  return launch_k("prefetch_l2", prefetch_l2_kernel, dim3(blocks), dim3(256), 0, (cudaStream_t)stream, (const char*)ptr, bytes);
 }
 
 extern "C" int icaf_copy_channels(const void* x, int64_t x_ld, void* y, int64_t y_ld, int64_t pixels, int C, void* stream) {
   if (!x || !y || C % 8 || x_ld % 8 || y_ld % 8) return set_error(ICAF_ERR_BAD_ARG, "copy_channels: bad argument");
-  launch_k(copy_channels_kernel, dim3(blocks_for(pixels * (C / 8), 256)), dim3(256), 0, (cudaStream_t)stream, (const __half*)x, x_ld, (__half*)y, y_ld,
-                                                                                          pixels, C / 8);
-  return check_launch("copy_channels");
+  return launch_k("copy_channels", copy_channels_kernel, dim3(blocks_for(pixels * (C / 8), 256)), dim3(256), 0, (cudaStream_t)stream,
+                  (const __half*)x, x_ld, (__half*)y, y_ld, pixels, C / 8);
 }
 
 extern "C" int icaf_dmff_pool_tokens(const void* x_vis, const void* x_ir, int64_t x_ld, const void* pos_vis,
@@ -869,8 +840,7 @@ extern "C" int icaf_dmff_pool_tokens(const void* x_vis, const void* x_ir, int64_
   P.kh = H - (nh - 1) * P.sh; P.kw = W - (nw - 1) * P.sw;
   long long total = (long long)B * n_pad * P.C8;
   dim3 grid(blocks_for(total, 128), 2);
-  launch_k(dmff_pool_tokens_kernel, dim3(grid), dim3(128), 0, (cudaStream_t)stream, P);
-  return check_launch("dmff_pool_tokens");
+  return launch_k("dmff_pool_tokens", dmff_pool_tokens_kernel, dim3(grid), dim3(128), 0, (cudaStream_t)stream, P);
 }
 
 extern "C" int icaf_layernorm(const void* x0, const void* x1, const float* g0, const float* b0, const float* g1,
@@ -881,8 +851,7 @@ extern "C" int icaf_layernorm(const void* x0, const void* x1, const float* g0, c
   P.x[0] = (const __half*)x0; P.x[1] = (const __half*)x1; P.y[0] = (__half*)y0; P.y[1] = (__half*)y1;
   P.g[0] = g0; P.g[1] = g1; P.b[0] = b0; P.b[1] = b1; P.rows = rows; P.C = C; P.eps = eps;
   dim3 grid(blocks_for(rows, 4), x1 ? 2 : 1);
-  launch_k(layernorm_kernel, dim3(grid), dim3(128), 0, (cudaStream_t)stream, P);
-  return check_launch("layernorm");
+  return launch_k("layernorm", layernorm_kernel, dim3(grid), dim3(128), 0, (cudaStream_t)stream, P);
 }
 
 extern "C" int icaf_dmff_upsample_cat(const void* tok_vis, const void* tok_ir, int n_pad, const void* x_vis,
@@ -897,8 +866,7 @@ extern "C" int icaf_dmff_upsample_cat(const void* tok_vis, const void* tok_ir, i
   P.sy = float(nh) / float(H); P.sx = float(nw) / float(W);
   long long total = (long long)B * H * W * P.C8;
   dim3 grid(blocks_for(total, 256), 2);
-  launch_k(dmff_upsample_cat_kernel, dim3(grid), dim3(256), 0, (cudaStream_t)stream, P);
-  return check_launch("dmff_upsample_cat");
+  return launch_k("dmff_upsample_cat", dmff_upsample_cat_kernel, dim3(grid), dim3(256), 0, (cudaStream_t)stream, P);
 }
 
 extern "C" int icaf_detect_decode(const void* p, int64_t p_ld, void* x_out, void* z, void* logits, int B, int ny, int nx,
@@ -912,16 +880,14 @@ extern "C" int icaf_detect_decode(const void* p, int64_t p_ld, void* x_out, void
   P.B = B; P.ny = ny; P.nx = nx; P.na = na; P.no = no; P.total_rows = total_rows; P.row_off = row_off; P.stride = stride;
   for (int i = 0; i < na * 2; ++i) P.anchors[i] = anchors_host[i];
   long long total = (long long)B * na * ny * nx;
-  launch_k(detect_decode_kernel, dim3(blocks_for(total, 128)), dim3(128), 0, (cudaStream_t)stream, P);
-  return check_launch("detect_decode");
+  return launch_k("detect_decode", detect_decode_kernel, dim3(blocks_for(total, 128)), dim3(128), 0, (cudaStream_t)stream, P);
 }
 
 extern "C" int icaf_axpby(const void* x, const void* y, const float* a, const float* b, void* out, int64_t n, void* stream) {
   if (!x || !a || !out || (y && !b) || n < 0 || n % 8) return set_error(ICAF_ERR_BAD_ARG, "axpby: null pointer or element count not a multiple of 8");
   if (n == 0) return ICAF_OK;
-  launch_k(axpby_kernel, dim3(blocks_for(n / 8, 256)), dim3(256), 0, (cudaStream_t)stream, (const __half*)x, (const __half*)y, a, b, (__half*)out,
-           (long long)(n / 8));
-  return check_launch("axpby");
+  return launch_k("axpby", axpby_kernel, dim3(blocks_for(n / 8, 256)), dim3(256), 0, (cudaStream_t)stream, (const __half*)x, (const __half*)y, a, b,
+                  (__half*)out, (long long)(n / 8));
 }
 
 extern "C" size_t icaf_nms_workspace_bytes(int B, int R) {
@@ -949,28 +915,23 @@ static int nms_launch(const void* z, int B, int R, int no, float conf_thres, flo
   P.multi_label = multi_label;
   P.conf_thres = conf_thres; P.iou_thres = iou_thres; P.class_mask = class_mask; P.det = det; P.count = count;
   cudaStream_t st = (cudaStream_t)stream;
-  const dim3 grid((unsigned)((R + 255) / 256), (unsigned)B);
+  const dim3 grid(blocks_for(R, 256), (unsigned)B);
   if (multi_label) {
     const size_t slots = (size_t)B * R * (no - 5);
     P.mkeys[0] = (unsigned*)workspace; P.mids[0] = (int*)(P.mkeys[0] + slots);
     P.mkeys[1] = (unsigned*)(P.mids[0] + slots); P.mids[1] = (int*)(P.mkeys[1] + slots);
     P.order = P.mids[0];
-    launch_k(nms_filter_kernel, grid, dim3(256), 0, st, P);
-    if (int rc = check_launch("nms(filter)")) return rc;
-    launch_k(nms_sort_kernel, dim3(B), dim3(kNmsSortThreads), 0, st, P);
-    if (int rc = check_launch("nms(sort)")) return rc;
+    if (int rc = launch_k("nms(filter)", nms_filter_kernel, grid, dim3(256), 0, st, P)) return rc;
+    if (int rc = launch_k("nms(sort)", nms_sort_kernel, dim3(B), dim3(kNmsSortThreads), 0, st, P)) return rc;
   } else {
     P.keys = (unsigned long long*)workspace;
     P.order = (int*)((char*)workspace + (size_t)B * R * sizeof(unsigned long long));
     cudaError_t e = cudaMemsetAsync(count, 0, (size_t)B * sizeof(int), st);      // candidate counters
     if (e != cudaSuccess) return set_cuda_error(e, "nms: cudaMemsetAsync");
-    launch_k(nms_filter_kernel, grid, dim3(256), 0, st, P);
-    if (int rc = check_launch("nms(filter)")) return rc;
-    launch_k(nms_rank_kernel, grid, dim3(256), 0, st, P);
-    if (int rc = check_launch("nms(rank)")) return rc;
+    if (int rc = launch_k("nms(filter)", nms_filter_kernel, grid, dim3(256), 0, st, P)) return rc;
+    if (int rc = launch_k("nms(rank)", nms_rank_kernel, grid, dim3(256), 0, st, P)) return rc;
   }
-  launch_k(nms_kernel, dim3(B), dim3(kNmsThreads), 0, st, P);
-  return check_launch("nms");
+  return launch_k("nms", nms_kernel, dim3(B), dim3(kNmsThreads), 0, st, P);
 }
 
 extern "C" int icaf_nms(const void* z, int B, int R, int no, float conf_thres, float iou_thres, int agnostic, uint64_t class_mask,
@@ -989,9 +950,8 @@ extern "C" int icaf_nms_multi_label(const void* z, int B, int R, int no, float c
 extern "C" int icaf_row_stats(const void* x0, const void* x1, float* stats0, float* stats1, int64_t rows, int C, void* stream) {
   if (!x0 || !stats0 || (x1 && !stats1) || rows < 1 || C < 8 || C % 8) return set_error(ICAF_ERR_BAD_ARG, "row_stats: bad argument");
   dim3 grid(blocks_for(rows, 4), x1 ? 2 : 1);
-  launch_k(row_stats_kernel, dim3(grid), dim3(128), 0, (cudaStream_t)stream, (const __half*)x0, (const __half*)x1, (float2*)stats0,
-           (float2*)stats1, (long long)rows, C);
-  return check_launch("row_stats");
+  return launch_k("row_stats", row_stats_kernel, dim3(grid), dim3(128), 0, (cudaStream_t)stream, (const __half*)x0, (const __half*)x1,
+                  (float2*)stats0, (float2*)stats1, (long long)rows, C);
 }
 
 extern "C" int icaf_letterbox(const void* src, int B, int H0, int W0, void* dst, int H, int W, int top, int left, int new_h, int new_w,
@@ -1005,6 +965,5 @@ extern "C" int icaf_letterbox(const void* src, int B, int H0, int W0, void* dst,
   LetterboxParams P;
   P.src = (const unsigned char*)src; P.dst = (unsigned char*)dst; P.xtab = resize ? xtab : nullptr; P.ytab = resize ? ytab : nullptr;
   P.B = B; P.H0 = H0; P.W0 = W0; P.H = H; P.W = W; P.top = top; P.left = left; P.new_h = new_h; P.new_w = new_w; P.pad = pad_value;
-  launch_k(letterbox_kernel, dim3(blocks_for((long long)B * H * W, 256)), dim3(256), 0, (cudaStream_t)stream, P);
-  return check_launch("letterbox");
+  return launch_k("letterbox", letterbox_kernel, dim3(blocks_for((long long)B * H * W, 256)), dim3(256), 0, (cudaStream_t)stream, P);
 }

@@ -347,6 +347,6 @@ extern "C" int icaf_bottleneck_fwd(int B, int H, int W, const icaf_bottleneck_io
   if (per < 1) per = 1;
   static bool configured[kMaxDevices] = {};
   if (int rc = configure_smem(bottleneck_kernel, BnLayout::kTotal, configured, "bottleneck: cudaFuncSetAttribute")) return rc;
-  launch_k(bottleneck_kernel, dim3(unsigned(per * n_io)), dim3(kThreadsBn), size_t(BnLayout::kTotal), (cudaStream_t)stream, P, maps);
-  return check_launch("bottleneck_fwd");
+  return launch_k("bottleneck_fwd", bottleneck_kernel, dim3(unsigned(per * n_io)), dim3(kThreadsBn), size_t(BnLayout::kTotal), (cudaStream_t)stream,
+                  P, maps);
 }

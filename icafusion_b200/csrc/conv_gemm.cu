@@ -771,8 +771,7 @@ static int launch_conv(const ConvParams& P, const ConvPlan& pl, const __half* co
   if (int rc = encode_maps<BN>(P, w, g, n_io, P.tma_epi != 0, maps)) return rc;
   // the one-tile kernel takes the tile grid (split-K: in clusters along x); the persistent one `ctas` CTAs
   const dim3 grid = pl.persist ? dim3(unsigned(pl.ctas)) : dim3(pl.grid_x, pl.grid_y, pl.grid_z);
-  launch_kc(kernel, grid, dim3(pl.persist ? kPersistThreads : kThreads), (size_t)pl.smem, st, pl.cluster, P, maps);
-  return check_launch("conv2d_fwd");
+  return launch_kc("conv2d_fwd", kernel, grid, dim3(pl.persist ? kPersistThreads : kThreads), (size_t)pl.smem, st, pl.cluster, P, maps);
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -861,7 +860,6 @@ extern "C" int icaf_conv2d_fwd_simt(const icaf_conv_geom* g, const icaf_conv_io*
   int rc = fill_params(g, io, n_io, S.P, S.w);
   if (rc) return rc;
   long long total = (long long)S.P.M * S.P.N;
-  dim3 grid((unsigned)((total + 255) / 256), 1, n_io);
-  launch_k(conv_gemm_simt_kernel, dim3(grid), dim3(256), 0, (cudaStream_t)stream, S);
-  return check_launch("conv2d_fwd_simt");
+  dim3 grid(blocks_for(total, 256), 1, n_io);
+  return launch_k("conv2d_fwd_simt", conv_gemm_simt_kernel, dim3(grid), dim3(256), 0, (cudaStream_t)stream, S);
 }

@@ -10,18 +10,6 @@
 
 namespace icaf {
 
-__device__ __forceinline__ void unpack8b(const uint4& v, float (&f)[8]) {
-  const __half2* h = reinterpret_cast<const __half2*>(&v);
-#pragma unroll
-  for (int i = 0; i < 4; ++i) { float2 t = __half22float2(h[i]); f[2 * i] = t.x; f[2 * i + 1] = t.y; }
-}
-__device__ __forceinline__ uint4 pack8b(const float (&f)[8]) {
-  uint4 v;
-  v.x = pack_half2(f[0], f[1]); v.y = pack_half2(f[2], f[3]); v.z = pack_half2(f[4], f[5]); v.w = pack_half2(f[6], f[7]);
-  return v;
-}
-__device__ __forceinline__ uint4 ld16(const __half* p) { return __ldg(reinterpret_cast<const uint4*>(p)); }
-
 struct PoolBwdParams {
   const __half* x[2]; const __half* dtok[2]; __half* dx[2];
   uint2* code[2];          // [B][N][C8]: per window and channel, the position code (ky*kw + kx) of its first maximum
@@ -49,15 +37,12 @@ __global__ void __launch_bounds__(128) dmff_pool_argmax_kernel(const PoolBwdPara
   for (int k = 0; k < P.kh * P.kw; ++k) {
     const int ky = k / P.kw, kx = k - ky * P.kw;
     float f[8];
-    unpack8b(ld16(x0 + ((long long)ky * P.W + kx) * P.x_ld), f);
+    unpack8(ldg16(x0 + ((long long)ky * P.W + kx) * P.x_ld), f);
 #pragma unroll
     for (int e = 0; e < 8; ++e)
       if (f[e] > best[e]) { best[e] = f[e]; arg[e] = uint32_t(k); }       // strict: the first maximum in row-major order wins
   }
-  uint2 o;
-  o.x = arg[0] | (arg[1] << 8) | (arg[2] << 16) | (arg[3] << 24);
-  o.y = arg[4] | (arg[5] << 8) | (arg[6] << 16) | (arg[7] << 24);
-  (mod ? P.code[1] : P.code[0])[i] = o;
+  (mod ? P.code[1] : P.code[0])[i] = pack_argmax8(arg);
 }
 // 2 of 2: every pixel gathers from the windows that contain it
 __global__ void __launch_bounds__(128) dmff_pool_tokens_bwd_kernel(const PoolBwdParams P) {
@@ -88,17 +73,16 @@ __global__ void __launch_bounds__(128) dmff_pool_tokens_bwd_kernel(const PoolBwd
       if (w < tx * P.sw || w >= tx * P.sw + P.kw) continue;
       const int n = ty * P.nw + tx;
       float g[8];
-      unpack8b(ld16(dtok + (long long)n * C), g);
+      unpack8(ldg16(dtok + (long long)n * C), g);
       const uint2 cd = __ldg(code + (long long)n * P.C8);
       const uint32_t mine = uint32_t((h - ty * P.sh) * P.kw + (w - tx * P.sw));
 #pragma unroll
       for (int e = 0; e < 8; ++e) {
-        const uint32_t a = ((e < 4 ? cd.x : cd.y) >> (8 * (e & 3))) & 0xffu;
-        acc[e] += g[e] * (w1 + (a == mine ? w2 : 0.f));
+        acc[e] += g[e] * (w1 + (argmax_code(cd, e) == mine ? w2 : 0.f));
       }
     }
   }
-  *reinterpret_cast<uint4*>((mod ? P.dx[1] : P.dx[0]) + p * C + c * 8) = pack8b(acc);
+  *reinterpret_cast<uint4*>((mod ? P.dx[1] : P.dx[0]) + p * C + c * 8) = pack8(acc);
 }
 
 struct UpCatBwdParams {
@@ -133,35 +117,42 @@ __global__ void __launch_bounds__(128) dmff_upsample_cat_bwd_kernel(const UpCatB
       for (int ox = ox0; ox <= ox1; ++ox) {
         if ((ident ? ox : min(int(floorf(ox * P.sx)), P.nw - 1)) != ix) continue;
         float g[8];
-        unpack8b(ld16(d + ((long long)(b * P.H + oy) * P.W + ox) * P.d_ld), g);
+        unpack8(ldg16(d + ((long long)(b * P.H + oy) * P.W + ox) * P.d_ld), g);
 #pragma unroll
         for (int e = 0; e < 8; ++e) acc[e] += g[e];
       }
     }
   }
-  *reinterpret_cast<uint4*>((mod ? P.dtok[1] : P.dtok[0]) + t * C + c * 8) = pack8b(acc);
+  *reinterpret_cast<uint4*>((mod ? P.dtok[1] : P.dtok[0]) + t * C + c * 8) = pack8(acc);
 }
 
-// mode 0: out[n][(ky*kw + kx)*cin_p + c]                  = w[n][c][ky][kx]      (rows >= Cout, k_pad >= kh*kw*cin_p)
-// mode 1: out[c][((kh-1-ky)*kw + (kw-1-kx))*cout_p + n]   = w[n][c][ky][kx]      (rows >= Cin,  k_pad >= kh*kw*cout_p)
+// Element i of a packed [rows][k_pad] filter bank (pad rows / columns are 0):
+//   forward:         out[n][(ky*kw + kx)*chan_p + c]                  = w[n][c][ky][kx]      (rows >= Cout, k_pad >= kh*kw*chan_p)
+//   flip_transpose:  out[c][((kh-1-ky)*kw + (kw-1-kx))*chan_p + n]    = w[n][c][ky][kx]      (rows >= Cin,  k_pad >= kh*kw*chan_p)
+__device__ __forceinline__ __half packed_weight(const float* __restrict__ w, long long i, int k_pad, int chan_p, int Cout, int Cin, int kh,
+                                                int kw, bool flip_transpose) {
+  const int r = int(i / k_pad), k = int(i - (long long)r * k_pad);
+  const int tap = k / chan_p, ch = k - tap * chan_p;
+  float v = 0.f;
+  if (tap < kh * kw) {
+    const int ky = tap / kw, kx = tap - ky * kw;
+    if (!flip_transpose) {
+      if (r < Cout && ch < Cin) v = w[(((long long)r * Cin + ch) * kh + ky) * kw + kx];
+    } else {
+      if (r < Cin && ch < Cout) v = w[(((long long)ch * Cin + r) * kh + (kh - 1 - ky)) * kw + (kw - 1 - kx)];
+    }
+  }
+  return __float2half(v);
+}
+
+// mode 0: the forward bank; mode 1: the flipped and transposed one
 __global__ void __launch_bounds__(256) pack_weight_kernel(const float* __restrict__ w, __half* __restrict__ out, int Cout, int Cin, int kh, int kw,
                                                           int chan_p, int rows, int k_pad, int mode) {
   pdl_launch_dependents();
   pdl_wait();
   const long long i = blockIdx.x * 256ll + threadIdx.x;
   if (i >= (long long)rows * k_pad) return;
-  const int r = int(i / k_pad), k = int(i - (long long)r * k_pad);
-  const int tap = k / chan_p, ch = k - tap * chan_p;
-  float v = 0.f;
-  if (tap < kh * kw) {
-    const int ky = tap / kw, kx = tap - ky * kw;
-    if (mode == 0) {
-      if (r < Cout && ch < Cin) v = w[(((long long)r * Cin + ch) * kh + ky) * kw + kx];
-    } else {
-      if (r < Cin && ch < Cout) v = w[(((long long)ch * Cin + r) * kh + (kh - 1 - ky)) * kw + (kw - 1 - kx)];
-    }
-  }
-  out[i] = __float2half(v);
+  out[i] = packed_weight(w, i, k_pad, chan_p, Cout, Cin, kh, kw, mode != 0);
 }
 
 // both banks of one filter in one launch (the training step packs every filter once per step, forward and data-gradient form)
@@ -174,19 +165,7 @@ __global__ void __launch_bounds__(256) pack_weight_pair_kernel(const float* __re
   if (i >= nf + nd) return;
   const bool dg = i >= nf;
   if (dg) i -= nf;
-  const int k_pad = dg ? kpad_d : kpad_f, chan_p = dg ? chan_d : Cin;
-  const int r = int(i / k_pad), k = int(i - (long long)r * k_pad);
-  const int tap = k / chan_p, ch = k - tap * chan_p;
-  float v = 0.f;
-  if (tap < kh * kw) {
-    const int ky = tap / kw, kx = tap - ky * kw;
-    if (!dg) {
-      if (r < Cout && ch < Cin) v = w[(((long long)r * Cin + ch) * kh + ky) * kw + kx];
-    } else {
-      if (r < Cin && ch < Cout) v = w[(((long long)ch * Cin + r) * kh + (kh - 1 - ky)) * kw + (kw - 1 - kx)];
-    }
-  }
-  (dg ? out_d : out_f)[i] = __float2half(v);
+  (dg ? out_d : out_f)[i] = packed_weight(w, i, dg ? kpad_d : kpad_f, dg ? chan_d : Cin, Cout, Cin, kh, kw, dg);
 }
 
 }  // namespace icaf
@@ -210,11 +189,9 @@ extern "C" int icaf_dmff_pool_tokens_bwd(const void* x_vis, const void* x_ir, in
   if (P.kh * P.kw > 255) return set_error(ICAF_ERR_UNSUPPORTED, "dmff_pool_tokens_bwd: pooling windows of more than 255 pixels");
   P.code[0] = (uint2*)workspace; P.code[1] = P.code[0] + size_t(B) * nh * nw * P.C8;
   const long long nwin = (long long)B * nh * nw * P.C8;
-  launch_k(dmff_pool_argmax_kernel, dim3((unsigned)((nwin + 127) / 128), 2), dim3(128), 0, (cudaStream_t)stream, P);
-  if (int rc = check_launch("dmff_pool_tokens_bwd(argmax)")) return rc;
+  if (int rc = launch_k("dmff_pool_tokens_bwd(argmax)", dmff_pool_argmax_kernel, dim3(blocks_for(nwin, 128), 2), dim3(128), 0, (cudaStream_t)stream, P)) return rc;
   const long long total = (long long)B * H * W * P.C8;
-  launch_k(dmff_pool_tokens_bwd_kernel, dim3((unsigned)((total + 127) / 128), 2), dim3(128), 0, (cudaStream_t)stream, P);
-  return check_launch("dmff_pool_tokens_bwd");
+  return launch_k("dmff_pool_tokens_bwd", dmff_pool_tokens_bwd_kernel, dim3(blocks_for(total, 128), 2), dim3(128), 0, (cudaStream_t)stream, P);
 }
 
 extern "C" int icaf_dmff_upsample_cat_bwd(const void* dcat, int64_t d_ld, void* dtok_vis, void* dtok_ir, int B, int H, int W, int C, int nh, int nw,
@@ -228,8 +205,7 @@ extern "C" int icaf_dmff_upsample_cat_bwd(const void* dcat, int64_t d_ld, void* 
   P.B = B; P.H = H; P.W = W; P.C8 = C / 8; P.nh = nh; P.nw = nw; P.n_pad = n_pad;
   P.sy = float(nh) / float(H); P.sx = float(nw) / float(W);
   const long long total = (long long)B * n_pad * P.C8;
-  launch_k(dmff_upsample_cat_bwd_kernel, dim3((unsigned)((total + 127) / 128), 2), dim3(128), 0, (cudaStream_t)stream, P);
-  return check_launch("dmff_upsample_cat_bwd");
+  return launch_k("dmff_upsample_cat_bwd", dmff_upsample_cat_bwd_kernel, dim3(blocks_for(total, 128), 2), dim3(128), 0, (cudaStream_t)stream, P);
 }
 
 extern "C" int icaf_pack_weight(const float* w, int Cout, int Cin, int kh, int kw, int chan_pad, int rows, int k_pad, int transpose_flip, void* out,
@@ -238,9 +214,8 @@ extern "C" int icaf_pack_weight(const float* w, int Cout, int Cin, int kh, int k
   const int chan = transpose_flip ? Cout : Cin, need_rows = transpose_flip ? Cin : Cout;
   if (chan_pad < chan || rows < need_rows || k_pad < kh * kw * chan_pad) return set_error(ICAF_ERR_BAD_ARG, "pack_weight: padded sizes smaller than the filter");
   const long long total = (long long)rows * k_pad;
-  launch_k(pack_weight_kernel, dim3((unsigned)((total + 255) / 256)), dim3(256), 0, (cudaStream_t)stream, w, (__half*)out, Cout, Cin, kh, kw, chan_pad,
-           rows, k_pad, transpose_flip ? 1 : 0);
-  return check_launch("pack_weight");
+  return launch_k("pack_weight", pack_weight_kernel, dim3(blocks_for(total, 256)), dim3(256), 0, (cudaStream_t)stream, w, (__half*)out, Cout, Cin, kh,
+                  kw, chan_pad, rows, k_pad, transpose_flip ? 1 : 0);
 }
 
 extern "C" int icaf_pack_weight_pair(const float* w, int Cout, int Cin, int kh, int kw, int rows_f, int kpad_f, void* out_fwd, int chan_pad_d, int rows_d,
@@ -249,7 +224,6 @@ extern "C" int icaf_pack_weight_pair(const float* w, int Cout, int Cin, int kh, 
   if (rows_f < Cout || kpad_f < kh * kw * Cin || chan_pad_d < Cout || rows_d < Cin || kpad_d < kh * kw * chan_pad_d)
     return set_error(ICAF_ERR_BAD_ARG, "pack_weight_pair: padded sizes smaller than the filter");
   const long long total = (long long)rows_f * kpad_f + (long long)rows_d * kpad_d;
-  launch_k(pack_weight_pair_kernel, dim3((unsigned)((total + 255) / 256)), dim3(256), 0, (cudaStream_t)stream, w, (__half*)out_fwd, (__half*)out_dgrad, Cout, Cin,
-           kh, kw, rows_f, kpad_f, chan_pad_d, rows_d, kpad_d);
-  return check_launch("pack_weight_pair");
+  return launch_k("pack_weight_pair", pack_weight_pair_kernel, dim3(blocks_for(total, 256)), dim3(256), 0, (cudaStream_t)stream, w, (__half*)out_fwd,
+                  (__half*)out_dgrad, Cout, Cin, kh, kw, rows_f, kpad_f, chan_pad_d, rows_d, kpad_d);
 }

@@ -1,4 +1,4 @@
-// Shared internals of libicaf_b200: error reporting, launch checks, device info.
+// Shared internals of libicaf_b200: error reporting, checked launches, device info.
 #pragma once
 #include <cstdio>
 #include <cuda.h>          // CUtensorMap + enums only; the driver entry point is resolved at run time (no -lcuda)
@@ -13,18 +13,19 @@ namespace icaf {
 int set_error(int code, const char* msg);
 int set_cuda_error(cudaError_t e, const char* where);
 const uint32_t* seed_offset_ptr();    // see icaf_set_seed_offset
-int check_launch(const char* where);   // cudaGetLastError after a launch; never synchronises
 int sm_count_cached();   // SM count of the CURRENT device (cached per device ordinal)
 int current_device();    // cudaGetDevice; -1 on error
 bool pdl_enabled();        // programmatic dependent launch on every kernel (env ICAF_PDL, default on)
 
-// Launch with the programmatic-stream-serialization attribute when PDL is enabled (every kernel of this library
-// executes griddepcontrol.wait before it touches memory another kernel may have produced).
 void count_launch();   // api.cu: process-wide tally behind icaf_kernel_launches()
 
+// Launch with the programmatic-stream-serialization attribute when PDL is enabled (every kernel of this library
+// executes griddepcontrol.wait before it touches memory another kernel may have produced).  Returns ICAF_OK, or the
+// launch's own error under `where` (the prefix of icaf_last_error()); never synchronises.  Only launches the runtime
+// accepted are counted.
 template <typename... KArgs, typename... Args>
-inline cudaError_t launch_kc(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, unsigned cluster_x,
-                             Args&&... args) {
+inline int launch_kc(const char* where, void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st,
+                     unsigned cluster_x, Args&&... args) {
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = st;
   cudaLaunchAttribute attr[2];
@@ -41,13 +42,21 @@ inline cudaError_t launch_kc(void (*kernel)(KArgs...), dim3 grid, dim3 block, si
   }
   cfg.attrs = attr;
   cfg.numAttrs = n;
+  const cudaError_t e = cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
+  if (e != cudaSuccess) {
+    (void)cudaGetLastError();   // the refused launch also set the runtime's last error: clear it so no later check reports it again
+    return set_cuda_error(e, where);
+  }
   count_launch();
-  return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
+  return ICAF_OK;
 }
 template <typename... KArgs, typename... Args>
-inline cudaError_t launch_k(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args) {
-  return launch_kc(kernel, grid, block, smem, st, 1u, static_cast<Args&&>(args)...);
+inline int launch_k(const char* where, void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args) {
+  return launch_kc(where, kernel, grid, block, smem, st, 1u, static_cast<Args&&>(args)...);
 }
+
+// Blocks of `block` threads that cover n items (a 1-D grid, or the x extent of one)
+inline unsigned blocks_for(long long n, int block) { return unsigned((n + block - 1) / block); }
 
 // Opt a kernel into > 48 KB of dynamic shared memory once per device (the attribute is per device and per function):
 // `done` is the caller's static per-device flag array.

@@ -363,13 +363,10 @@ extern "C" int icaf_compute_loss_fwd(const void* const* p, int p_fp32, int p_ld,
   if (e != cudaSuccess) return set_cuda_error(e, "compute_loss: cudaMemsetAsync");
   if (nt > 0) {
     const long long total = (long long)nl * nt * na * 5;
-    launch_k(loss_candidates_kernel, dim3((unsigned)((total + 127) / 128)), dim3(128), 0, st, P);
-    if (int rc = check_launch("compute_loss(candidates)")) return rc;
+    if (int rc = launch_k("compute_loss(candidates)", loss_candidates_kernel, dim3(blocks_for(total, 128)), dim3(128), 0, st, P)) return rc;
   }
-  launch_k(loss_obj_kernel, dim3(kLossObjBlocks, nl), dim3(256), 0, st, P);
-  if (int rc = check_launch("compute_loss(objectness)")) return rc;
-  launch_k(loss_finalize_kernel, dim3(1), dim3(256), 0, st, P);
-  return check_launch("compute_loss(finalize)");
+  if (int rc = launch_k("compute_loss(objectness)", loss_obj_kernel, dim3(kLossObjBlocks, nl), dim3(256), 0, st, P)) return rc;
+  return launch_k("compute_loss(finalize)", loss_finalize_kernel, dim3(1), dim3(256), 0, st, P);
 }
 
 extern "C" int icaf_compute_loss_bwd(const void* const* p, int p_fp32, int p_ld, const int* ny, const int* nx, int nl, int B, int na, int no,
@@ -390,9 +387,7 @@ extern "C" int icaf_compute_loss_bwd(const void* const* p, int p_fp32, int p_ld,
   if (e != cudaSuccess) return set_cuda_error(e, "compute_loss_bwd: cudaMemsetAsync");
   if (nt > 0) {
     const long long total = (long long)nl * nt * na * 5;
-    launch_k(loss_candidates_bwd_kernel, dim3((unsigned)((total + 127) / 128)), dim3(128), 0, st, P);
-    if (int rc = check_launch("compute_loss_bwd(candidates)")) return rc;
+    if (int rc = launch_k("compute_loss_bwd(candidates)", loss_candidates_bwd_kernel, dim3(blocks_for(total, 128)), dim3(128), 0, st, P)) return rc;
   }
-  launch_k(loss_obj_bwd_kernel, dim3(kLossObjBlocks, nl), dim3(256), 0, st, P);
-  return check_launch("compute_loss_bwd(objectness)");
+  return launch_k("compute_loss_bwd(objectness)", loss_obj_bwd_kernel, dim3(kLossObjBlocks, nl), dim3(256), 0, st, P);
 }

@@ -292,15 +292,16 @@ __device__ __forceinline__ void ld_cluster_v4(uint32_t addr, float4& v) {
   asm volatile("ld.shared::cluster.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr) : "memory");
 }
 
-// ------------------------------------------------------------------ counter-based dropout mask of the attention probabilities
-// keep(dir, batch*head, query, key): the training forward (attn.cu) and the backward (attn_bwd.cu) regenerate the same mask.
-__device__ __forceinline__ uint32_t attn_hash(uint32_t a, uint32_t b, uint32_t c) {
+// ------------------------------------------------------------------ counter-based dropout masks
+// A hash of (a, b, c): element-wise dropout (train.cu) and the attention probabilities' mask share it.
+__device__ __forceinline__ uint32_t dropout_hash(uint32_t a, uint32_t b, uint32_t c) {
   uint32_t h = a * 0x9E3779B1u ^ (b + 0x7F4A7C15u) * 0x85EBCA77u ^ (c + 0x165667B1u) * 0xC2B2AE3Du;
   h ^= h >> 15; h *= 0x2C1B3C6Du; h ^= h >> 12; h *= 0x297A2D39u; h ^= h >> 15;
   return h;
 }
+// keep(dir, batch*head, query, key): the training forward (attn.cu) and the backward (attn_bwd.cu) regenerate the same mask.
 __device__ __forceinline__ bool attn_keep(uint32_t seed, int dir, int bh, int q, int k, float p) {
-  const uint32_t h = attn_hash(uint32_t(q) * 65536u + uint32_t(k & 0xffff), uint32_t(bh) * 2u + uint32_t(dir) + (uint32_t(k) >> 16) * 0x10001u, seed);
+  const uint32_t h = dropout_hash(uint32_t(q) * 65536u + uint32_t(k & 0xffff), uint32_t(bh) * 2u + uint32_t(dir) + (uint32_t(k) >> 16) * 0x10001u, seed);
   return float(h >> 8) * (1.f / 16777216.f) >= p;
 }
 
@@ -312,5 +313,46 @@ __device__ __forceinline__ uint32_t pack_half2(float a, float b) {
   __half2 h = __floats2half2_rn(a, b);
   return *reinterpret_cast<uint32_t*>(&h);
 }
+
+// 8 fp16 values as one 16-byte vector: load (read-only path), unpack to fp32, pack from fp32, element-wise max
+__device__ __forceinline__ uint4 ldg16(const __half* p) { return __ldg(reinterpret_cast<const uint4*>(p)); }
+__device__ __forceinline__ void unpack8(const uint4& v, float (&f)[8]) {
+  const __half2* h = reinterpret_cast<const __half2*>(&v);
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    float2 t = __half22float2(h[i]);
+    f[2 * i] = t.x;
+    f[2 * i + 1] = t.y;
+  }
+}
+__device__ __forceinline__ uint4 pack8(const float (&f)[8]) {
+  uint4 v;
+  v.x = pack_half2(f[0], f[1]); v.y = pack_half2(f[2], f[3]);
+  v.z = pack_half2(f[4], f[5]); v.w = pack_half2(f[6], f[7]);
+  return v;
+}
+__device__ __forceinline__ uint4 hmax8(const uint4& a, const uint4& b) {
+  uint4 r;
+  const __half2* x = reinterpret_cast<const __half2*>(&a);
+  const __half2* y = reinterpret_cast<const __half2*>(&b);
+  __half2* z = reinterpret_cast<__half2*>(&r);
+#pragma unroll
+  for (int i = 0; i < 4; ++i) z[i] = __hmax2(x[i], y[i]);
+  return r;
+}
+// 8 consecutive fp32 values (16-byte aligned) through the read-only path
+__device__ __forceinline__ void ld8f(const float* __restrict__ p, float (&v)[8]) {
+  const float4 a = __ldg(reinterpret_cast<const float4*>(p)), b = __ldg(reinterpret_cast<const float4*>(p) + 1);
+  v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
+}
+
+// Arg-max codes of the max-pool backwards: the window position (< 256) of each of 8 channels, one byte per channel
+__device__ __forceinline__ uint2 pack_argmax8(const uint32_t (&arg)[8]) {
+  uint2 o;
+  o.x = arg[0] | (arg[1] << 8) | (arg[2] << 16) | (arg[3] << 24);
+  o.y = arg[4] | (arg[5] << 8) | (arg[6] << 16) | (arg[7] << 24);
+  return o;
+}
+__device__ __forceinline__ uint32_t argmax_code(const uint2& cd, int e) { return ((e < 4 ? cd.x : cd.y) >> (8 * (e & 3))) & 0xffu; }
 
 }  // namespace icaf

@@ -9,21 +9,7 @@ namespace icaf {
 
 constexpr int kRedChunks = 1024;      // upper bound of the row chunks of a two-stage reduction (sizes the workspace); the launch picks <= this many
 
-__device__ __forceinline__ void unpack8h(const uint4& v, float (&f)[8]) {
-  const __half2* h = reinterpret_cast<const __half2*>(&v);
-#pragma unroll
-  for (int i = 0; i < 4; ++i) { float2 t = __half22float2(h[i]); f[2 * i] = t.x; f[2 * i + 1] = t.y; }
-}
-__device__ __forceinline__ uint4 pack8h(const float (&f)[8]) {
-  uint4 v;
-  v.x = pack_half2(f[0], f[1]); v.y = pack_half2(f[2], f[3]); v.z = pack_half2(f[4], f[5]); v.w = pack_half2(f[6], f[7]);
-  return v;
-}
 __device__ __forceinline__ float sigmoidf_(float z) { return __fdividef(1.f, 1.f + __expf(-z)); }
-__device__ __forceinline__ void ld8f(const float* __restrict__ p, float (&v)[8]) {
-  const float4 a = __ldg(reinterpret_cast<const float4*>(p)), b = __ldg(reinterpret_cast<const float4*>(p) + 1);
-  v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
-}
 
 // ---------------------------------------------------------------------------------------------------------------
 // per-channel partial sums over row chunks: out[chunk][which][c], which = 0 / 1.
@@ -63,14 +49,14 @@ __global__ void __launch_bounds__(256) chan_partial_kernel(const __half* __restr
       const long long rb = r + rpp;
       const bool two = rb < r1;
       float xv[2][8], dv[2][8];
-      const uint4 xa = __ldg(reinterpret_cast<const uint4*>(x + r * C + cg * 8));
-      const uint4 xb = two ? __ldg(reinterpret_cast<const uint4*>(x + rb * C + cg * 8)) : make_uint4(0, 0, 0, 0);
+      const uint4 xa = ldg16(x + r * C + cg * 8);
+      const uint4 xb = two ? ldg16(x + rb * C + cg * 8) : make_uint4(0, 0, 0, 0);
       uint4 da = make_uint4(0, 0, 0, 0), db = make_uint4(0, 0, 0, 0);
       if (MODE != 0) {
-        da = __ldg(reinterpret_cast<const uint4*>(dy + r * C + cg * 8));
-        if (two) db = __ldg(reinterpret_cast<const uint4*>(dy + rb * C + cg * 8));
+        da = ldg16(dy + r * C + cg * 8);
+        if (two) db = ldg16(dy + rb * C + cg * 8);
       }
-      unpack8h(xa, xv[0]); unpack8h(xb, xv[1]); unpack8h(da, dv[0]); unpack8h(db, dv[1]);
+      unpack8(xa, xv[0]); unpack8(xb, xv[1]); unpack8(da, dv[0]); unpack8(db, dv[1]);
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         if (h == 1 && !two) break;
@@ -192,7 +178,7 @@ __global__ void __launch_bounds__(256) affine_act_kernel(const __half* __restric
   if (i >= n8) return;
   const int cg = int(i % C8), C = C8 * 8;
   float v[8], a[8], b[8];
-  unpack8h(__ldg(reinterpret_cast<const uint4*>(x) + i), v);
+  unpack8(ldg16(x + i * 8), v);
   ld8f(ab + cg * 8, a);
   ld8f(ab + C + cg * 8, b);
 #pragma unroll
@@ -200,7 +186,7 @@ __global__ void __launch_bounds__(256) affine_act_kernel(const __half* __restric
     const float z = fmaf(v[e], a[e], b[e]);
     v[e] = act ? z * sigmoidf_(z) : z;
   }
-  reinterpret_cast<uint4*>(y)[i] = pack8h(v);
+  reinterpret_cast<uint4*>(y)[i] = pack8(v);
 }
 // dx = a * (dz - k1 - (x - mean) * k2),  dz = dy * act'(z), z = x * a + b   (`coef` = [5][C]: a, b, mean, k1 = S1 / M, k2 = invstd * S2 / M)
 __global__ void __launch_bounds__(256) bn_bwd_apply_kernel(const __half* __restrict__ x, const __half* __restrict__ dy, const float* __restrict__ coef,
@@ -211,8 +197,8 @@ __global__ void __launch_bounds__(256) bn_bwd_apply_kernel(const __half* __restr
   if (i >= n8) return;
   const int cg = int(i % C8), C = C8 * 8;
   float xv[8], dv[8], a[8], b[8], m[8], k1[8], k2[8];
-  unpack8h(__ldg(reinterpret_cast<const uint4*>(x) + i), xv);
-  unpack8h(__ldg(reinterpret_cast<const uint4*>(dy) + i), dv);
+  unpack8(ldg16(x + i * 8), xv);
+  unpack8(ldg16(dy + i * 8), dv);
   ld8f(coef + cg * 8, a); ld8f(coef + C + cg * 8, b); ld8f(coef + 2 * C + cg * 8, m); ld8f(coef + 3 * C + cg * 8, k1); ld8f(coef + 4 * C + cg * 8, k2);
 #pragma unroll
   for (int e = 0; e < 8; ++e) {
@@ -220,16 +206,11 @@ __global__ void __launch_bounds__(256) bn_bwd_apply_kernel(const __half* __restr
     if (act) { const float z = fmaf(xv[e], a[e], b[e]); const float sg = sigmoidf_(z); dz *= sg * fmaf(z, 1.f - sg, 1.f); }
     xv[e] = a[e] * (dz - k1[e] - (xv[e] - m[e]) * k2[e]);
   }
-  reinterpret_cast<uint4*>(dx)[i] = pack8h(xv);
+  reinterpret_cast<uint4*>(dx)[i] = pack8(xv);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
 // element-wise: MODE 0 gelu(x) [erf], 1 dy * gelu'(x), 2 dropout (x * keep / (1 - p); the same call is its own backward on dy)
-__device__ __forceinline__ uint32_t hash_u32(uint32_t a, uint32_t b, uint32_t c) {
-  uint32_t h = a * 0x9E3779B1u ^ (b + 0x7F4A7C15u) * 0x85EBCA77u ^ (c + 0x165667B1u) * 0xC2B2AE3Du;
-  h ^= h >> 15; h *= 0x2C1B3C6Du; h ^= h >> 12; h *= 0x297A2D39u; h ^= h >> 15;
-  return h;
-}
 template <int MODE>
 __global__ void eltwise_kernel(const __half* __restrict__ x, const __half* __restrict__ dy, __half* __restrict__ y, long long n8, float p, uint32_t seed,
                                const uint32_t* __restrict__ seed_off) {
@@ -238,8 +219,8 @@ __global__ void eltwise_kernel(const __half* __restrict__ x, const __half* __res
   const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
   if (i >= n8) return;
   float xv[8], dv[8];
-  unpack8h(__ldg(reinterpret_cast<const uint4*>(x) + i), xv);
-  if (MODE == 1) unpack8h(__ldg(reinterpret_cast<const uint4*>(dy) + i), dv);
+  unpack8(ldg16(x + i * 8), xv);
+  if (MODE == 1) unpack8(ldg16(dy + i * 8), dv);
 #pragma unroll
   for (int e = 0; e < 8; ++e) {
     if (MODE == 0) xv[e] = gelu_erf_f(xv[e]);
@@ -250,11 +231,11 @@ __global__ void eltwise_kernel(const __half* __restrict__ x, const __half* __res
     }
     if (MODE == 2) {
       const long long idx = i * 8 + e;
-      const uint32_t h = hash_u32(uint32_t(idx), uint32_t(idx >> 32), seed + (seed_off ? __ldg(seed_off) : 0u));
+      const uint32_t h = dropout_hash(uint32_t(idx), uint32_t(idx >> 32), seed + (seed_off ? __ldg(seed_off) : 0u));
       xv[e] = (float(h >> 8) * (1.f / 16777216.f) >= p) ? xv[e] / (1.f - p) : 0.f;
     }
   }
-  reinterpret_cast<uint4*>(y)[i] = pack8h(xv);
+  reinterpret_cast<uint4*>(y)[i] = pack8(xv);
 }
 
 // LayerNorm backward, dx part (one warp per row, C <= 2048): dx = rstd * (g - mean(g) - xhat * mean(g * xhat)), g = dy * gamma
@@ -271,7 +252,7 @@ __global__ void ln_bwd_kernel(const __half* __restrict__ x, const __half* __rest
   for (int j = 0; j < 8; ++j) {
     const int ch = lane + 32 * j;
     if (ch < nch) {
-      unpack8h(__ldg(reinterpret_cast<const uint4*>(x + row * C + ch * 8)), xv[j]);
+      unpack8(ldg16(x + row * C + ch * 8), xv[j]);
 #pragma unroll
       for (int e = 0; e < 8; ++e) s += xv[j][e];
     }
@@ -293,7 +274,7 @@ __global__ void ln_bwd_kernel(const __half* __restrict__ x, const __half* __rest
   for (int j = 0; j < 8; ++j) {
     const int ch = lane + 32 * j;
     if (ch < nch) {
-      unpack8h(__ldg(reinterpret_cast<const uint4*>(dy + row * C + ch * 8)), gv[j]);
+      unpack8(ldg16(dy + row * C + ch * 8), gv[j]);
 #pragma unroll
       for (int e = 0; e < 8; ++e) {
         gv[j][e] *= gamma[ch * 8 + e];
@@ -312,7 +293,7 @@ __global__ void ln_bwd_kernel(const __half* __restrict__ x, const __half* __rest
       float o[8];
 #pragma unroll
       for (int e = 0; e < 8; ++e) o[e] = rstd * (gv[j][e] - sg - xv[j][e] * sgx);
-      *reinterpret_cast<uint4*>(dx + row * C + ch * 8) = pack8h(o);
+      *reinterpret_cast<uint4*>(dx + row * C + ch * 8) = pack8(o);
     }
   }
   if (lane == 0) { row_mean[row] = mean; row_rstd[row] = rstd; }
@@ -333,11 +314,11 @@ __global__ void upsample2x_bwd_kernel(const __half* __restrict__ dy, __half* __r
   for (int dyy = 0; dyy < 2; ++dyy)
     for (int dxx = 0; dxx < 2; ++dxx) {
       float v[8];
-      unpack8h(__ldg(reinterpret_cast<const uint4*>(dy + ((size_t(b) * 2 * H + 2 * y + dyy) * (2 * W) + 2 * x + dxx) * (C8 * 8) + c * 8)), v);
+      unpack8(ldg16(dy + ((size_t(b) * 2 * H + 2 * y + dyy) * (2 * W) + 2 * x + dxx) * (C8 * 8) + c * 8), v);
 #pragma unroll
       for (int e = 0; e < 8; ++e) acc[e] += v[e];
     }
-  reinterpret_cast<uint4*>(dx)[i] = pack8h(acc);
+  reinterpret_cast<uint4*>(dx)[i] = pack8(acc);
 }
 
 // MaxPool2d(5, 1, 2) backward (one stage of SPPF's chain): dx[q] = sum over the windows w containing q of dy[w] * [argmax_w == q],
@@ -366,16 +347,13 @@ __global__ void __launch_bounds__(256) maxpool5_argmax_kernel(const __half* __re
       const int xx = wx + kx - 2;
       if (xx < 0 || xx >= W) continue;
       float v[8];
-      unpack8h(__ldg(reinterpret_cast<const uint4*>(xb + (size_t(yy) * W + xx) * (C8 * 8))), v);
+      unpack8(ldg16(xb + (size_t(yy) * W + xx) * (C8 * 8)), v);
 #pragma unroll
       for (int e = 0; e < 8; ++e)
         if (v[e] > best[e]) { best[e] = v[e]; arg[e] = uint32_t(ky * 5 + kx); }
     }
   }
-  uint2 o;
-  o.x = arg[0] | (arg[1] << 8) | (arg[2] << 16) | (arg[3] << 24);
-  o.y = arg[4] | (arg[5] << 8) | (arg[6] << 16) | (arg[7] << 24);
-  code[i] = o;
+  code[i] = pack_argmax8(arg);
 }
 __global__ void __launch_bounds__(256) maxpool5_bwd_kernel(const uint2* __restrict__ code, const __half* __restrict__ dy, __half* __restrict__ dx, int B, int H, int W,
                                                            int C8) {
@@ -397,17 +375,15 @@ __global__ void __launch_bounds__(256) maxpool5_bwd_kernel(const uint2* __restri
       const uint2 cd = __ldg(code + w);
       const uint32_t mine = uint32_t((qy - wy + 2) * 5 + (qx - wx + 2));      // q's position code inside window w
       float g[8];
-      unpack8h(__ldg(reinterpret_cast<const uint4*>(dy) + w), g);
+      unpack8(ldg16(dy + w * 8), g);
 #pragma unroll
       for (int e = 0; e < 8; ++e) {
-        const uint32_t a = ((e < 4 ? cd.x : cd.y) >> (8 * (e & 3))) & 0xffu;
-        if (a == mine) acc[e] += g[e];
+        if (argmax_code(cd, e) == mine) acc[e] += g[e];
       }
     }
-  reinterpret_cast<uint4*>(dx)[i] = pack8h(acc);
+  reinterpret_cast<uint4*>(dx)[i] = pack8(acc);
 }
 
-static inline unsigned nblk(long long n, int bs) { return (unsigned)((n + bs - 1) / bs); }
 // row chunks of a two-stage channel reduction: about 8 blocks per SM over the whole grid, at least four passes of work per block
 static inline int pick_chunks(long long rows, int C, int cap_chunks = kRedChunks) {
   const int C8 = C / 8, bx = (C8 + 31) / 32, g = C8 < 32 ? C8 : 32, rpp = 256 / g;
@@ -432,15 +408,15 @@ extern "C" int icaf_bn_act_fwd(const void* x, const float* gamma, const float* b
   if (workspace_bytes < icaf_train_workspace_bytes(C)) return set_error(ICAF_ERR_BAD_ARG, "bn_act_fwd: workspace too small (icaf_train_workspace_bytes)");
   cudaStream_t st = (cudaStream_t)stream;
   const int chunks = pick_chunks(rows, C);
-  launch_k(chan_partial_kernel<0>, dim3(nblk(C / 8, 32), chunks), dim3(256), 0, st, (const __half*)x, (const __half*)nullptr, (const float*)nullptr,
-           (const float*)nullptr, (const float*)nullptr, (const float*)nullptr, workspace, (long long)rows, C, 0, chunks);
-  if (int rc = check_launch("bn_act_fwd(stats)")) return rc;
-  launch_k(bn_finalize_kernel, dim3(nblk(C, 32)), dim3(32, kFinLanes), 0, st, (const float*)workspace, save_mean, save_invstd, run_mean, run_var, C, (long long)rows, eps, momentum, chunks,
-           gamma, beta, workspace + size_t(kRedChunks) * 2 * C);
-  if (int rc = check_launch("bn_act_fwd(finalize)")) return rc;
+  if (int rc = launch_k("bn_act_fwd(stats)", chan_partial_kernel<0>, dim3(blocks_for(C / 8, 32), chunks), dim3(256), 0, st, (const __half*)x,
+                        (const __half*)nullptr, (const float*)nullptr, (const float*)nullptr, (const float*)nullptr, (const float*)nullptr, workspace,
+                        (long long)rows, C, 0, chunks)) return rc;
+  if (int rc = launch_k("bn_act_fwd(finalize)", bn_finalize_kernel, dim3(blocks_for(C, 32)), dim3(32, kFinLanes), 0, st, (const float*)workspace,
+                        save_mean, save_invstd, run_mean, run_var, C, (long long)rows, eps, momentum, chunks, gamma, beta,
+                        workspace + size_t(kRedChunks) * 2 * C)) return rc;
   const long long n8 = rows * (C / 8);
-  launch_k(affine_act_kernel, dim3(nblk(n8, 256)), dim3(256), 0, st, (const __half*)x, (const float*)(workspace + size_t(kRedChunks) * 2 * C), (__half*)y, n8, C / 8, act);
-  return check_launch("bn_act_fwd");
+  return launch_k("bn_act_fwd", affine_act_kernel, dim3(blocks_for(n8, 256)), dim3(256), 0, st, (const __half*)x,
+                  (const float*)(workspace + size_t(kRedChunks) * 2 * C), (__half*)y, n8, C / 8, act);
 }
 
 extern "C" int icaf_bn_act_bwd(const void* x, const void* dy, const float* gamma, const float* beta, const float* save_mean, const float* save_invstd,
@@ -451,16 +427,15 @@ extern "C" int icaf_bn_act_bwd(const void* x, const void* dy, const float* gamma
   cudaStream_t st = (cudaStream_t)stream;
   float* coef = workspace + size_t(kRedChunks) * 2 * C;     // [5][C] coefficients of the apply pass
   const int chunks = pick_chunks(rows, C);
-  launch_k(chan_partial_kernel<1>, dim3(nblk(C / 8, 32), chunks), dim3(256), 0, st, (const __half*)x, (const __half*)dy, gamma, beta, save_mean, save_invstd,
-           workspace, (long long)rows, C, act, chunks);
-  if (int rc = check_launch("bn_act_bwd(partial)")) return rc;
+  if (int rc = launch_k("bn_act_bwd(partial)", chan_partial_kernel<1>, dim3(blocks_for(C / 8, 32), chunks), dim3(256), 0, st, (const __half*)x,
+                        (const __half*)dy, gamma, beta, save_mean, save_invstd, workspace, (long long)rows, C, act, chunks)) return rc;
   // one second stage: the apply pass's coefficients and the parameter gradients dbeta = S1, dgamma = S2 (scaled by grad_scale)
-  launch_k(chan_final_kernel, dim3(nblk(C, 32)), dim3(32, kFinLanes), 0, st, (const float*)workspace, dbeta, dgamma, C, grad_scale, accumulate, chunks,
-           (float*)nullptr, (float*)nullptr, gamma, beta, save_mean, save_invstd, 1.0f / float(rows), coef);
-  if (int rc = check_launch("bn_act_bwd(sums)")) return rc;
+  if (int rc = launch_k("bn_act_bwd(sums)", chan_final_kernel, dim3(blocks_for(C, 32)), dim3(32, kFinLanes), 0, st, (const float*)workspace, dbeta,
+                        dgamma, C, grad_scale, accumulate, chunks, (float*)nullptr, (float*)nullptr, gamma, beta, save_mean, save_invstd,
+                        1.0f / float(rows), coef)) return rc;
   const long long n8 = rows * (C / 8);
-  launch_k(bn_bwd_apply_kernel, dim3(nblk(n8, 256)), dim3(256), 0, st, (const __half*)x, (const __half*)dy, (const float*)coef, (__half*)dx, n8, C / 8, act);
-  return check_launch("bn_act_bwd");
+  return launch_k("bn_act_bwd", bn_bwd_apply_kernel, dim3(blocks_for(n8, 256)), dim3(256), 0, st, (const __half*)x, (const __half*)dy,
+                  (const float*)coef, (__half*)dx, n8, C / 8, act);
 }
 
 // mode 0: y = gelu(x); 1: y = dy * gelu'(x); 2: y = dropout(x; p, seed) (apply it to dy with the same seed for the backward)
@@ -469,10 +444,9 @@ extern "C" int icaf_eltwise(int mode, const void* x, const void* dy, void* y, in
   if (n == 0) return ICAF_OK;
   cudaStream_t st = (cudaStream_t)stream;
   const long long n8 = n / 8;
-  if (mode == 0) launch_k(eltwise_kernel<0>, dim3(nblk(n8, 256)), dim3(256), 0, st, (const __half*)x, (const __half*)dy, (__half*)y, n8, p, seed, seed_offset_ptr());
-  else if (mode == 1) launch_k(eltwise_kernel<1>, dim3(nblk(n8, 256)), dim3(256), 0, st, (const __half*)x, (const __half*)dy, (__half*)y, n8, p, seed, seed_offset_ptr());
-  else launch_k(eltwise_kernel<2>, dim3(nblk(n8, 256)), dim3(256), 0, st, (const __half*)x, (const __half*)dy, (__half*)y, n8, p, seed, seed_offset_ptr());
-  return check_launch("eltwise");
+  auto kernel = mode == 0 ? eltwise_kernel<0> : (mode == 1 ? eltwise_kernel<1> : eltwise_kernel<2>);
+  return launch_k("eltwise", kernel, dim3(blocks_for(n8, 256)), dim3(256), 0, st, (const __half*)x, (const __half*)dy, (__half*)y, n8, p, seed,
+                  seed_offset_ptr());
 }
 
 extern "C" int icaf_layernorm_bwd(const void* x, const void* dy, const float* gamma, void* dx, float* dgamma, float* dbeta, int64_t rows, int C, float eps,
@@ -482,16 +456,16 @@ extern "C" int icaf_layernorm_bwd(const void* x, const void* dy, const float* ga
   cudaStream_t st = (cudaStream_t)stream;
   float* rmean = workspace + ws_floats(C);
   float* rrstd = rmean + rows;
-  launch_k(ln_bwd_kernel, dim3(nblk(rows, 4)), dim3(128), 0, st, (const __half*)x, (const __half*)dy, gamma, (__half*)dx, rmean, rrstd, (long long)rows, C, eps);
-  if (int rc = check_launch("layernorm_bwd(dx)")) return rc;
+  if (int rc = launch_k("layernorm_bwd(dx)", ln_bwd_kernel, dim3(blocks_for(rows, 4)), dim3(128), 0, st, (const __half*)x, (const __half*)dy, gamma,
+                        (__half*)dx, rmean, rrstd, (long long)rows, C, eps)) return rc;
   if (dgamma || dbeta) {
     const int chunks = pick_chunks(rows, C);
-    launch_k(chan_partial_kernel<2>, dim3(nblk(C / 8, 32), chunks), dim3(256), 0, st, (const __half*)x, (const __half*)dy, (const float*)nullptr, (const float*)nullptr,
-             (const float*)rmean, (const float*)rrstd, workspace, (long long)rows, C, 0, chunks);
-    if (int rc = check_launch("layernorm_bwd(partial)")) return rc;
-    launch_k(chan_final_kernel, dim3(nblk(C, 32)), dim3(32, kFinLanes), 0, st, (const float*)workspace, dbeta, dgamma, C, grad_scale, accumulate, chunks,
-             (float*)nullptr, (float*)nullptr, (const float*)nullptr, (const float*)nullptr, (const float*)nullptr, (const float*)nullptr, 0.f, (float*)nullptr);
-    if (int rc = check_launch("layernorm_bwd(param grads)")) return rc;
+    if (int rc = launch_k("layernorm_bwd(partial)", chan_partial_kernel<2>, dim3(blocks_for(C / 8, 32), chunks), dim3(256), 0, st, (const __half*)x,
+                          (const __half*)dy, (const float*)nullptr, (const float*)nullptr, (const float*)rmean, (const float*)rrstd, workspace,
+                          (long long)rows, C, 0, chunks)) return rc;
+    if (int rc = launch_k("layernorm_bwd(param grads)", chan_final_kernel, dim3(blocks_for(C, 32)), dim3(32, kFinLanes), 0, st,
+                          (const float*)workspace, dbeta, dgamma, C, grad_scale, accumulate, chunks, (float*)nullptr, (float*)nullptr,
+                          (const float*)nullptr, (const float*)nullptr, (const float*)nullptr, (const float*)nullptr, 0.f, (float*)nullptr)) return rc;
   }
   return ICAF_OK;
 }
@@ -503,17 +477,16 @@ extern "C" int icaf_dot(const void* x, const void* y, int64_t rows, int C, float
   if (workspace_bytes < icaf_train_workspace_bytes(C)) return set_error(ICAF_ERR_BAD_ARG, "dot: workspace too small");
   cudaStream_t st = (cudaStream_t)stream;
   const int chunks = pick_chunks(rows, C, 64);
-  launch_k(chan_partial_kernel<3>, dim3(nblk(C / 8, 32), chunks), dim3(256), 0, st, (const __half*)x, (const __half*)y, (const float*)nullptr, (const float*)nullptr,
-           (const float*)nullptr, (const float*)nullptr, workspace, (long long)rows, C, 0, chunks);
-  if (int rc = check_launch("dot(partial)")) return rc;
-  launch_k(scalar_final_kernel, dim3(1), dim3(1024), 0, st, (const float*)workspace, out, C, scale, accumulate, chunks);
-  return check_launch("dot");
+  if (int rc = launch_k("dot(partial)", chan_partial_kernel<3>, dim3(blocks_for(C / 8, 32), chunks), dim3(256), 0, st, (const __half*)x,
+                        (const __half*)y, (const float*)nullptr, (const float*)nullptr, (const float*)nullptr, (const float*)nullptr, workspace,
+                        (long long)rows, C, 0, chunks)) return rc;
+  return launch_k("dot", scalar_final_kernel, dim3(1), dim3(1024), 0, st, (const float*)workspace, out, C, scale, accumulate, chunks);
 }
 
 extern "C" int icaf_upsample2x_bwd(const void* dy, void* dx, int B, int H, int W, int C, void* stream) {
   if (!dy || !dx || C % 8) return set_error(ICAF_ERR_BAD_ARG, "upsample2x_bwd: bad argument");
-  launch_k(upsample2x_bwd_kernel, dim3(nblk((long long)B * H * W * (C / 8), 256)), dim3(256), 0, (cudaStream_t)stream, (const __half*)dy, (__half*)dx, B, H, W, C / 8);
-  return check_launch("upsample2x_bwd");
+  return launch_k("upsample2x_bwd", upsample2x_bwd_kernel, dim3(blocks_for((long long)B * H * W * (C / 8), 256)), dim3(256), 0, (cudaStream_t)stream,
+                  (const __half*)dy, (__half*)dx, B, H, W, C / 8);
 }
 
 extern "C" int icaf_maxpool5_bwd(const void* x, const void* dy, void* dx, int B, int H, int W, int C, void* workspace, size_t workspace_bytes, void* stream) {
@@ -521,8 +494,8 @@ extern "C" int icaf_maxpool5_bwd(const void* x, const void* dy, void* dx, int B,
   if (workspace_bytes < size_t(B) * H * W * C || (reinterpret_cast<uintptr_t>(workspace) & 7)) return set_error(ICAF_ERR_BAD_ARG, "maxpool5_bwd: workspace needs B*H*W*C bytes, 8-byte aligned");
   const long long n8 = (long long)B * H * W * (C / 8);
   cudaStream_t st = (cudaStream_t)stream;
-  launch_k(maxpool5_argmax_kernel, dim3(nblk(n8, 256)), dim3(256), 0, st, (const __half*)x, (uint2*)workspace, B, H, W, C / 8);
-  if (int rc = check_launch("maxpool5_bwd(argmax)")) return rc;
-  launch_k(maxpool5_bwd_kernel, dim3(nblk(n8, 256)), dim3(256), 0, st, (const uint2*)workspace, (const __half*)dy, (__half*)dx, B, H, W, C / 8);
-  return check_launch("maxpool5_bwd");
+  if (int rc = launch_k("maxpool5_bwd(argmax)", maxpool5_argmax_kernel, dim3(blocks_for(n8, 256)), dim3(256), 0, st, (const __half*)x,
+                        (uint2*)workspace, B, H, W, C / 8)) return rc;
+  return launch_k("maxpool5_bwd", maxpool5_bwd_kernel, dim3(blocks_for(n8, 256)), dim3(256), 0, st, (const uint2*)workspace, (const __half*)dy,
+                  (__half*)dx, B, H, W, C / 8);
 }

@@ -295,24 +295,21 @@ extern "C" int icaf_conv2d_wgrad(const icaf_conv_geom* g, const void* x, int64_t
   static bool configured[kMaxDevices] = {false};
   if (int r2 = configure_smem(wgrad_kernel, kWSmem, configured, "wgrad: cudaFuncSetAttribute")) return r2;
   cudaStream_t st = (cudaStream_t)stream;
-  launch_k(wgrad_kernel, dim3(pl.grid), dim3(288), (size_t)kWSmem, st, P, maps);
-  if (int r3 = check_launch("conv2d_wgrad")) return r3;
+  if (int r3 = launch_k("conv2d_wgrad", wgrad_kernel, dim3(pl.grid), dim3(288), (size_t)kWSmem, st, P, maps)) return r3;
   if (P.taps == 1) {
-    launch_k(wgrad_reduce_flat_kernel, dim3((unsigned)(((long long)g->Cout * g->Cin + 255) / 256)), dim3(256), 0, st, (const float*)P.partial, dw, P.splits, P.n_pad,
-             P.c_pad, g->Cout, g->Cin, scale, accumulate);
-    return check_launch("conv2d_wgrad(reduce)");
+    return launch_k("conv2d_wgrad(reduce)", wgrad_reduce_flat_kernel, dim3(blocks_for((long long)g->Cout * g->Cin, 256)), dim3(256), 0, st,
+                    (const float*)P.partial, dw, P.splits, P.n_pad, P.c_pad, g->Cout, g->Cin, scale, accumulate);
   }
   const unsigned red_blocks = (unsigned)g->Cout * (unsigned)((g->Cin + kRedC - 1) / kRedC);
-  launch_k(wgrad_reduce_kernel, dim3(red_blocks), dim3(256), size_t(P.taps) * (kRedC + 1) * sizeof(float), st, (const float*)P.partial, dw, P.splits, P.n_pad,
-           P.taps, P.c_pad, g->Cout, g->Cin, scale, accumulate);
-  return check_launch("conv2d_wgrad(reduce)");
+  return launch_k("conv2d_wgrad(reduce)", wgrad_reduce_kernel, dim3(red_blocks), dim3(256), size_t(P.taps) * (kRedC + 1) * sizeof(float), st,
+                  (const float*)P.partial, dw, P.splits, P.n_pad, P.taps, P.c_pad, g->Cout, g->Cin, scale, accumulate);
 }
 
 extern "C" int icaf_zero_stuff2(const void* x, void* y, int B, int H, int W, int C, int H2, int W2, void* stream) {
   if (!x || !y || C % 8 || B < 1 || H2 < 2 * H - 1 || W2 < 2 * W - 1) return set_error(ICAF_ERR_BAD_ARG, "zero_stuff2: bad argument");
   const long long total = (long long)B * H2 * W2 * (C / 8);
-  launch_k(zero_stuff2_kernel, dim3((unsigned)((total + 255) / 256)), dim3(256), 0, (cudaStream_t)stream, (const __half*)x, (__half*)y, B, H, W, C / 8, H2, W2);
-  return check_launch("zero_stuff2");
+  return launch_k("zero_stuff2", zero_stuff2_kernel, dim3(blocks_for(total, 256)), dim3(256), 0, (cudaStream_t)stream, (const __half*)x, (__half*)y,
+                  B, H, W, C / 8, H2, W2);
 }
 
 extern "C" int icaf_colsum(const void* x, int64_t rows, int C, float* out, float scale, int accumulate, float* workspace, size_t workspace_bytes,
@@ -321,8 +318,8 @@ extern "C" int icaf_colsum(const void* x, int64_t rows, int C, float* out, float
   if (!x || !out || !workspace || rows < 1 || C < 1) return set_error(ICAF_ERR_BAD_ARG, "colsum: bad argument");
   if (workspace_bytes < size_t(kChunks) * C * sizeof(float)) return set_error(ICAF_ERR_BAD_ARG, "colsum: workspace needs 64 * C floats");
   cudaStream_t st = (cudaStream_t)stream;
-  launch_k(colsum_partial_kernel, dim3((unsigned)((C + 127) / 128), kChunks), dim3(128), 0, st, (const __half*)x, workspace, (long long)rows, C, kChunks);
-  if (int rc = check_launch("colsum(partial)")) return rc;
-  launch_k(colsum_final_kernel, dim3((unsigned)((C + 127) / 128)), dim3(128), 0, st, (const float*)workspace, out, C, kChunks, scale, accumulate);
-  return check_launch("colsum");
+  if (int rc = launch_k("colsum(partial)", colsum_partial_kernel, dim3(blocks_for(C, 128), kChunks), dim3(128), 0, st, (const __half*)x, workspace,
+                        (long long)rows, C, kChunks)) return rc;
+  return launch_k("colsum", colsum_final_kernel, dim3(blocks_for(C, 128)), dim3(128), 0, st, (const float*)workspace, out, C, kChunks, scale,
+                  accumulate);
 }
