@@ -3,7 +3,7 @@
 ``loss.backward()`` (train.py:344) on the output of ``Model.forward`` in training mode runs these nodes: every forward and
 every backward computation is a kernel of libicaf_b200 (wgmma implicit-GEMM convolutions for the forward, data- and
 weight-gradient passes; the BatchNorm / SiLU / LayerNorm / GELU / dropout / pooling / attention kernels of csrc/train.cu,
-attn_bwd.cu, dmff_bwd.cu).  torch provides the graph walk, the gradient accumulation where a tensor has several consumers,
+pool.cu, dmff.cu, attn_bwd.cu).  torch provides the graph walk, the gradient accumulation where a tensor has several consumers,
 and the ``.grad`` buffers -- so the reference's optimiser, GradScaler, EMA and DDP (train.py:120-235) work unchanged.
 
 Activations and activation gradients are fp16 NHWC (the reference trains under autocast, train.py:334); parameters stay

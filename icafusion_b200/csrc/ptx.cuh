@@ -346,6 +346,13 @@ __device__ __forceinline__ void ld8f(const float* __restrict__ p, float (&v)[8])
   v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
 }
 
+// Coordinates of 16-byte vector i of a (B, H, W, 8 * C8) NHWC map: channel chunk c of pixel p = (b * H + y) * W + x
+struct Nhwc8 { int c; long long p; int x, y, b; };
+__device__ __forceinline__ Nhwc8 nhwc8(long long i, int H, int W, int C8) {
+  const long long p = i / C8, t = p / W;
+  return {int(i % C8), p, int(p % W), int(t % H), int(t / H)};
+}
+
 // Arg-max codes of the max-pool backwards: the window position (< 256) of each of 8 channels, one byte per channel
 __device__ __forceinline__ uint2 pack_argmax8(const uint32_t (&arg)[8]) {
   uint2 o;
@@ -354,5 +361,34 @@ __device__ __forceinline__ uint2 pack_argmax8(const uint32_t (&arg)[8]) {
   return o;
 }
 __device__ __forceinline__ uint32_t argmax_code(const uint2& cd, int e) { return ((e < 4 ? cd.x : cd.y) >> (8 * (e & 3))) & 0xffu; }
+
+// LayerNorm statistics of row `row` of a (rows, C <= 2048) fp16 matrix, one warp per row (the forward and the backward share
+// them): lane l caches the row's 16-byte chunks l, l + 32, ... in v[0..7]; every lane gets the mean and 1 / sqrt(var + eps),
+// the variance taken in a second pass over the registers.
+__device__ __forceinline__ void ln_row_moments(const __half* x, long long row, int C, float eps, float (&v)[8][8], float& mean, float& rstd) {
+  const int lane = threadIdx.x & 31, nch = C >> 3;
+  float s = 0.f;
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    const int ch = lane + 32 * j;
+    if (ch < nch) {
+      unpack8(ldg16(x + row * C + ch * 8), v[j]);
+#pragma unroll
+      for (int e = 0; e < 8; ++e) s += v[j][e];
+    }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+  mean = s / float(C);
+  float q = 0.f;
+#pragma unroll
+  for (int j = 0; j < 8; ++j)
+    if (lane + 32 * j < nch)
+#pragma unroll
+      for (int e = 0; e < 8; ++e) { const float d = v[j][e] - mean; q += d * d; }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) q += __shfl_xor_sync(0xffffffffu, q, o);
+  rstd = rsqrtf(q / float(C) + eps);
+}
 
 }  // namespace icaf

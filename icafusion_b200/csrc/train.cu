@@ -1,6 +1,6 @@
 // Training-mode kernels of the hot path that are not GEMMs (forward and backward): BatchNorm with batch statistics + SiLU
-// (Conv.forward, models/common.py:56-57), exact-erf GELU, LayerNorm backward, the SPPF max-pool chain, nearest up-sampling,
-// the DMFF token pooling / nearest tail, dropout, and the small reductions behind scalar-parameter gradients.
+// (Conv.forward, models/common.py:56-57), exact-erf GELU and dropout, the LayerNorm backward (its parameter gradients are
+// two-stage channel reductions; the forward is in dmff.cu), and the small reductions behind scalar-parameter gradients.
 // fp16 activations / gradients, fp32 statistics and parameter gradients.  Every reduction is two-stage with a fixed
 // summation order (deterministic; the reference trains with torch.use_deterministic_algorithms, utils/general.py:53-54).
 #include "icaf_internal.cuh"
@@ -246,29 +246,8 @@ __global__ void ln_bwd_kernel(const __half* __restrict__ x, const __half* __rest
   const long long row = blockIdx.x * (long long)(blockDim.x >> 5) + (threadIdx.x >> 5);
   if (row >= rows) return;
   const int lane = threadIdx.x & 31, nch = C >> 3;
-  float xv[8][8], gv[8][8];
-  float s = 0.f;
-#pragma unroll
-  for (int j = 0; j < 8; ++j) {
-    const int ch = lane + 32 * j;
-    if (ch < nch) {
-      unpack8(ldg16(x + row * C + ch * 8), xv[j]);
-#pragma unroll
-      for (int e = 0; e < 8; ++e) s += xv[j][e];
-    }
-  }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-  const float mean = s / float(C);
-  float q = 0.f;
-#pragma unroll
-  for (int j = 0; j < 8; ++j)
-    if (lane + 32 * j < nch)
-#pragma unroll
-      for (int e = 0; e < 8; ++e) { const float d = xv[j][e] - mean; q += d * d; }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) q += __shfl_xor_sync(0xffffffffu, q, o);
-  const float rstd = rsqrtf(q / float(C) + eps);
+  float xv[8][8], gv[8][8], mean, rstd;
+  ln_row_moments(x, row, C, eps, xv, mean, rstd);
   float sg = 0.f, sgx = 0.f;
 #pragma unroll
   for (int j = 0; j < 8; ++j) {
@@ -297,91 +276,6 @@ __global__ void ln_bwd_kernel(const __half* __restrict__ x, const __half* __rest
     }
   }
   if (lane == 0) { row_mean[row] = mean; row_rstd[row] = rstd; }
-}
-
-// nearest 2x up-sampling backward: dx[b, y, x] = sum of the 2x2 block of dy
-__global__ void upsample2x_bwd_kernel(const __half* __restrict__ dy, __half* __restrict__ dx, int B, int H, int W, int C8) {
-  pdl_launch_dependents();
-  pdl_wait();
-  const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
-  if (i >= (long long)B * H * W * C8) return;
-  const int c = int(i % C8);
-  long long p = i / C8;
-  const int x = int(p % W);
-  p /= W;
-  const int y = int(p % H), b = int(p / H);
-  float acc[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-  for (int dyy = 0; dyy < 2; ++dyy)
-    for (int dxx = 0; dxx < 2; ++dxx) {
-      float v[8];
-      unpack8(ldg16(dy + ((size_t(b) * 2 * H + 2 * y + dyy) * (2 * W) + 2 * x + dxx) * (C8 * 8) + c * 8), v);
-#pragma unroll
-      for (int e = 0; e < 8; ++e) acc[e] += v[e];
-    }
-  reinterpret_cast<uint4*>(dx)[i] = pack8(acc);
-}
-
-// MaxPool2d(5, 1, 2) backward (one stage of SPPF's chain): dx[q] = sum over the windows w containing q of dy[w] * [argmax_w == q],
-// argmax = first maximum in row-major window order (torch's max_pool2d_with_indices).  Two gather kernels, deterministic:
-//   1. per window (= per output pixel) and channel: the position code (ky*5 + kx) of its first maximum -> one byte;
-//   2. per input pixel q: the <= 25 windows that contain q; those whose code points at q contribute their dy.
-__global__ void __launch_bounds__(256) maxpool5_argmax_kernel(const __half* __restrict__ x, uint2* __restrict__ code, int B, int H, int W, int C8) {
-  pdl_launch_dependents();
-  pdl_wait();
-  const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
-  if (i >= (long long)B * H * W * C8) return;
-  const int c = int(i % C8);
-  long long p = i / C8;
-  const int wx = int(p % W);
-  p /= W;
-  const int wy = int(p % H), b = int(p / H);
-  const __half* xb = x + (size_t(b) * H * W) * (C8 * 8) + c * 8;
-  float best[8];
-  uint32_t arg[8];
-#pragma unroll
-  for (int e = 0; e < 8; ++e) { best[e] = -INFINITY; arg[e] = 0u; }
-  for (int ky = 0; ky < 5; ++ky) {
-    const int yy = wy + ky - 2;
-    if (yy < 0 || yy >= H) continue;
-    for (int kx = 0; kx < 5; ++kx) {
-      const int xx = wx + kx - 2;
-      if (xx < 0 || xx >= W) continue;
-      float v[8];
-      unpack8(ldg16(xb + (size_t(yy) * W + xx) * (C8 * 8)), v);
-#pragma unroll
-      for (int e = 0; e < 8; ++e)
-        if (v[e] > best[e]) { best[e] = v[e]; arg[e] = uint32_t(ky * 5 + kx); }
-    }
-  }
-  code[i] = pack_argmax8(arg);
-}
-__global__ void __launch_bounds__(256) maxpool5_bwd_kernel(const uint2* __restrict__ code, const __half* __restrict__ dy, __half* __restrict__ dx, int B, int H, int W,
-                                                           int C8) {
-  pdl_launch_dependents();
-  pdl_wait();
-  const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
-  if (i >= (long long)B * H * W * C8) return;
-  const int c = int(i % C8);
-  long long p = i / C8;
-  const int qx = int(p % W);
-  p /= W;
-  const int qy = int(p % H), b = int(p / H);
-  float acc[8];
-#pragma unroll
-  for (int e = 0; e < 8; ++e) acc[e] = 0.f;
-  for (int wy = max(qy - 2, 0); wy <= min(qy + 2, H - 1); ++wy)
-    for (int wx = max(qx - 2, 0); wx <= min(qx + 2, W - 1); ++wx) {
-      const size_t w = ((size_t(b) * H + wy) * W + wx) * C8 + c;
-      const uint2 cd = __ldg(code + w);
-      const uint32_t mine = uint32_t((qy - wy + 2) * 5 + (qx - wx + 2));      // q's position code inside window w
-      float g[8];
-      unpack8(ldg16(dy + w * 8), g);
-#pragma unroll
-      for (int e = 0; e < 8; ++e) {
-        if (argmax_code(cd, e) == mine) acc[e] += g[e];
-      }
-    }
-  reinterpret_cast<uint4*>(dx)[i] = pack8(acc);
 }
 
 // row chunks of a two-stage channel reduction: about 8 blocks per SM over the whole grid, at least four passes of work per block
@@ -481,21 +375,4 @@ extern "C" int icaf_dot(const void* x, const void* y, int64_t rows, int C, float
                         (const __half*)y, (const float*)nullptr, (const float*)nullptr, (const float*)nullptr, (const float*)nullptr, workspace,
                         (long long)rows, C, 0, chunks)) return rc;
   return launch_k("dot", scalar_final_kernel, dim3(1), dim3(1024), 0, st, (const float*)workspace, out, C, scale, accumulate, chunks);
-}
-
-extern "C" int icaf_upsample2x_bwd(const void* dy, void* dx, int B, int H, int W, int C, void* stream) {
-  if (!dy || !dx || C % 8) return set_error(ICAF_ERR_BAD_ARG, "upsample2x_bwd: bad argument");
-  return launch_k("upsample2x_bwd", upsample2x_bwd_kernel, dim3(blocks_for((long long)B * H * W * (C / 8), 256)), dim3(256), 0, (cudaStream_t)stream,
-                  (const __half*)dy, (__half*)dx, B, H, W, C / 8);
-}
-
-extern "C" int icaf_maxpool5_bwd(const void* x, const void* dy, void* dx, int B, int H, int W, int C, void* workspace, size_t workspace_bytes, void* stream) {
-  if (!x || !dy || !dx || !workspace || C % 8 || B < 1 || H < 1 || W < 1) return set_error(ICAF_ERR_BAD_ARG, "maxpool5_bwd: null pointer or C % 8");
-  if (workspace_bytes < size_t(B) * H * W * C || (reinterpret_cast<uintptr_t>(workspace) & 7)) return set_error(ICAF_ERR_BAD_ARG, "maxpool5_bwd: workspace needs B*H*W*C bytes, 8-byte aligned");
-  const long long n8 = (long long)B * H * W * (C / 8);
-  cudaStream_t st = (cudaStream_t)stream;
-  if (int rc = launch_k("maxpool5_bwd(argmax)", maxpool5_argmax_kernel, dim3(blocks_for(n8, 256)), dim3(256), 0, st, (const __half*)x,
-                        (uint2*)workspace, B, H, W, C / 8)) return rc;
-  return launch_k("maxpool5_bwd", maxpool5_bwd_kernel, dim3(blocks_for(n8, 256)), dim3(256), 0, st, (const uint2*)workspace, (const __half*)dy,
-                  (__half*)dx, B, H, W, C / 8);
 }

@@ -10,6 +10,7 @@
 //   D[128 n][c tile] in registers and writes one fp32 partial; wgrad_reduce_kernel sums the splits in a fixed order into the
 //   (Cout, Cin, kh, kw) fp32 gradient (deterministic: no atomics).
 // 288 threads: warps 0-7 two consumer warpgroups (n rows 0-63 / 64-127 of the tile), warp 8 TMA producer.
+// Also here: the fp32 -> fp16 filter packing and the zero-stuffing the training GEMMs consume, and the bias-gradient column sums.
 #include <cstring>
 
 #include "icaf_internal.cuh"
@@ -226,6 +227,48 @@ __global__ void colsum_final_kernel(const float* __restrict__ part, float* __res
   out[c] = (accumulate ? out[c] : 0.f) + scale * s;
 }
 
+// Element i of a packed [rows][k_pad] filter bank (pad rows / columns are 0):
+//   forward:         out[n][(ky*kw + kx)*chan_p + c]                  = w[n][c][ky][kx]      (rows >= Cout, k_pad >= kh*kw*chan_p)
+//   flip_transpose:  out[c][((kh-1-ky)*kw + (kw-1-kx))*chan_p + n]    = w[n][c][ky][kx]      (rows >= Cin,  k_pad >= kh*kw*chan_p)
+__device__ __forceinline__ __half packed_weight(const float* __restrict__ w, long long i, int k_pad, int chan_p, int Cout, int Cin, int kh,
+                                                int kw, bool flip_transpose) {
+  const int r = int(i / k_pad), k = int(i - (long long)r * k_pad);
+  const int tap = k / chan_p, ch = k - tap * chan_p;
+  float v = 0.f;
+  if (tap < kh * kw) {
+    const int ky = tap / kw, kx = tap - ky * kw;
+    if (!flip_transpose) {
+      if (r < Cout && ch < Cin) v = w[(((long long)r * Cin + ch) * kh + ky) * kw + kx];
+    } else {
+      if (r < Cin && ch < Cout) v = w[(((long long)ch * Cin + r) * kh + (kh - 1 - ky)) * kw + (kw - 1 - kx)];
+    }
+  }
+  return __float2half(v);
+}
+
+// mode 0: the forward bank; mode 1: the flipped and transposed one
+__global__ void __launch_bounds__(256) pack_weight_kernel(const float* __restrict__ w, __half* __restrict__ out, int Cout, int Cin, int kh, int kw,
+                                                          int chan_p, int rows, int k_pad, int mode) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const long long i = blockIdx.x * 256ll + threadIdx.x;
+  if (i >= (long long)rows * k_pad) return;
+  out[i] = packed_weight(w, i, k_pad, chan_p, Cout, Cin, kh, kw, mode != 0);
+}
+
+// both banks of one filter in one launch (the training step packs every filter once per step, forward and data-gradient form)
+__global__ void __launch_bounds__(256) pack_weight_pair_kernel(const float* __restrict__ w, __half* __restrict__ out_f, __half* __restrict__ out_d, int Cout, int Cin,
+                                                               int kh, int kw, int rows_f, int kpad_f, int chan_d, int rows_d, int kpad_d) {
+  pdl_launch_dependents();
+  pdl_wait();
+  long long i = blockIdx.x * 256ll + threadIdx.x;
+  const long long nf = (long long)rows_f * kpad_f, nd = (long long)rows_d * kpad_d;
+  if (i >= nf + nd) return;
+  const bool dg = i >= nf;
+  if (dg) i -= nf;
+  (dg ? out_d : out_f)[i] = packed_weight(w, i, dg ? kpad_d : kpad_f, dg ? chan_d : Cin, Cout, Cin, kh, kw, dg);
+}
+
 struct WgradPlan { WgradParams P; int grid; size_t ws_bytes; };
 
 static int plan_wgrad(const icaf_conv_geom* g, int sms, WgradPlan& pl) {
@@ -322,4 +365,24 @@ extern "C" int icaf_colsum(const void* x, int64_t rows, int C, float* out, float
                         (long long)rows, C, kChunks)) return rc;
   return launch_k("colsum", colsum_final_kernel, dim3(blocks_for(C, 128)), dim3(128), 0, st, (const float*)workspace, out, C, kChunks, scale,
                   accumulate);
+}
+
+extern "C" int icaf_pack_weight(const float* w, int Cout, int Cin, int kh, int kw, int chan_pad, int rows, int k_pad, int transpose_flip, void* out,
+                                void* stream) {
+  if (!w || !out || Cout < 1 || Cin < 1 || kh < 1 || kw < 1) return set_error(ICAF_ERR_BAD_ARG, "pack_weight: bad argument");
+  const int chan = transpose_flip ? Cout : Cin, need_rows = transpose_flip ? Cin : Cout;
+  if (chan_pad < chan || rows < need_rows || k_pad < kh * kw * chan_pad) return set_error(ICAF_ERR_BAD_ARG, "pack_weight: padded sizes smaller than the filter");
+  const long long total = (long long)rows * k_pad;
+  return launch_k("pack_weight", pack_weight_kernel, dim3(blocks_for(total, 256)), dim3(256), 0, (cudaStream_t)stream, w, (__half*)out, Cout, Cin, kh,
+                  kw, chan_pad, rows, k_pad, transpose_flip ? 1 : 0);
+}
+
+extern "C" int icaf_pack_weight_pair(const float* w, int Cout, int Cin, int kh, int kw, int rows_f, int kpad_f, void* out_fwd, int chan_pad_d, int rows_d,
+                                     int kpad_d, void* out_dgrad, void* stream) {
+  if (!w || !out_fwd || !out_dgrad || Cout < 1 || Cin < 1 || kh < 1 || kw < 1) return set_error(ICAF_ERR_BAD_ARG, "pack_weight_pair: bad argument");
+  if (rows_f < Cout || kpad_f < kh * kw * Cin || chan_pad_d < Cout || rows_d < Cin || kpad_d < kh * kw * chan_pad_d)
+    return set_error(ICAF_ERR_BAD_ARG, "pack_weight_pair: padded sizes smaller than the filter");
+  const long long total = (long long)rows_f * kpad_f + (long long)rows_d * kpad_d;
+  return launch_k("pack_weight_pair", pack_weight_pair_kernel, dim3(blocks_for(total, 256)), dim3(256), 0, (cudaStream_t)stream, w, (__half*)out_fwd,
+                  (__half*)out_dgrad, Cout, Cin, kh, kw, rows_f, kpad_f, chan_pad_d, rows_d, kpad_d);
 }
