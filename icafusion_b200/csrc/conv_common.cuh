@@ -34,6 +34,7 @@ struct ConvParams {
   float ln_eps, ln_inv_k;                 // LN fold: epsilon, 1 / (normalised features = K)
   int m_tiles, n_tiles, tiles;            // persistent kernel: tile grid (m, n, problem) and its product
   int tma_epi;                            // register epilogue + TMA-stored output tile (else staged rows), set by plan_conv
+  int halo_bytes;                         // persistent stride-1 3x3: bytes of one input-halo slot (0: a shifted box per tap)
 };
 struct ConvMaps {          // TMA descriptors, passed by value as a __grid_constant__ kernel parameter
   CUtensorMap w[2];

@@ -24,9 +24,13 @@
 // keep the staged rows.  plan_conv makes that choice for both kernels (ConvParams::tma_epi).
 // conv_gemm_persist_kernel: BN = 128 grids of more than one wave with TMA-staged A -- one persistent CTA per SM, a TMA
 // producer warpgroup and two consumer warpgroups that take turns on the main loop; each consumer runs the epilogue on its
-// accumulator registers and writes the tile with TMA stores (see its own comment below).
+// accumulator registers and writes the tile with TMA stores (see its own comment below).  Its stride-1 3x3 launches
+// (pad 1, A_TMA4D) stage A differently: one (64 ch, tw+2, th+2) input halo per 64-channel block feeds all nine taps, with
+// the A fragments read from it by ldmatrix (wgmma RS, halo_mma_loop), instead of nine shifted boxes that each bring the
+// same pixels in again from L2.
 // The two kernels share the TMA producer stage (load_stage), the main loop (mma_loop), the tile origin, the per-element
-// epilogue expression (epi_value), so they compute bit-identical tiles, and every other epilogue piece (conv_common.cuh):
+// epilogue expression (epi_value), so they compute bit-identical tiles (the halo launches sum K in another order: equal up
+// to fp32 summation order), and every other epilogue piece (conv_common.cuh):
 // register epilogue (fragment_row_bias, epi_tile_fragments, tma_store_tile, tma_load_tile), staged rows (staged_row,
 // epi_staged_chunk) and the mode selection (epi_mode_act).
 #include <cstdlib>
@@ -361,17 +365,86 @@ conv_gemm_tc_kernel(const ConvParams P, const __grid_constant__ ConvMaps maps) {
 // into the same buffer when the tile starts and overwritten in place.  XM (LayerNorm fold / row statistics) keeps the
 // row epilogue of epi_chunk: the accumulators are staged 32 columns at a time through the first 18 KB of the buffer
 // (thread t owns tile row t).
+// Halo launches (P.halo_bytes != 0, stride-1 3x3): the ring holds filter boxes only, and beside it kHaloSlots input halos
+// take turns, one per (tile, 64-channel block).  A tile's K order is channel-block-major (cb outer, tap inner), so only
+// the current block's halo has to be resident; a tile's halos are ring blocks of their own ring, j*ncb ... j*ncb + ncb - 1.
 constexpr int kPersistThreads = 384;
+constexpr int kHaloSlots = 2;
 struct PersistLayout {
   static constexpr int kStageBytes = SmemLayout<128>::kStageBytes;
+  static constexpr int kFilterBytes = SmemLayout<128>::kBBytes; // halo launches: a ring stage is the filter box alone
   static constexpr int kOutBytes = 2 * kOutHalfBytes;          // per consumer, 1024-byte aligned (TMA 128B swizzle)
   static constexpr int kPitch = 32 + 4;                        // XM: floats per staged row of a 32-column chunk
   static constexpr int kChunkBytes = BM * kPitch * 4;
   static_assert(kChunkBytes <= kOutBytes, "the XM staged chunk lives in the output tile");
-  // [ring: stages x (A|B)] [2 x output tile] [barriers 256 B] [2 x bias 128 fp32] ; + 1024 B alignment slack
-  __host__ __device__ static int bar_off(int stages) { return stages * kStageBytes + 2 * kOutBytes; }
-  static int total(int stages) { return bar_off(stages) + 256 + 2 * 128 * 4 + 1024; }
+  // [ring: stages x (A|B), or stages x B + kHaloSlots x halo] [2 x output tile] [barriers 256 B] [2 x bias 128 fp32]
+  // ; + 1024 B alignment slack
+  __host__ __device__ static int ring_bytes(int stages, int halo_bytes) {
+    return halo_bytes ? stages * kFilterBytes + kHaloSlots * halo_bytes : stages * kStageBytes;
+  }
+  __host__ __device__ static int bar_off(int stages, int halo_bytes) { return ring_bytes(stages, halo_bytes) + 2 * kOutBytes; }
+  static int total(int stages, int halo_bytes) { return bar_off(stages, halo_bytes) + 256 + 2 * 128 * 4 + 1024; }
 };
+
+// Consumer main loop of a halo launch over one tile: per 64-channel block cb, wait for its halo (ring block h0 + cb),
+// then per tap wait for the filter stage (ring block g0 + 9 cb + tap) and issue two groups of four m64n128k16 wgmma RS,
+// one per 64-row accumulator block hm.  Tile row m = (py, px) of tap (ky, kx) reads halo pixel r = (py + ky)(tw + 2) +
+// px + kx, whose 16-byte chunk k sits at chunk k ^ (r % 8) (128B swizzle of the TMA box); lane_px[hm] is r at tap (0, 0)
+// for the row this lane addresses in ldmatrix.  Fragments rotate through three register sets, so the two groups before
+// a group stay in flight while its fragments load: a group's set is free once the group three back has retired.  A filter
+// stage goes back once both groups of its tap have retired, a halo once its ninth tap's have.  Returns the last filter
+// stage and halo slot, which the caller's final wgmma_wait frees.
+template <class FullBar, class HaloFull, class HandBack, class HaloBack>
+__device__ __forceinline__ void halo_mma_loop(float (&acc0)[64], float (&acc1)[64], const ConvParams& P, uint32_t smem_base,
+                                              int kStages, int g0, int h0, const int (&lane_px)[2], int l, FullBar full_bar,
+                                              HaloFull halo_full, HandBack hand_back, HaloBack halo_back, int& s_last, int& h_last) {
+  const int ncb = P.Cin / BK, hw = P.tw + 2;
+  const uint32_t halo_base = smem_base + uint32_t(kStages * PersistLayout::kFilterBytes);
+  int s = g0 % kStages, h = h0 % kHaloSlots;
+  uint32_t ph = uint32_t(g0 / kStages) & 1u, hph = uint32_t(h0 / kHaloSlots) & 1u;
+  int s_prev = s, h_prev = h;
+  uint32_t fa[3][4][4];
+  for (int cb = 0; cb < ncb; ++cb) {
+    mbar_wait_quiet(halo_full(h), hph);
+    const uint32_t sh = halo_base + uint32_t(h * P.halo_bytes);
+#pragma unroll 1
+    for (int ky = 0; ky < 3; ++ky) {
+#pragma unroll
+      for (int kx = 0; kx < 3; ++kx) {
+        const int tap = 3 * ky + kx;
+        mbar_wait_quiet(full_bar(s), ph);
+        const uint32_t sb = smem_base + uint32_t(s * PersistLayout::kFilterBytes);
+#pragma unroll
+        for (int hm = 0; hm < 2; ++hm) {
+          const int f = (2 * kx + hm) % 3;          // group 2 tap + hm of the block, mod 3 (6 groups per filter row)
+          const int r = lane_px[hm] + ky * hw + kx;
+          const uint32_t a = sh + uint32_t(r) * 128u;
+#pragma unroll
+          for (int kc = 0; kc < 4; ++kc) ldmatrix_x4(fa[f][kc], a + (uint32_t((2 * kc + (l >> 4)) ^ (r & 7)) << 4));
+          wgmma_fence();
+#pragma unroll
+          for (int kc = 0; kc < 4; ++kc) {
+            const uint64_t bd = gmma_desc_sw128(sb + 32 * kc);
+            if (hm == 0) wgmma_rs<0>(acc0, fa[f][kc], bd, (cb | tap | kc) != 0);
+            else wgmma_rs<0>(acc1, fa[f][kc], bd, (cb | tap | kc) != 0);
+          }
+          wgmma_commit();
+          wgmma_wait<2>();
+          if (hm == 1 && (cb | tap) != 0) {   // group (previous tap, hm 1) has retired, and with it every MMA of that tap
+            hand_back(s_prev);
+            if (tap == 0) halo_back(h_prev);
+          }
+        }
+        s_prev = s;
+        if (++s == kStages) { s = 0; ph ^= 1; }
+      }
+    }
+    h_prev = h;
+    if (++h == kHaloSlots) { h = 0; hph ^= 1; }
+  }
+  s_last = s_prev;
+  h_last = h_prev;
+}
 
 // tile t of the launch: n-tile fastest, then m-tile, then problem z
 struct PersistTile { int z, n0; TileOrigin o; };
@@ -404,18 +477,24 @@ conv_gemm_persist_kernel(const ConvParams P, const __grid_constant__ ConvMaps ma
   using L = SmemLayout<128>;
   using PL = PersistLayout;
   const int kStages = P.stages;
-  const uint32_t bar_off = uint32_t(PL::bar_off(kStages));
+  const bool halo = !XM && P.halo_bytes != 0;                 // stride-1 3x3: one input halo per 64-channel block
+  const uint32_t ring_bytes = uint32_t(PL::ring_bytes(kStages, P.halo_bytes));
+  const uint32_t bar_off = uint32_t(PL::bar_off(kStages, P.halo_bytes));
   const uint32_t bar_base = smem_base + bar_off;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (kMaxStages + s); };
   auto order_bar = [&](int c) { return bar_base + 8u * (2 * kMaxStages + c); };   // consumer c may start its main loop
   auto res_bar = [&](int c) { return bar_base + 8u * (2 * kMaxStages + 2 + c); }; // consumer c's residual tile has landed
+  auto halo_full = [&](int h) { return bar_base + 8u * (2 * kMaxStages + 4 + h); };
+  auto halo_empty = [&](int h) { return bar_base + 8u * (2 * kMaxStages + 4 + kHaloSlots + h); };
+  static_assert(8 * (2 * kMaxStages + 4 + 2 * kHaloSlots) <= 256, "barriers");
   uint8_t* smem_gen = smem_raw + (smem_base - smem_u32(smem_raw));
 
   pdl_launch_dependents();
   const int tid = threadIdx.x;
   const int wg = tid >> 7;
-  const int nkb = P.k_pad / BK;
+  const int ncb = P.Cin / BK;                                 // halo: 64-channel blocks, 9 filter blocks each
+  const int nkb = halo ? 9 * ncb : P.k_pad / BK;
   const int a_mode = P.a_mode;
   const bool has_res = (P.epi & (ICAF_EPI_ADD_RES | ICAF_EPI_SCALED_RES)) != 0;
   if (tid == 0) {
@@ -427,6 +506,10 @@ conv_gemm_persist_kernel(const ConvParams P, const __grid_constant__ ConvMaps ma
     mbar_init(order_bar(1), 4);
     mbar_init(res_bar(0), 1);
     mbar_init(res_bar(1), 1);
+    for (int h = 0; h < kHaloSlots; ++h) {
+      mbar_init(halo_full(h), 1);
+      mbar_init(halo_empty(h), 4);
+    }
     fence_mbar_init();
   }
   if (tid == 32) {
@@ -447,12 +530,31 @@ conv_gemm_persist_kernel(const ConvParams P, const __grid_constant__ ConvMaps ma
     if (tid < 32 && elect_one()) {
       const uint32_t a_bytes = a_mode == A_TMA2D ? L::kABytes : uint32_t(P.tw * P.th) * 128u;
       const uint32_t bytes = L::kBBytes + a_bytes;
-      int s = 0;
-      uint32_t ph = 0;
+      int s = 0, h = 0;
+      uint32_t ph = 0, hph = 0;
       for (int tile = blockIdx.x; tile < P.tiles; tile += gridDim.x) {
         const PersistTile pt = persist_tile(P, tile);
         const CUtensorMap* mw = pt.z ? &maps.w[1] : &maps.w[0];
         const CUtensorMap* ma = pt.z ? &maps.a[1] : &maps.a[0];
+        if (halo) {
+          // per 64-channel block: the (64, tw+2, th+2) halo around the tile (zero-filled outside the map), then the
+          // block's nine filter boxes at K column tap * Cin + cb * 64 (pack_conv_weight's tap-major K)
+          const uint32_t halo_tx = uint32_t((P.tw + 2) * (P.th + 2)) * 128u;
+          for (int cb = 0; cb < ncb; ++cb) {
+            mbar_wait_quiet(halo_empty(h), hph ^ 1);
+            mbar_arrive_expect_tx(halo_full(h), halo_tx);
+            tma_load_4d(smem_base + uint32_t(kStages * PL::kFilterBytes + h * P.halo_bytes), ma, halo_full(h), cb * BK,
+                        pt.o.ox0 - 1, pt.o.oy0 - 1, pt.o.tb);
+            if (++h == kHaloSlots) { h = 0; hph ^= 1; }
+            for (int tap = 0; tap < 9; ++tap) {
+              mbar_wait_quiet(empty_bar(s), ph ^ 1);
+              mbar_arrive_expect_tx(full_bar(s), PL::kFilterBytes);
+              tma_load_2d(smem_base + uint32_t(s * PL::kFilterBytes), mw, full_bar(s), tap * P.Cin + cb * BK, pt.n0);
+              if (++s == kStages) { s = 0; ph ^= 1; }
+            }
+          }
+          continue;
+        }
         for (int kb = 0; kb < nkb; ++kb) {
           mbar_wait_quiet(empty_bar(s), ph ^ 1);
           load_stage<128, true>(P, a_mode, smem_base + s * L::kStageBytes, full_bar(s), bytes, mw, ma, kb, pt.n0, pt.o);
@@ -468,9 +570,20 @@ conv_gemm_persist_kernel(const ConvParams P, const __grid_constant__ ConvMaps ma
   const int c = wg - 1;
   const int t = tid & 127, w = t >> 5, l = t & 31;
   const int bar_id = 2 + c;                                   // warpgroup-local named barrier
-  const uint32_t sout = smem_base + uint32_t(kStages * L::kStageBytes + c * PL::kOutBytes);   // this consumer's output tile
-  float* sacc = reinterpret_cast<float*>(smem_gen + kStages * L::kStageBytes + c * PL::kOutBytes);   // XM: staged chunk
+  const uint32_t sout = smem_base + ring_bytes + uint32_t(c * PL::kOutBytes);                  // this consumer's output tile
+  float* sacc = reinterpret_cast<float*>(smem_gen + ring_bytes + c * PL::kOutBytes);           // XM: staged chunk
   float* sbias = reinterpret_cast<float*>(smem_gen + bar_off + 256 + c * 128 * 4);
+  // halo: the halo pixel at tap (0, 0) of the tile row this lane addresses in ldmatrix (matrix l / 8 of an x4 covers rows
+  // 8 ((l / 8) % 2) ... of the 16-row group, chunk (l / 16) of the 16-channel K step) for the accumulator blocks 0-63 and
+  // 64-127.  Rows past the tw x th patch (20 x 6 tiles) read the patch's last pixel: they are never stored.
+  int lane_px[2];
+#pragma unroll
+  for (int hm = 0; hm < 2; ++hm) {
+    int m = 64 * hm + 16 * w + (l & 7) + 8 * ((l >> 3) & 1);
+    if (m > P.tw * P.th - 1) m = P.tw * P.th - 1;
+    const int py = P.tw ? m / P.tw : 0;
+    lane_px[hm] = py * (P.tw + 2) + m - py * P.tw;
+  }
   for (int tile = blockIdx.x + c * gridDim.x; tile < P.tiles; tile += 2 * gridDim.x) {
     const int j = (tile - int(blockIdx.x)) / int(gridDim.x);  // ordinal of the tile among this CTA's tiles
     const PersistTile pt = persist_tile(P, tile);
@@ -503,14 +616,21 @@ conv_gemm_persist_kernel(const ConvParams P, const __grid_constant__ ConvMaps ma
 #pragma unroll
     for (int i = 0; i < 64; ++i) { acc0[i] = 0.f; acc1[i] = 0.f; }
     auto hand_back = [&](int s) { if (l == 0) mbar_arrive(empty_bar(s)); };   // one arrival per consumer warp
+    auto halo_back = [&](int h) { if (l == 0) mbar_arrive(halo_empty(h)); };
     const int g0 = j * nkb;
-    const int s0 = g0 % kStages;
-    const uint32_t ph0 = uint32_t(g0 / kStages) & 1u;
     if (j > 0) mbar_wait_quiet(order_bar(c), uint32_t((j >> 1) - (1 - c)) & 1u);
-    const int s_last = mma_loop<128>(acc0, acc1, smem_base, kStages, nkb, s0, ph0, full_bar, hand_back);
+    int s_last, h_last = 0;
+    if (halo) {
+      halo_mma_loop(acc0, acc1, P, smem_base, kStages, g0, j * ncb, lane_px, l, full_bar, halo_full, hand_back, halo_back,
+                    s_last, h_last);
+    } else {
+      s_last = mma_loop<128>(acc0, acc1, smem_base, kStages, nkb, g0 % kStages, uint32_t(g0 / kStages) & 1u, full_bar,
+                             hand_back);
+    }
     if (l == 0) mbar_arrive(order_bar(c ^ 1));          // every MMA of this tile is issued: the other consumer's turn
     wgmma_wait<0>();
     hand_back(s_last);
+    if (halo) halo_back(h_last);
 
     if constexpr (!XM) {
       // ---- epilogue on the accumulator registers, 16 columns at a time, then the TMA store of the tile
@@ -610,6 +730,7 @@ static int fill_geom(const icaf_conv_geom* g, int n_io, ConvParams& P) {
   P.ln_parts = 0; P.ln_eps = 0.f; P.ln_inv_k = 0.f;
   P.m_tiles = P.n_tiles = P.tiles = 0;
   P.tma_epi = 0;
+  P.halo_bytes = 0;
   memset(P.p, 0, sizeof(P.p));
   return ICAF_OK;
 }
@@ -712,18 +833,22 @@ static int plan_tc(ConvParams& P, int n_io, ConvPlan& pl) {
 
 // A 128 x 128 plan with TMA-staged A, no split-K and more tiles than SMs runs on conv_gemm_persist_kernel: one CTA per SM
 // walks the tiles, so the ring fill and the epilogue of one tile overlap the main loop of the next.  The ring takes what
-// the staged chunks leave of the 227 KB (it is not clamped to the K loop: it runs on across tiles).
+// the output tiles (and, for stride-1 3x3 patch tiles, the input halos) leave of the 227 KB (it is not clamped to the K
+// loop: it runs on across tiles).  A halo slot holds (tw+2)(th+2) pixels of 128 B, rounded up to the 1 KB the 128B
+// swizzle needs (23 KB for 16 x 8 and 8 x 16 tiles, 22 KB for 20 x 6), which leaves 7 filter stages.
 static int plan_persist(ConvParams& P, ConvPlan& pl) {
   constexpr int kSmemCap = 227 * 1024;
+  const bool halo = !pl.xm && P.a_mode == A_TMA4D && P.kh == 3 && P.kw == 3 && P.stride == 1 && P.pad == 1;
+  P.halo_bytes = halo ? ((P.tw + 2) * (P.th + 2) * 128 + 1023) / 1024 * 1024 : 0;
   int stages = kMaxStages;
-  while (stages > 2 && PersistLayout::total(stages) > kSmemCap) --stages;
-  if (PersistLayout::total(stages) > kSmemCap)
+  while (stages > 2 && PersistLayout::total(stages, P.halo_bytes) > kSmemCap) --stages;
+  if (PersistLayout::total(stages, P.halo_bytes) > kSmemCap)
     return set_error(ICAF_ERR_BAD_ARG, "conv2d(persist): shared-memory plan exceeds 227 KB");
   P.stages = stages;
   P.m_tiles = pl.m_tiles; P.n_tiles = pl.n_tiles; P.tiles = pl.tiles;
   pl.persist = true;
   pl.ctas = pl.tiles < pl.sms ? pl.tiles : pl.sms;
-  pl.smem = PersistLayout::total(stages);
+  pl.smem = PersistLayout::total(stages, P.halo_bytes);
   return ICAF_OK;
 }
 
@@ -740,6 +865,8 @@ static int encode_maps(const ConvParams& P, const __half* const (&w)[2], const i
     const ConvProblem& pr = P.p[i];
     if (P.a_mode == A_TMA2D)
       rc = encode_tmap_2d(&maps.a[i], pr.x, (uint64_t)P.Cin, (uint64_t)P.M, (uint64_t)pr.x_ld * 2, BK, BM);
+    else if (P.a_mode == A_TMA4D && P.halo_bytes)       // persistent stride-1 3x3: the tile's input halo
+      rc = encode_tmap_nhwc(&maps.a[i], pr.x, P.Cin, P.Wi, P.Hi, P.B, pr.x_ld, BK, P.tw + 2, P.th + 2, 1, 1);
     else if (P.a_mode == A_TMA4D)
       rc = encode_tmap_nhwc(&maps.a[i], pr.x, P.Cin, P.Wi, P.Hi, P.B, pr.x_ld, BK, P.tw * P.stride, P.th * P.stride, P.stride,
                             P.stride);
