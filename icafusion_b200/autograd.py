@@ -22,7 +22,9 @@ import torch.nn as nn
 from torch.autograd import Function
 
 from . import ops
+from .common import C3, SPPF, Concat, Conv, TransformerFusionBlock
 from .ops import ACT_NONE, ACT_SILU
+from .yolo_test import Detect
 
 _STATE = {"seed": 0x1234567, "count": 0, "defer_bn": False, "bn": []}
 
@@ -475,16 +477,14 @@ def model_forward(model, rgb_img: torch.Tensor, ir_img: torch.Tensor, taps: list
 def _walk(model, rgb_img, ir_img, taps):
     """The IR backbone (layers s .. 2s-1, fed by `f == -4`) is independent of the RGB one until the first DMFF block: it is
     issued on a side stream, so the two streams' kernels overlap -- and so do their backward nodes, which autograd runs on the
-    stream each forward ran on.  Inside a CUDA-graph capture the fork / join become parallel branches of the graph."""
+    stream each forward ran on.  Inside a CUDA-graph capture the fork / join become parallel branches of the graph.  Sources,
+    the stream split and the side-stream DMFF blocks come from the model's layer plan (yolo_test.plan_layers)."""
     import contextlib
     import os
-    from .common import C3, SPPF, Concat, Conv, TransformerFusionBlock
-    from .yolo_test import Detect
+    plan = model._layer_plan()
     y: list = []
     x = None
-    if "_ir_start" not in model.__dict__:
-        model._plan_streams()
-    s_ir = model._ir_start if os.environ.get("ICAF_TRAIN_STREAMS", "1") != "0" else None
+    s_ir = plan.ir_start if os.environ.get("ICAF_TRAIN_STREAMS", "1") != "0" else None
     main = side = None
     if s_ir is not None and rgb_img.is_cuda:
         main = torch.cuda.current_stream(rgb_img.device)
@@ -493,6 +493,7 @@ def _walk(model, rgb_img, ir_img, taps):
     joined = side is None
     forked = {}                                      # layer index -> side stream a DMFF block is running on
     for m in model.model:
+        srcs = plan.srcs[m.i]
         on_side = side is not None and s_ir <= m.i < 2 * s_ir
         if not joined and m.i >= 2 * s_ir:           # first consumer of both branches
             main.wait_stream(side)
@@ -501,14 +502,13 @@ def _walk(model, rgb_img, ir_img, taps):
                     t.record_stream(main)            # produced in the side stream's pool, read (and saved for backward) on main
             joined = True
         st = side if on_side else None
-        if side is not None and joined and isinstance(m, TransformerFusionBlock):
+        if side is not None and m.i in plan.side_dmff:
             # the DMFF blocks only read backbone maps and are independent of each other: one side stream each (they are chains
             # of small token-level kernels that leave most of the GPU idle when run one after the other)
             st = model._side_streams(rgb_img.device, 2 + len(forked))[1 + len(forked)]
             st.wait_stream(main)
-            srcs = m.f if isinstance(m.f, (list, tuple)) else [m.f]
             for j in srcs:
-                if j != -1 and y[j] is not None:
+                if y[j] is not None:
                     y[j].record_stream(st)
             forked[m.i] = st
         elif forked:                                 # any other layer: join the DMFF streams it may read from
@@ -520,39 +520,34 @@ def _walk(model, rgb_img, ir_img, taps):
                 x.record_stream(main)                # the previous layer's output arrives as `-1` even when it is not in `save`
             forked = {}
         with (torch.cuda.stream(st) if st is not None else contextlib.nullcontext()):
-            x = _layer(model, m, x, y, rgb_img, ir_img, Conv, C3, SPPF, Concat, TransformerFusionBlock, Detect)
+            x = _layer(model, m, [x if j == m.i - 1 else y[j] for j in srcs], rgb_img, ir_img)
         y.append(x if m.i in model.save else None)
         if taps is not None:
             taps.append(x)
     return x
 
 
-def _layer(model, m, x, y, rgb_img, ir_img, Conv, C3, SPPF, Concat, TransformerFusionBlock, Detect):
-    stem = False
-    if m.f == -4 or x is None:                                # image stems: RGB is the first layer, IR enters at f == -4
-        img = ir_img if m.f == -4 else rgb_img
-        x = model._stage(img, m)
-        stem = isinstance(m, Conv) and m.is_s2d_stem()
-        if not stem:
+def _layer(model, m, xs, rgb_img, ir_img):
+    """Layer `m` on the maps `xs` of its sources (none: an image stem, RGB is the first layer, IR enters at f == -4)."""
+    stem = not xs
+    if stem:
+        xs = [model._stage(ir_img if m.f == -4 else rgb_img, m)]
+        if not (isinstance(m, Conv) and m.is_s2d_stem()):
             raise NotImplementedError("training: the image stem must be the 6x6 / stride 2 Conv of the yolov5 YAMLs")
-    elif m.f != -1:
-        x = y[m.f] if isinstance(m.f, int) else [x if j == -1 else y[j] for j in m.f]
     if isinstance(m, Conv):
-        x = conv_bn_act(m, x, stem)
-    elif isinstance(m, C3):
-        x = c3(m, x)
-    elif isinstance(m, SPPF):
-        x = sppf(m, x)
-    elif isinstance(m, nn.Upsample):
+        return conv_bn_act(m, xs[0], stem)
+    if isinstance(m, C3):
+        return c3(m, xs[0])
+    if isinstance(m, SPPF):
+        return sppf(m, xs[0])
+    if isinstance(m, nn.Upsample):
         if m.mode != "nearest" or m.scale_factor is None or float(m.scale_factor) != 2.0:
             raise NotImplementedError("Upsample: only nearest x2 is supported")
-        x = Upsample2xFn.apply(x)
-    elif isinstance(m, Concat):
-        x = ConcatFn.apply(*x)
-    elif isinstance(m, TransformerFusionBlock):
-        x = fusion_block(m, x[0], x[1])
-    elif isinstance(m, Detect):
-        x = detect(m, x)
-    else:
-        raise NotImplementedError(type(m).__name__)
-    return x
+        return Upsample2xFn.apply(xs[0])
+    if isinstance(m, Concat):
+        return ConcatFn.apply(*xs)
+    if isinstance(m, TransformerFusionBlock):
+        return fusion_block(m, xs[0], xs[1])
+    if isinstance(m, Detect):
+        return detect(m, xs)
+    raise NotImplementedError(type(m).__name__)

@@ -12,7 +12,7 @@ from __future__ import annotations
 import logging
 import math
 from copy import deepcopy
-from typing import List
+from typing import List, NamedTuple, Optional, Tuple
 
 import torch
 import torch.nn as nn
@@ -172,6 +172,75 @@ def parse_model(d: dict, ch: List[int]):
     return nn.Sequential(*layers), sorted(save)
 
 
+class LayerPlan(NamedTuple):
+    """What the inference and training layer walks need to know about the layer list, derived from it once.
+
+    ir_start:  index of the IR stream's first layer (the one layer with from == -4) when the IR stream mirrors the RGB
+               stream layer by layer, so that layers k and ir_start + k run as one grouped launch; else None.
+    srcs:      per layer, the indices of the layers it reads (-1 and other relative indices resolved); () for a layer
+               fed an image (the RGB stem, or from == -4: the IR stem).
+    ch:        per layer, its output channels (None for Detect).
+    stride:    per layer, the input image's size over its output's (Conv strides, Upsample x2).
+    dst:       per layer, (Concat layer, channel offset) when the layer writes its output straight into that slice of
+               the Concat's buffer (see plan_layers), else None.
+    side_dmff: the DMFF blocks whose inputs all lie in the two backbones: they may run on a side stream."""
+    ir_start: Optional[int]
+    srcs: Tuple[Tuple[int, ...], ...]
+    ch: Tuple[Optional[int], ...]
+    stride: Tuple[Optional[int], ...]
+    dst: Tuple[Optional[Tuple[int, int]], ...]
+    side_dmff: Tuple[int, ...]
+
+
+def plan_layers(layers) -> LayerPlan:
+    """The LayerPlan of a parsed layer list.  Concat elimination (`dst`): every tensor that feeds a Concat layer is produced
+    directly inside that layer's output buffer (all kernels take channel-slice views), so the Concat itself launches
+    nothing.  A producer feeding two concats keeps the first and is copied for the rest; the two streams' layers, which run
+    as grouped launches, are never producers."""
+    layers = list(layers)
+    starts = [m.i for m in layers if m.f == -4]
+    ir = starts[0] if len(starts) == 1 and 2 * starts[0] <= len(layers) else None
+
+    def sig(m):
+        return (type(m), [tuple(p.shape) for p in m.parameters()])
+    for k in range(ir or 0):                      # the IR stream must mirror the RGB stream layer by layer
+        a, b = layers[k], layers[ir + k]
+        if sig(a) != sig(b) or (k > 0 and (a.f != -1 or b.f != -1)):
+            ir = None
+            break
+    paired = 2 * ir if ir is not None else 0
+    n = len(layers)
+    srcs, ch, stride, dst = [()] * n, [None] * n, [None] * n, [None] * n
+    for m in layers:
+        i = m.i
+        if i > 0 and m.f != -4:
+            srcs[i] = tuple(j % i for j in ([m.f] if isinstance(m.f, int) else m.f))
+        s_in = stride[srcs[i][0]] if srcs[i] else 1
+        stride[i] = (s_in * m.conv.stride[0] if isinstance(m, Conv) else s_in // 2 if isinstance(m, nn.Upsample) else
+                     None if isinstance(m, Detect) else s_in)
+        if isinstance(m, Conv):
+            ch[i] = m.conv.out_channels
+        elif isinstance(m, C3):
+            ch[i] = m.cv3.conv.out_channels
+        elif isinstance(m, SPPF):
+            ch[i] = m.cv2.conv.out_channels
+        elif isinstance(m, TransformerFusionBlock):
+            ch[i] = m.n_embd
+        elif isinstance(m, nn.Upsample):
+            ch[i] = ch[srcs[i][0]]
+        elif isinstance(m, Concat):
+            if m.d == 1 and not isinstance(m.f, int) and \
+                    all(ch[j] and j >= paired and dst[j] is None and not isinstance(layers[j], (Concat, Detect)) for j in srcs[i]):
+                off = 0
+                for j in srcs[i]:
+                    dst[j] = (i, off)
+                    off += ch[j]
+            ch[i] = sum(ch[j] for j in srcs[i])
+    side_dmff = tuple(m.i for m in layers[paired:] if isinstance(m, TransformerFusionBlock) and not isinstance(m.f, int)
+                      and all(j < paired for j in srcs[m.i]))
+    return LayerPlan(ir, tuple(srcs), tuple(ch), tuple(stride), tuple(dst), side_dmff)
+
+
 class Model(nn.Module):
     """reference: models/yolo_test.py:73-213"""
 
@@ -196,63 +265,17 @@ class Model(nn.Module):
             if type(mod) is nn.BatchNorm2d:
                 mod.eps = 1e-3
                 mod.momentum = 0.03
-        self._plan_streams()
-        self._plan_concats()
+        self._plan = plan_layers(self.model)
 
-    # -- two-stream pairing ----------------------------------------------------------------------
-    def _plan_streams(self):
-        """Find the IR stream (first layer with from == -4) and check it mirrors the RGB stream layer by layer."""
-        layers = list(self.model)
-        starts = [m.i for m in layers if m.f == -4]
-        self._ir_start = None
-        if len(starts) != 1:
-            return
-        s = starts[0]
-        if 2 * s > len(layers):
-            return
-        def sig(m):
-            return (type(m), [tuple(p.shape) for p in m.parameters()])
-        for k in range(s):
-            a, b = layers[k], layers[s + k]
-            if sig(a) != sig(b) or (k > 0 and (a.f != -1 or b.f != -1)):
-                return
-        self._ir_start = s
+    def _layer_plan(self) -> LayerPlan:
+        if "_plan" not in self.__dict__:          # an unpickled checkpoint (models/experimental.py:118) never ran __init__
+            self._plan = plan_layers(self.model)
+        return self._plan
 
-    def _plan_concats(self):
-        """Concat elimination: every tensor that feeds a Concat layer is produced directly inside that layer's output
-        buffer (all kernels take channel-slice views), so Concat itself launches nothing.  Maps producer layer index ->
-        (concat layer index, channel offset); a producer feeding two concats keeps the first and is copied for the rest."""
-        self._concat_dst, self._concat_width = {}, {}
-        ch = self._layer_ch = {}
-        paired = 2 * self._ir_start if self._ir_start is not None else 0     # stream layers run in the grouped loop
-        for m in self.model:
-            if isinstance(m, Concat) and m.d == 1 and isinstance(m.f, (list, tuple)):
-                srcs = [m.i - 1 if j == -1 else j for j in m.f]
-                ok = all(j in ch and ch[j] and j >= paired and j not in self._concat_dst and
-                         not isinstance(self.model[j], (Concat, Detect)) for j in srcs)
-                if ok:
-                    off = 0
-                    for j in srcs:
-                        self._concat_dst[j] = (m.i, off)
-                        off += ch[j]
-                    self._concat_width[m.i] = off
-            ch[m.i] = self._out_channels(m, ch)
-
-    @staticmethod
-    def _out_channels(m, ch):
-        if isinstance(m, Conv):
-            return m.conv.out_channels
-        if isinstance(m, (C3,)):
-            return m.cv3.conv.out_channels
-        if isinstance(m, SPPF):
-            return m.cv2.conv.out_channels
-        if isinstance(m, TransformerFusionBlock):
-            return m.n_embd
-        if isinstance(m, nn.Upsample):
-            return ch[m.i - 1] if m.f == -1 else ch[m.f]
-        if isinstance(m, Concat):
-            return sum(ch[m.i - 1 if j == -1 else j] for j in m.f)
-        return None
+    @property
+    def _ir_start(self):
+        """Index of the IR stream's first layer, or None when the two streams do not pair up (see plan_layers)."""
+        return self._layer_plan().ir_start
 
     def forward(self, x, x2, augment=False, profile=False):
         if augment:
@@ -273,24 +296,26 @@ class Model(nn.Module):
         z, logits, xs = self._forward_nhwc(x, x2)
         return z, logits, xs
 
-    def _run_layer(self, m, v, out=None):
-        o = None if out is None else [out]
+    @staticmethod
+    def _run_layer(ms, xs, out=None):
+        """Run one layer, ms = [m], on the NHWC maps xs of its sources; or the twin layers ms = [rgb, ir] of the two
+        streams, one map each, as grouped launches.  `out`: the view a single layer writes into.  Returns one map per
+        module.  (Detect runs level by level in the walk.)"""
+        m, outs = ms[0], None if out is None else [out]
         if isinstance(m, Conv):
-            return Conv.run([m], [v], o)[0]
+            return Conv.run(ms, xs, outs)
         if isinstance(m, C3):
-            return C3.run([m], [v], o)[0]
+            return C3.run(ms, xs, outs)
         if isinstance(m, SPPF):
-            return SPPF.run([m], [v], o)[0]
+            return SPPF.run(ms, xs, outs)
         if isinstance(m, nn.Upsample):             # ours, or torch's own class inside an unpickled reference checkpoint
             if m.mode != "nearest" or m.scale_factor is None or float(m.scale_factor) != 2.0:
                 raise NotImplementedError("Upsample: only nearest x2 is supported")
-            return ops.upsample2x(v, out)
+            return [ops.upsample2x(xs[0], out)]
         if isinstance(m, Concat):
-            return Concat.run(v)
+            return [Concat.run(xs)]
         if isinstance(m, TransformerFusionBlock):
-            return m.run(v[0], v[1], out)
-        if isinstance(m, Detect):
-            return m.run(list(v))
+            return [m.run(xs[0], xs[1], out)]
         raise NotImplementedError(type(m).__name__)
 
     def _stage(self, img, stem):
@@ -314,141 +339,100 @@ class Model(nn.Module):
 
     def _forward_nhwc(self, rgb, ir):
         """Layer walk with branch-level concurrency: the RGB/IR streams run as grouped launches on the current stream;
-        a DMFF block is forked onto a side stream as soon as both of its inputs exist (P3 and P4 fusion overlap the rest of
-        the backbone), Detect levels are forked as soon as their head output exists; consumers join before they read."""
-        if "_ir_start" not in self.__dict__:       # an unpickled checkpoint (models/experimental.py:118) never ran __init__
-            self._plan_streams()
-            self._plan_concats()
+        a side-stream DMFF block is forked as soon as both of its inputs exist (P3 and P4 fusion overlap the rest of the
+        backbone; the last block feeds the head directly and stays in order), every Detect level but the last is forked as
+        soon as its input exists; consumers join before they read, and the end of the walk joins whatever is left."""
+        plan = self._layer_plan()
         if not (ops.on_device(rgb) and ops.on_device(ir)):     # before any stream lookup: torch rejects a CPU device there
             raise RuntimeError("icafusion_b200 runs on CUDA tensors only (no CPU fallback)")
         layers = list(self.model)
         y: List = [None] * len(layers)
         dev = rgb.device
+        B, H, W = rgb.shape[0], rgb.shape[2], rgb.shape[3]
         dry = ops.dry_running()                   # shape-only walk on meta tensors (no streams, nothing launched)
         main = None if dry else torch.cuda.current_stream(dev)
-        forked = {}                               # layer index -> side stream its result is being produced on
-        n_side = [0]
+        forked = {}                               # layer index (or Detect level) -> side stream its result is produced on
+        n_side = 0
         concurrent = self.__dict__.get("_icaf_concurrent", True) and not dry
 
-        def fork():
-            st = self._side_streams(dev, n_side[0] + 1)[n_side[0]]
-            n_side[0] += 1
+        def fork(key):
+            nonlocal n_side
+            st = self._side_streams(dev, n_side + 1)[n_side]
+            n_side += 1
             st.wait_stream(main)
-            return st
+            forked[key] = st
+            return torch.cuda.stream(st)
 
-        def join(idxs):
-            for j in idxs:
-                st = forked.pop(j, None)
+        def join(keys):
+            for k in keys:
+                st = forked.pop(k, None)
                 if st is not None:
                     main.wait_stream(st)
 
-        cats = {}                                 # concat layer index -> its (lazily allocated) output buffer
+        cats = {}                                 # concat layer index -> its output buffer, allocated by its first producer
 
-        def dest(m, shape_hw):
-            """Slice of the consumer Concat's buffer this layer should write into (or None)."""
-            d = self._concat_dst.get(m.i)
-            if d is None:
+        def dest(i):
+            """The slice of its Concat's buffer layer i writes into (or None); allocated on the main stream."""
+            if plan.dst[i] is None:
                 return None
-            ci, off = d
-            if ci not in cats:
-                B, H, W = shape_hw
-                cats[ci] = torch.empty(B, H, W, self._concat_width[ci], dtype=torch.float16, device=dev)
-            return cats[ci][..., off:off + self._layer_ch[m.i]]
+            c, off = plan.dst[i]
+            if c not in cats:
+                s = plan.stride[i]
+                cats[c] = torch.empty(B, H // s, W // s, plan.ch[c], dtype=torch.float16, device=dev)
+            return cats[c][..., off:off + plan.ch[i]]
 
         arena = self.__dict__.get("_icaf_arena")
         if concurrent and arena is not None and arena.numel() * 2 <= (96 << 20):
             # the whole packed filter set fits the 126 MB L2: stream it in once, concurrently with the first layers
-            st = fork()
-            with torch.cuda.stream(st):
+            with fork("prefetch"):
                 ops.prefetch_l2(arena)
-            forked[("prefetch",)] = st
         ir_first = next((m for m in layers if m.f == -4), layers[0])
-        v_rgb, v_ir = self._stage(rgb, layers[0]), self._stage(ir, ir_first)
-        start = 0
-        if self._ir_start is not None:
-            s = self._ir_start
-            fusion = [m for m in layers[2 * s:] if isinstance(m, TransformerFusionBlock) and isinstance(m.f, (list, tuple))
-                      and all(0 <= j < 2 * s for j in m.f)]
-            a, b = v_rgb, v_ir
-            for k in range(s):                       # both streams, one grouped launch per operator
-                ma, mb = layers[k], layers[s + k]
-                run = Conv.run if isinstance(ma, Conv) else C3.run if isinstance(ma, C3) else SPPF.run
-                a, b = run([ma, mb], [a, b])
-                y[k], y[s + k] = a, b
-                if concurrent:
-                    for m in fusion[:-1]:            # the last fusion block feeds the head directly: it stays in order
-                        if y[m.i] is None and all(y[j] is not None for j in m.f):
-                            xa, xb = y[m.f[0]], y[m.f[1]]
-                            out = dest(m, (xa.shape[0], xa.shape[1], xa.shape[2]))     # allocated on the main stream
-                            st = fork()
-                            with torch.cuda.stream(st):
-                                y[m.i] = m.run(xa, xb, out)
-                            forked[m.i] = st
-            start = 2 * s
-            x = b
-        else:
-            x = v_rgb
+        images = self._stage(rgb, layers[0]), self._stage(ir, ir_first)
+        side_dmff = plan.side_dmff[:-1] if concurrent else ()
+        s = plan.ir_start or 0
+        for k in range(s):                        # both streams, one grouped launch per operator
+            y[k], y[s + k] = self._run_layer([layers[k], layers[s + k]], [y[k - 1], y[s + k - 1]] if k else images)
+            for i in side_dmff:
+                if y[i] is None and all(y[j] is not None for j in plan.srcs[i]):
+                    out = dest(i)
+                    with fork(i):
+                        y[i] = self._run_layer([layers[i]], [y[j] for j in plan.srcs[i]], out)[0]
 
-        det = layers[-1] if isinstance(layers[-1], Detect) and isinstance(layers[-1].f, (list, tuple)) else None
-        det_state = None
-        for m in layers[start:]:
-            if y[m.i] is not None and m.i in forked or (y[m.i] is not None and isinstance(m, TransformerFusionBlock)):
-                x = y[m.i]                         # already produced (possibly still in flight on a side stream)
+        det = layers[-1] if isinstance(layers[-1], Detect) else None
+        det_srcs = plan.srcs[-1] if det is not None else ()
+        det_early = det_srcs[:-1] if concurrent else ()     # forked as their input appears; the last level closes the forward
+        det_out = None                            # (z, logits, row offsets, level maps)
+
+        def det_outputs():
+            nonlocal det_out
+            if det_out is None:
+                z, logits, offs = det.alloc_outputs(B, [(H // plan.stride[j], W // plan.stride[j]) for j in det_srcs], dev)
+                det_out = (z, logits, offs, [None] * len(det_srcs))
+            return det_out
+
+        for m in layers[2 * s:]:
+            i = m.i
+            if y[i] is not None:                  # a DMFF block forked during the streams
                 continue
-            srcs = [m.i - 1] if m.f == -1 else ([] if m.f == -4 else ([m.f] if isinstance(m.f, int) else
-                                                                         [m.i - 1 if j == -1 else j for j in m.f]))
-            if m.f == -4:
-                x = v_ir
-            elif m.f != -1:
-                x = y[m.f] if isinstance(m.f, int) else [x if j == -1 else y[j] for j in m.f]
-            if m is det and concurrent and det_state is not None:
-                # levels whose inputs were ready were forked earlier; run the rest here and join everything
-                z, logits, offs, xs = det_state
-                for i, j in enumerate(m.f):
-                    if xs[i] is None:
-                        join([j])
-                        xs[i] = m.run_level(i, y[j], z, logits, offs[i])
-                for st in list(forked.values()):
-                    main.wait_stream(st)
-                forked.clear()
-                x = (z, logits, xs)
-                y[m.i] = x
-                continue
-            join(srcs)
-            if isinstance(m, Concat) and m.i in cats:
-                join([j for j, (ci, _) in self._concat_dst.items() if ci == m.i])
-                x = cats[m.i]                      # every source already wrote its slice
+            join(plan.srcs[i])
+            if m is det:
+                z, logits, offs, maps = det_outputs()
+                for lvl, j in enumerate(det_srcs):
+                    if maps[lvl] is None:
+                        maps[lvl] = m.run_level(lvl, y[j], z, logits, offs[lvl])
+                y[i] = (z, logits, maps)
+            elif isinstance(m, Concat) and i in cats:
+                y[i] = cats[i]                    # every source already wrote its slice
             else:
-                out = None
-                if m.i in self._concat_dst and not isinstance(m, (Concat, Detect)):
-                    ref = x[0] if isinstance(x, (list, tuple)) else x
-                    B, H, W = ref.shape[0], ref.shape[1], ref.shape[2]
-                    if isinstance(m, nn.Upsample):
-                        H, W = 2 * H, 2 * W
-                    elif isinstance(m, Conv):
-                        k, s_, p = m.conv.kernel_size[0], m.conv.stride[0], m.conv.padding[0]
-                        H, W = (H + 2 * p - k) // s_ + 1, (W + 2 * p - k) // s_ + 1
-                    out = dest(m, (B, H, W))
-                x = self._run_layer(m, x, out)
-            y[m.i] = x
-            # fork Detect levels as soon as their input exists (all but the last one, which closes the forward)
-            if det is not None and concurrent and m.i in det.f and m.i != det.f[-1] and not isinstance(x, (list, tuple)):
-                if det_state is None:
-                    B = x.shape[0]
-                    Himg, Wimg = rgb.shape[2], rgb.shape[3]
-                    hw = [(int(Himg // float(st_)), int(Wimg // float(st_))) for st_ in det.stride]
-                    z, logits, offs = det.alloc_outputs(B, hw, dev)
-                    det_state = (z, logits, offs, [None] * det.nl)
-                i = det.f.index(m.i)
-                z, logits, offs, xs = det_state
-                if (x.shape[1], x.shape[2]) == (int(rgb.shape[2] // float(det.stride[i])), int(rgb.shape[3] // float(det.stride[i]))):
-                    st = fork()
-                    with torch.cuda.stream(st):
-                        xs[i] = det.run_level(i, x, z, logits, offs[i])
-                    forked[("det", i)] = st
-        for st in forked.values():                 # nothing may outlive the forward on a side stream
-            main.wait_stream(st)
-        return x
+                xs = [y[j] for j in plan.srcs[i]] if plan.srcs[i] else [images[1] if m.f == -4 else images[0]]
+                y[i] = self._run_layer([m], xs, dest(i))[0]
+            if i in det_early:
+                z, logits, offs, maps = det_outputs()
+                lvl = det_srcs.index(i)
+                with fork(("det", lvl)):
+                    maps[lvl] = det.run_level(lvl, y[i], z, logits, offs[lvl])
+        join(list(forked))                        # nothing may outlive the forward on a side stream
+        return y[-1]
 
     def consolidate_weights(self, rgb, ir):
         """Run one forward on (rgb, ir), collect every packed filter it touches and move them into one contiguous arena
