@@ -642,6 +642,47 @@ def nms(z: torch.Tensor, conf_thres: float = 0.25, iou_thres: float = 0.45, agno
     return det, count
 
 
+def match_detections(det: torch.Tensor, count: torch.Tensor, targets: torch.Tensor, ratio_pad: torch.Tensor, height: int,
+                     width: int, iouv: torch.Tensor, single_cls: bool = False, correct: Optional[torch.Tensor] = None,
+                     native: Optional[torch.Tensor] = None, workspace: Optional[torch.Tensor] = None):
+    """test.py:196-227 for one batch on the device: which NMS detections are true positives at each IoU threshold.
+    det / count: what :func:`nms` returns.  targets: fp32 (T, 6) rows [image, cls, x, y, w, h] normalised to the
+    (height, width) batch.  ratio_pad: fp32 (B, 5) rows [h0, w0, gain, padw, padh] (the loader's ``shapes``).  iouv: fp32
+    (niou,) thresholds on the device.  Returns (correct uint8 (B, max_det, niou), native): ``native`` (fp32 (B, max_det, 4),
+    the scale_coords boxes) is written only when passed in.  Rows at or past ``count`` are zero.  No host sync."""
+    if det.dim() != 3 or det.shape[2] != 6 or det.dtype != torch.float32 or not det.is_contiguous() or not on_device(det):
+        raise ValueError(f"match_detections: det must be contiguous CUDA fp32 (B, max_det, 6), got {det.dtype} {tuple(det.shape)}")
+    B, max_det = det.shape[0], det.shape[1]
+    niou = iouv.numel()
+    if tuple(count.shape) != (B,) or count.dtype != torch.int32:
+        raise ValueError("match_detections: count must be int32 (B,)")
+    if targets.dim() != 2 or targets.shape[1] != 6 or targets.dtype != torch.float32 or not targets.is_contiguous():
+        raise ValueError(f"match_detections: targets must be contiguous fp32 (T, 6), got {targets.dtype} {tuple(targets.shape)}")
+    if tuple(ratio_pad.shape) != (B, 5) or ratio_pad.dtype != torch.float32 or not ratio_pad.is_contiguous():
+        raise ValueError("match_detections: ratio_pad must be contiguous fp32 (B, 5)")
+    if iouv.dtype != torch.float32 or iouv.dim() != 1 or not 1 <= niou <= 32:
+        raise ValueError("match_detections: iouv must be fp32 (niou,) with 1 <= niou <= 32")
+    for t, what in ((count, "count"), (targets, "targets"), (ratio_pad, "ratio_pad"), (iouv, "iouv")):
+        if t.device != det.device:
+            raise ValueError(f"match_detections: {what} is on {t.device}, det on {det.device}")
+    if correct is None:
+        correct = torch.empty(B, max_det, niou, dtype=torch.uint8, device=det.device)
+    elif tuple(correct.shape) != (B, max_det, niou) or correct.dtype not in (torch.uint8, torch.bool) or not correct.is_contiguous():
+        raise ValueError(f"match_detections: correct must be contiguous uint8 / bool {(B, max_det, niou)}")
+    if native is not None and (tuple(native.shape) != (B, max_det, 4) or native.dtype != torch.float32 or not native.is_contiguous()):
+        raise ValueError(f"match_detections: native must be contiguous fp32 {(B, max_det, 4)}")
+    T = int(targets.shape[0])
+    need = int(_lib.lib().icaf_match_detections_workspace_bytes(T))
+    if workspace is None or workspace.numel() * workspace.element_size() < need:
+        workspace = torch.empty(max((need + 3) // 4, 1), dtype=torch.int32, device=det.device)
+    _call("icaf_match_detections", _lib.lib().icaf_match_detections,
+          (_ptr(det), _ptr(count), B, max_det, _ptr(targets if T else None), T, _ptr(ratio_pad), int(height), int(width),
+           _ptr(iouv), niou, int(bool(single_cls)), _ptr(correct), _ptr(native), _ptr(workspace),
+           C.c_size_t(workspace.numel() * workspace.element_size())),
+          {"bytes": float(det.numel() * 4 + B * max_det * niou + T * 24 * B)})
+    return correct, native
+
+
 # ---------------------------------------------------------------------------------------------------------------
 # Training-step building blocks (operator level; see include/icaf_b200.h).  Gradients of Conv2d / Linear layers.
 def conv2d_wgrad(x: torch.Tensor, dy: torch.Tensor, kh: int, kw: int, stride: int, pad: int, scale: float = 1.0,

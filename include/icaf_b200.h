@@ -245,6 +245,23 @@ int icaf_nms_multi_label(const void* z, int B, int R, int no, float conf_thres, 
                          void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * Validation: match one batch's NMS detections to its labels (test.py:196-227), one launch, no host round trip.
+ * det / count: what icaf_nms / icaf_nms_multi_label write, fp32 (B, max_det, 6) and int32 (B).
+ * targets: fp32 (T, 6) rows [image, cls, x, y, w, h] normalised to the (height, width) batch, in any order; rows whose image
+ * is not one of 0..B-1 are ignored.  ratio_pad: fp32 (B, 5) rows [h0, w0, gain, padw, padh] (the loader's shapes[i]).
+ * iouv: device fp32 (niou), 1 <= niou <= 32.  single_cls: every prediction counts as class 0.
+ * Per image: both box sets go through scale_coords (pad, IEEE division by gain, clip to h0 x w0); each prediction takes the
+ * first label of its class with the largest IoU; in row order, a prediction with IoU > iouv[0] whose label is not yet taken
+ * takes it, and correct[b, r, k] = IoU > iouv[k].  correct: uint8 (B, max_det, niou); rows at or past count[b] are zero.
+ * native: optional fp32 (B, max_det, 4), 16-byte aligned: the scale_coords boxes of the predictions (zero past count[b]).
+ * workspace: icaf_match_detections_workspace_bytes(T) bytes of device memory, 4-byte aligned (may be NULL when T == 0).
+ * ------------------------------------------------------------------------------------------- */
+size_t icaf_match_detections_workspace_bytes(int T);
+int icaf_match_detections(const float* det, const int* count, int B, int max_det, const float* targets, int T,
+                          const float* ratio_pad, int height, int width, const float* iouv, int niou, int single_cls,
+                          unsigned char* correct, float* native, void* workspace, size_t workspace_bytes, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * Detection loss, forward only (the validation loss test.py:132-133 accumulates; the training backward is not built):
  * utils/loss.py:325-463 ComputeLoss.__call__ + build_targets -- anchor-ratio matching with the four half-cell neighbour
  * offsets, CIoU box loss, objectness BCE against IoU-valued targets (largest IoU wins a contested cell), class BCE.
