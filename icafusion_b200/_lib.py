@@ -99,6 +99,10 @@ SIGNATURES = {
     "icaf_train_workspace_bytes": [_i],
     "icaf_bn_act_fwd": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _i, _f, _f, _i, _vp, C.c_size_t, _vp],
     "icaf_bn_act_bwd": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _i, _i, _f, _i, _vp, C.c_size_t, _vp],
+    "icaf_bn_act_fwd_stats": [_vp, _i64, _i, _vp, _vp, C.c_size_t, _vp],
+    "icaf_bn_act_fwd_apply": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _i, _f, _f, _i, _vp, C.c_size_t, _vp],
+    "icaf_bn_act_bwd_sums": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _i, _i, _f, _i, _vp, C.c_size_t, _vp],
+    "icaf_bn_act_bwd_apply": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _i, _i, _vp, C.c_size_t, _vp],
     "icaf_eltwise": [_i, _vp, _vp, _vp, _i64, _f, C.c_uint32, _vp],
     "icaf_layernorm_bwd": [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _i, _f, _f, _i, _vp, C.c_size_t, _vp],
     "icaf_dot": [_vp, _vp, _i64, _i, _vp, _f, _i, _vp, C.c_size_t, _vp],

@@ -47,6 +47,10 @@ def _f32(t: torch.Tensor) -> torch.Tensor:
 # ------------------------------------------------------------------------------------------------
 # Conv2d (no bias) + BatchNorm2d (batch statistics) + activation            models/common.py:48-57
 class ConvBnActFn(Function):
+    """A SyncBatchNorm `bn` (train.py --sync-bn) takes the two-phase BatchNorm with one exchange per direction when sync_group
+    says so.  The exchange is queued on the current stream, which is the one this node's kernels (and, by autograd, its
+    backward's) run on, side streams included."""
+
     @staticmethod
     def forward(ctx, x, weight, gamma, beta, bn: nn.BatchNorm2d, stride: int, pad: int, act: int, stem: bool):
         w = _f32(weight)
@@ -59,22 +63,35 @@ class ConvBnActFn(Function):
             pk = ops.pack_weight(w, stride, pad)
         z = ops.conv2d([x], [pk])[0]
         mom = 0.1 if bn.momentum is None else bn.momentum
-        y, sm, si = ops.bn_act_fwd(z, _f32(gamma), _f32(beta), bn.running_mean, bn.running_var, bn.eps, mom, act)
+        ctx.group = sync_group(bn)
+        count = None
+        if ctx.group is None:
+            y, sm, si = ops.bn_act_fwd(z, _f32(gamma), _f32(beta), bn.running_mean, bn.running_var, bn.eps, mom, act)
+        else:         # SyncBatchNorm: statistics over the rows of every rank of the group
+            stats = ops.all_reduce_(ops.bn_act_fwd_stats(z), ctx.group)
+            y, sm, si = ops.bn_act_fwd_apply(z, _f32(gamma), _f32(beta), bn.running_mean, bn.running_var, stats, bn.eps, mom, act)
+            count = stats[-1:]                      # the global row count, for the backward
         if bn.num_batches_tracked is not None:     # nn.BatchNorm2d's step counter: one fused increment per model forward
             _STATE["bn"].append(bn.num_batches_tracked)
             if not _STATE["defer_bn"]:
                 _flush_bn_counters()
-        ctx.save_for_backward(x, z, weight, gamma, beta, sm, si)
+        ctx.save_for_backward(x, z, weight, gamma, beta, sm, si, count)
         ctx.cfg = (stride, pad, act, stem)
         return y
 
     @staticmethod
     def backward(ctx, dy):
-        x, z, weight, gamma, beta, sm, si = ctx.saved_tensors
+        x, z, weight, gamma, beta, sm, si, count = ctx.saved_tensors
         stride, pad, act, stem = ctx.cfg
         dgamma = torch.empty(gamma.shape, dtype=torch.float32, device=z.device)
         dbeta = torch.empty_like(dgamma)
-        dz = ops.bn_act_bwd(z, dy, _f32(gamma), _f32(beta), sm, si, act, dgamma, dbeta)
+        if ctx.group is None:
+            dz = ops.bn_act_bwd(z, dy, _f32(gamma), _f32(beta), sm, si, act, dgamma, dbeta)
+        else:         # SyncBatchNorm: dgamma / dbeta stay local (DDP averages them); the two sums dx needs are summed over ranks
+            dy = dy.contiguous()
+            g32, b32 = _f32(gamma), _f32(beta)
+            sums = ops.all_reduce_(ops.bn_act_bwd_sums(z, dy, g32, b32, sm, si, act, dgamma, dbeta), ctx.group)
+            dz = ops.bn_act_bwd_apply(z, dy, g32, b32, sm, si, sums, count, act)
         cout, cin, kh, kw = weight.shape
         if stem:
             d16 = ops.conv2d_wgrad(x, dz, 3, 3, 1, 1)                         # (Cout, 16 = (dy,dx,c4), ty, tx)
@@ -84,6 +101,19 @@ class ConvBnActFn(Function):
             dw = ops.conv2d_wgrad(x, dz, kh, kw, stride, pad)
             dx = ops.conv2d_dgrad(dz, _f32(weight), stride, pad, (x.shape[1], x.shape[2]), ctx.pk_dgrad) if ctx.needs_input_grad[0] else None
         return dx, dw.to(weight.dtype), dgamma.to(gamma.dtype), dbeta.to(beta.dtype), None, None, None, None, None
+
+
+def sync_group(bn: nn.Module):
+    """The process group a BatchNorm's training statistics are summed over, or None for per-rank statistics: torch's own
+    SyncBatchNorm rule -- an nn.SyncBatchNorm in training mode, torch.distributed initialised, and more than one rank in
+    ``bn.process_group`` (WORLD when unset)."""
+    if not (isinstance(bn, nn.SyncBatchNorm) and bn.training):
+        return None
+    import torch.distributed as dist
+    if not (dist.is_available() and dist.is_initialized()):
+        return None
+    group = dist.group.WORLD if bn.process_group is None else bn.process_group
+    return group if dist.get_world_size(group) > 1 else None
 
 
 def _flush_bn_counters() -> None:

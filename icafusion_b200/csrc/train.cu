@@ -106,10 +106,14 @@ __device__ __forceinline__ void chunk_sums(const float* __restrict__ part, int C
     for (int y = 0; y < kFinLanes; ++y) { s += sm[0][y][threadIdx.x]; q += sm[1][y][threadIdx.x]; }
 }
 
-// BatchNorm statistics, second stage: mean, invstd, and the running statistics update (momentum, unbiased variance)
+// BatchNorm statistics, second stage: mean, invstd, and the running statistics update (momentum, unbiased variance).
+// DEV_COUNT: the row count is read as fp32 from device memory (`count`) in place of `rows` (the global count of a synchronised
+// BatchNorm); a template argument, so that the one-call path compiles to exactly the code it had before the synchronised form
+template <bool DEV_COUNT>
 __global__ void __launch_bounds__(1024) bn_finalize_kernel(const float* __restrict__ part, float* __restrict__ mean, float* __restrict__ invstd, float* run_mean,
                                                           float* run_var, int C, long long rows, float eps, float momentum, int chunks,
-                                                          const float* __restrict__ gamma, const float* __restrict__ beta, float* __restrict__ ab) {
+                                                          const float* __restrict__ gamma, const float* __restrict__ beta, float* __restrict__ ab,
+                                                          const float* __restrict__ count) {
   pdl_launch_dependents();
   pdl_wait();
   __shared__ float sm[2][kFinLanes][33];
@@ -117,8 +121,9 @@ __global__ void __launch_bounds__(1024) bn_finalize_kernel(const float* __restri
   float s, q;
   chunk_sums(part, C, chunks, c, s, q, sm);
   if (c >= C || threadIdx.y) return;
-  const float m = s / float(rows);
-  const float var = fmaxf(q / float(rows) - m * m, 0.f);
+  const float n = DEV_COUNT ? __ldg(count) : float(rows);
+  const float m = s / n;
+  const float var = fmaxf(q / n - m * m, 0.f);
   mean[c] = m;
   const float is = rsqrtf(var + eps);
   invstd[c] = is;
@@ -126,15 +131,19 @@ __global__ void __launch_bounds__(1024) bn_finalize_kernel(const float* __restri
   ab[c] = a; ab[C + c] = beta[c] - m * a;                   // the apply pass: y = act(x * a + b)
   if (run_mean) {
     run_mean[c] = (1.f - momentum) * run_mean[c] + momentum * m;
-    run_var[c] = (1.f - momentum) * run_var[c] + momentum * var * (rows > 1 ? float(rows) / float(rows - 1) : 1.f);
+    const float unbias = DEV_COUNT ? (n > 1.f ? n / (n - 1.f) : 1.f) : (rows > 1 ? float(rows) / float(rows - 1) : 1.f);
+    run_var[c] = (1.f - momentum) * run_var[c] + momentum * var * unbias;
   }
 }
 // generic second stage: out[which][c] = (accumulate ? out : 0) + scale * sum_chunks part
 // out0/out1: sums (scale, accumulate); raw0/raw1 (optional): the unscaled sums as well (BatchNorm backward needs both in one pass)
+// DEV_COUNT: count_out (optional): count_out[0] = n_rows; count (optional): inv_m = 1 / count[0], read from device memory
+template <bool DEV_COUNT>
 __global__ void __launch_bounds__(1024) chan_final_kernel(const float* __restrict__ part, float* __restrict__ out0, float* __restrict__ out1, int C, float scale,
                                                           int accumulate, int chunks, float* __restrict__ raw0, float* __restrict__ raw1,
                                                           const float* __restrict__ gamma, const float* __restrict__ beta, const float* __restrict__ mean,
-                                                          const float* __restrict__ invstd, float inv_m, float* __restrict__ coef) {
+                                                          const float* __restrict__ invstd, float inv_m, float* __restrict__ coef,
+                                                          const float* __restrict__ count, float* __restrict__ count_out, float n_rows) {
   pdl_launch_dependents();
   pdl_wait();
   __shared__ float sm[2][kFinLanes][33];
@@ -142,9 +151,11 @@ __global__ void __launch_bounds__(1024) chan_final_kernel(const float* __restric
   float s, q;
   chunk_sums(part, C, chunks, c, s, q, sm);
   if (c >= C || threadIdx.y) return;
+  if (DEV_COUNT && count_out && c == 0) count_out[0] = n_rows;
   if (raw0) raw0[c] = s;
   if (raw1) raw1[c] = q;
   if (coef) {      // BatchNorm backward apply pass: dx = a * (dz - k1 - (x - mean) * k2), z = x * a + b
+    if (DEV_COUNT && count) inv_m = 1.f / __ldg(count);
     const float is = invstd[c], a = gamma[c] * is, m = mean[c];
     coef[c] = a; coef[C + c] = beta[c] - m * a; coef[2 * C + c] = m; coef[3 * C + c] = s * inv_m; coef[4 * C + c] = q * inv_m * is;
   }
@@ -305,9 +316,9 @@ extern "C" int icaf_bn_act_fwd(const void* x, const float* gamma, const float* b
   if (int rc = launch_k("bn_act_fwd(stats)", chan_partial_kernel<0>, dim3(blocks_for(C / 8, 32), chunks), dim3(256), 0, st, (const __half*)x,
                         (const __half*)nullptr, (const float*)nullptr, (const float*)nullptr, (const float*)nullptr, (const float*)nullptr, workspace,
                         (long long)rows, C, 0, chunks)) return rc;
-  if (int rc = launch_k("bn_act_fwd(finalize)", bn_finalize_kernel, dim3(blocks_for(C, 32)), dim3(32, kFinLanes), 0, st, (const float*)workspace,
+  if (int rc = launch_k("bn_act_fwd(finalize)", bn_finalize_kernel<false>, dim3(blocks_for(C, 32)), dim3(32, kFinLanes), 0, st, (const float*)workspace,
                         save_mean, save_invstd, run_mean, run_var, C, (long long)rows, eps, momentum, chunks, gamma, beta,
-                        workspace + size_t(kRedChunks) * 2 * C)) return rc;
+                        workspace + size_t(kRedChunks) * 2 * C, (const float*)nullptr)) return rc;
   const long long n8 = rows * (C / 8);
   return launch_k("bn_act_fwd", affine_act_kernel, dim3(blocks_for(n8, 256)), dim3(256), 0, st, (const __half*)x,
                   (const float*)(workspace + size_t(kRedChunks) * 2 * C), (__half*)y, n8, C / 8, act);
@@ -324,11 +335,70 @@ extern "C" int icaf_bn_act_bwd(const void* x, const void* dy, const float* gamma
   if (int rc = launch_k("bn_act_bwd(partial)", chan_partial_kernel<1>, dim3(blocks_for(C / 8, 32), chunks), dim3(256), 0, st, (const __half*)x,
                         (const __half*)dy, gamma, beta, save_mean, save_invstd, workspace, (long long)rows, C, act, chunks)) return rc;
   // one second stage: the apply pass's coefficients and the parameter gradients dbeta = S1, dgamma = S2 (scaled by grad_scale)
-  if (int rc = launch_k("bn_act_bwd(sums)", chan_final_kernel, dim3(blocks_for(C, 32)), dim3(32, kFinLanes), 0, st, (const float*)workspace, dbeta,
+  if (int rc = launch_k("bn_act_bwd(sums)", chan_final_kernel<false>, dim3(blocks_for(C, 32)), dim3(32, kFinLanes), 0, st, (const float*)workspace, dbeta,
                         dgamma, C, grad_scale, accumulate, chunks, (float*)nullptr, (float*)nullptr, gamma, beta, save_mean, save_invstd,
-                        1.0f / float(rows), coef)) return rc;
+                        1.0f / float(rows), coef, (const float*)nullptr, (float*)nullptr, 0.f)) return rc;
   const long long n8 = rows * (C / 8);
   return launch_k("bn_act_bwd", bn_bwd_apply_kernel, dim3(blocks_for(n8, 256)), dim3(256), 0, st, (const __half*)x, (const __half*)dy,
+                  (const float*)coef, (__half*)dx, n8, C / 8, act);
+}
+
+// Synchronised BatchNorm: the two calls above, each split where its per-channel sums are complete.  The caller sums the
+// exchange buffer over the ranks between the phases.  Phase 2 reads the buffer as a one-chunk partial-sum array, so the
+// second stages are the ones above run over one chunk, with the row count read from the buffer.
+extern "C" int icaf_bn_act_fwd_stats(const void* x, int64_t rows, int C, float* stats, float* workspace, size_t workspace_bytes, void* stream) {
+  if (!x || !stats || !workspace || rows < 1 || C < 8 || C % 8) return set_error(ICAF_ERR_BAD_ARG, "bn_act_fwd_stats: bad argument");
+  if (workspace_bytes < icaf_train_workspace_bytes(C)) return set_error(ICAF_ERR_BAD_ARG, "bn_act_fwd_stats: workspace too small (icaf_train_workspace_bytes)");
+  cudaStream_t st = (cudaStream_t)stream;
+  const int chunks = pick_chunks(rows, C);
+  if (int rc = launch_k("bn_act_fwd_stats(partial)", chan_partial_kernel<0>, dim3(blocks_for(C / 8, 32), chunks), dim3(256), 0, st, (const __half*)x,
+                        (const __half*)nullptr, (const float*)nullptr, (const float*)nullptr, (const float*)nullptr, (const float*)nullptr, workspace,
+                        (long long)rows, C, 0, chunks)) return rc;
+  return launch_k("bn_act_fwd_stats(sums)", chan_final_kernel<true>, dim3(blocks_for(C, 32)), dim3(32, kFinLanes), 0, st, (const float*)workspace,
+                  (float*)nullptr, (float*)nullptr, C, 0.f, 0, chunks, stats, stats + C, (const float*)nullptr, (const float*)nullptr,
+                  (const float*)nullptr, (const float*)nullptr, 0.f, (float*)nullptr, (const float*)nullptr, stats + 2 * C, float(rows));
+}
+
+extern "C" int icaf_bn_act_fwd_apply(const void* x, const float* gamma, const float* beta, float* run_mean, float* run_var, const float* stats, void* y,
+                                     float* save_mean, float* save_invstd, int64_t rows, int C, float eps, float momentum, int act, float* workspace,
+                                     size_t workspace_bytes, void* stream) {
+  if (!x || !gamma || !beta || !stats || !y || !save_mean || !save_invstd || !workspace || rows < 1 || C < 8 || C % 8) return set_error(ICAF_ERR_BAD_ARG, "bn_act_fwd_apply: bad argument");
+  if (workspace_bytes < icaf_train_workspace_bytes(C)) return set_error(ICAF_ERR_BAD_ARG, "bn_act_fwd_apply: workspace too small (icaf_train_workspace_bytes)");
+  cudaStream_t st = (cudaStream_t)stream;
+  float* ab = workspace + size_t(kRedChunks) * 2 * C;
+  if (int rc = launch_k("bn_act_fwd_apply(finalize)", bn_finalize_kernel<true>, dim3(blocks_for(C, 32)), dim3(32, kFinLanes), 0, st, stats, save_mean,
+                        save_invstd, run_mean, run_var, C, (long long)rows, eps, momentum, 1, gamma, beta, ab, stats + 2 * C)) return rc;
+  const long long n8 = rows * (C / 8);
+  return launch_k("bn_act_fwd_apply", affine_act_kernel, dim3(blocks_for(n8, 256)), dim3(256), 0, st, (const __half*)x, (const float*)ab, (__half*)y,
+                  n8, C / 8, act);
+}
+
+extern "C" int icaf_bn_act_bwd_sums(const void* x, const void* dy, const float* gamma, const float* beta, const float* save_mean, const float* save_invstd,
+                                    float* dgamma, float* dbeta, float* sums, int64_t rows, int C, int act, float grad_scale, int accumulate, float* workspace,
+                                    size_t workspace_bytes, void* stream) {
+  if (!x || !dy || !gamma || !beta || !save_mean || !save_invstd || !sums || !workspace || rows < 1 || C < 8 || C % 8) return set_error(ICAF_ERR_BAD_ARG, "bn_act_bwd_sums: bad argument");
+  if (workspace_bytes < icaf_train_workspace_bytes(C)) return set_error(ICAF_ERR_BAD_ARG, "bn_act_bwd_sums: workspace too small (icaf_train_workspace_bytes)");
+  cudaStream_t st = (cudaStream_t)stream;
+  const int chunks = pick_chunks(rows, C);
+  if (int rc = launch_k("bn_act_bwd_sums(partial)", chan_partial_kernel<1>, dim3(blocks_for(C / 8, 32), chunks), dim3(256), 0, st, (const __half*)x,
+                        (const __half*)dy, gamma, beta, save_mean, save_invstd, workspace, (long long)rows, C, act, chunks)) return rc;
+  return launch_k("bn_act_bwd_sums(sums)", chan_final_kernel<false>, dim3(blocks_for(C, 32)), dim3(32, kFinLanes), 0, st, (const float*)workspace, dbeta,
+                  dgamma, C, grad_scale, accumulate, chunks, sums, sums + C, (const float*)nullptr, (const float*)nullptr, (const float*)nullptr,
+                  (const float*)nullptr, 0.f, (float*)nullptr, (const float*)nullptr, (float*)nullptr, 0.f);
+}
+
+extern "C" int icaf_bn_act_bwd_apply(const void* x, const void* dy, const float* gamma, const float* beta, const float* save_mean, const float* save_invstd,
+                                     const float* sums, const float* count, void* dx, int64_t rows, int C, int act, float* workspace, size_t workspace_bytes,
+                                     void* stream) {
+  if (!x || !dy || !gamma || !beta || !save_mean || !save_invstd || !sums || !count || !dx || !workspace || rows < 1 || C < 8 || C % 8) return set_error(ICAF_ERR_BAD_ARG, "bn_act_bwd_apply: bad argument");
+  if (workspace_bytes < icaf_train_workspace_bytes(C)) return set_error(ICAF_ERR_BAD_ARG, "bn_act_bwd_apply: workspace too small (icaf_train_workspace_bytes)");
+  cudaStream_t st = (cudaStream_t)stream;
+  float* coef = workspace + size_t(kRedChunks) * 2 * C;
+  if (int rc = launch_k("bn_act_bwd_apply(coef)", chan_final_kernel<true>, dim3(blocks_for(C, 32)), dim3(32, kFinLanes), 0, st, sums, (float*)nullptr,
+                        (float*)nullptr, C, 0.f, 0, 1, (float*)nullptr, (float*)nullptr, gamma, beta, save_mean, save_invstd, 0.f, coef, count,
+                        (float*)nullptr, 0.f)) return rc;
+  const long long n8 = rows * (C / 8);
+  return launch_k("bn_act_bwd_apply", bn_bwd_apply_kernel, dim3(blocks_for(n8, 256)), dim3(256), 0, st, (const __half*)x, (const __half*)dy,
                   (const float*)coef, (__half*)dx, n8, C / 8, act);
 }
 
@@ -357,9 +427,10 @@ extern "C" int icaf_layernorm_bwd(const void* x, const void* dy, const float* ga
     if (int rc = launch_k("layernorm_bwd(partial)", chan_partial_kernel<2>, dim3(blocks_for(C / 8, 32), chunks), dim3(256), 0, st, (const __half*)x,
                           (const __half*)dy, (const float*)nullptr, (const float*)nullptr, (const float*)rmean, (const float*)rrstd, workspace,
                           (long long)rows, C, 0, chunks)) return rc;
-    if (int rc = launch_k("layernorm_bwd(param grads)", chan_final_kernel, dim3(blocks_for(C, 32)), dim3(32, kFinLanes), 0, st,
+    if (int rc = launch_k("layernorm_bwd(param grads)", chan_final_kernel<false>, dim3(blocks_for(C, 32)), dim3(32, kFinLanes), 0, st,
                           (const float*)workspace, dbeta, dgamma, C, grad_scale, accumulate, chunks, (float*)nullptr, (float*)nullptr,
-                          (const float*)nullptr, (const float*)nullptr, (const float*)nullptr, (const float*)nullptr, 0.f, (float*)nullptr)) return rc;
+                          (const float*)nullptr, (const float*)nullptr, (const float*)nullptr, (const float*)nullptr, 0.f, (float*)nullptr,
+                          (const float*)nullptr, (float*)nullptr, 0.f)) return rc;
   }
   return ICAF_OK;
 }

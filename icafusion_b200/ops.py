@@ -831,6 +831,73 @@ def bn_act_bwd(x, dy, gamma, beta, sm, si, act: int, dgamma=None, dbeta=None, gr
     return dx
 
 
+# Synchronised BatchNorm (torch.nn.SyncBatchNorm): bn_act_fwd / bn_act_bwd in two phases each, with the per-channel sums of
+# phase 1 summed over the ranks (all_reduce_) before phase 2.  Fed phase 1's buffer unchanged, phase 2 equals the one-call form.
+def bn_act_fwd_stats(x: torch.Tensor) -> torch.Tensor:
+    """Phase 1 of the forward: -> fp32 [2C + 1] = (sum x, sum x^2 per channel, row count) of this rank's dense NHWC map."""
+    Cc = x.shape[-1]
+    rows = x.numel() // Cc
+    assert x.is_contiguous() and x.dtype == torch.float16
+    stats = torch.empty(2 * Cc + 1, dtype=torch.float32, device=x.device)
+    ws = _train_ws(Cc, 0, x.device)
+    _call("icaf_bn_act_fwd_stats", _lib.lib().icaf_bn_act_fwd_stats, (_ptr(x), rows, Cc, _ptr(stats), _ptr(ws), C.c_size_t(ws.numel() * 4)),
+          {"bytes": 2.0 * x.numel()})
+    return stats
+
+
+def bn_act_fwd_apply(x: torch.Tensor, gamma, beta, run_mean, run_var, stats, eps: float, momentum: float, act: int):
+    """Phase 2 of the forward from the summed `stats`: -> (y, save_mean, save_invstd) over the rows of every rank."""
+    Cc = x.shape[-1]
+    rows = x.numel() // Cc
+    assert x.is_contiguous() and x.dtype == torch.float16 and stats.numel() == 2 * Cc + 1
+    y = torch.empty_like(x)
+    sm = torch.empty(Cc, dtype=torch.float32, device=x.device)
+    si = torch.empty_like(sm)
+    ws = _train_ws(Cc, 0, x.device)
+    _call("icaf_bn_act_fwd_apply", _lib.lib().icaf_bn_act_fwd_apply,
+          (_ptr(x), _ptr(gamma), _ptr(beta), _ptr(run_mean), _ptr(run_var), _ptr(stats), _ptr(y), _ptr(sm), _ptr(si), rows, Cc, float(eps),
+           float(momentum), int(act), _ptr(ws), C.c_size_t(ws.numel() * 4)), {"bytes": 4.0 * x.numel()})
+    return y, sm, si
+
+
+def bn_act_bwd_sums(x, dy, gamma, beta, sm, si, act: int, dgamma=None, dbeta=None, grad_scale: float = 1.0, accumulate: bool = False):
+    """Phase 1 of the backward: dgamma / dbeta of this rank's rows, -> fp32 [2C] = (sum dz, sum dz * xhat) to be summed.
+    `dy` must be contiguous (phase 2 reads the same tensor)."""
+    Cc = x.shape[-1]
+    rows = x.numel() // Cc
+    assert dy.is_contiguous()
+    sums = torch.empty(2 * Cc, dtype=torch.float32, device=x.device)
+    ws = _train_ws(Cc, 0, x.device)
+    _call("icaf_bn_act_bwd_sums", _lib.lib().icaf_bn_act_bwd_sums,
+          (_ptr(x), _ptr(dy), _ptr(gamma), _ptr(beta), _ptr(sm), _ptr(si), _ptr(dgamma), _ptr(dbeta), _ptr(sums), rows, Cc, int(act), float(grad_scale),
+           int(accumulate), _ptr(ws), C.c_size_t(ws.numel() * 4)), {"bytes": 4.0 * x.numel()})
+    return sums
+
+
+def bn_act_bwd_apply(x, dy, gamma, beta, sm, si, sums, count, act: int):
+    """Phase 2 of the backward: dx from the summed `sums` and the forward's summed row count (`count`: fp32 [1] on the device)."""
+    Cc = x.shape[-1]
+    rows = x.numel() // Cc
+    assert dy.is_contiguous() and sums.numel() == 2 * Cc and count.numel() == 1
+    dx = torch.empty_like(x)
+    ws = _train_ws(Cc, 0, x.device)
+    _call("icaf_bn_act_bwd_apply", _lib.lib().icaf_bn_act_bwd_apply,
+          (_ptr(x), _ptr(dy), _ptr(gamma), _ptr(beta), _ptr(sm), _ptr(si), _ptr(sums), _ptr(count), _ptr(dx), rows, Cc, int(act), _ptr(ws),
+           C.c_size_t(ws.numel() * 4)), {"bytes": 6.0 * x.numel()})
+    return dx
+
+
+def all_reduce_(buf: torch.Tensor, group=None) -> torch.Tensor:
+    """Sum `buf` over the ranks of `group` in place: torch.distributed.all_reduce, ordered on the current stream (NCCL makes
+    the stream wait, not the host, so it can be captured in a CUDA graph).  A dry run records it as ("all_reduce", (buf,),
+    work) instead, so a walk counts exchanges as it counts launches."""
+    if _DRY is not None:
+        _DRY.append(("all_reduce", (buf,), {"bytes": 4.0 * buf.numel(), "group": group}))
+        return buf
+    torch.distributed.all_reduce(buf, group=group)
+    return buf
+
+
 def eltwise(mode: int, x, dy=None, p: float = 0.0, seed: int = 0):
     x = x.contiguous()
     y = torch.empty_like(x)

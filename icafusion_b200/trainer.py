@@ -48,12 +48,14 @@ def freeze_dead_parameters(model: nn.Module) -> List[str]:
 
 
 def param_groups(model: nn.Module):
-    """train.py:124-131: (BatchNorm weights [no decay], other weights [decay], biases), trainable parameters only."""
+    """train.py:124-131: (BatchNorm weights [no decay], other weights [decay], biases), trainable parameters only.  A model
+    converted to nn.SyncBatchNorm beforehand gets the groups of the unconverted one (the reference builds its groups before
+    converting, train.py:124-131 then 196)."""
     pg0, pg1, pg2 = [], [], []
     for _, v in model.named_modules():
         if hasattr(v, "bias") and isinstance(v.bias, nn.Parameter) and v.bias.requires_grad:
             pg2.append(v.bias)
-        if isinstance(v, nn.BatchNorm2d):
+        if isinstance(v, (nn.BatchNorm2d, nn.SyncBatchNorm)):
             if v.weight.requires_grad:
                 pg0.append(v.weight)
         elif hasattr(v, "weight") and isinstance(v.weight, nn.Parameter) and v.weight.requires_grad:
@@ -98,10 +100,14 @@ class ModelEMA:
 
 
 class TrainStep:
-    """model -> (optional DDP) -> loss -> scaled backward -> optimiser step, per call (train.py:334-349)."""
+    """model -> (optional DDP) -> loss -> scaled backward -> optimiser step, per call (train.py:334-349).
+
+    sync_bn (train.py --sync-bn): with world_size > 1, every BatchNorm2d is converted to nn.SyncBatchNorm after the optimiser
+    groups are built and before the DDP wrap (train.py:195-198), so BatchNorm normalises over the batch of all ranks.  At
+    world size 1 the model is left as it is.  A model the caller converted beforehand trains synchronised as well."""
 
     def __init__(self, model: nn.Module, hyp: Optional[Dict[str, float]] = None, total_batch_size: int = 64, world_size: int = 1,
-                 local_rank: Optional[int] = None, imgsz: int = 640, amp_scale: bool = True, ema: bool = False):
+                 local_rank: Optional[int] = None, imgsz: int = 640, amp_scale: bool = True, ema: bool = False, sync_bn: bool = False):
         hyp = dict(HYP_SCRATCH if hyp is None else hyp)
         det = model.model[-1]
         nl, nc = det.nl, det.nc
@@ -117,6 +123,8 @@ class TrainStep:
         hyp["cls"] *= nc / 80.0 * 3.0 / nl
         hyp["obj"] *= (imgsz / 640) ** 2 * 3.0 / nl
         model.nc, model.hyp, model.gr = nc, hyp, 1.0                                  # train.py:242-244
+        if sync_bn and world_size > 1:
+            model = nn.SyncBatchNorm.convert_sync_batchnorm(model)                     # train.py:195-198
         self.raw_model = model
         self.world_size = world_size
         if world_size > 1:
@@ -163,6 +171,12 @@ class GraphedTrainStep:
     before init_process_group, as torch's CUDA-graph notes require; 11 eager iterations run before the capture."""
 
     def __init__(self, ts: TrainStep, B: int, H: int, W: int, max_targets: int, device, warmup: Optional[int] = None):
+        from .autograd import sync_group
+        for m in ts.raw_model.modules():           # SyncBatchNorm exchanges are captured like DDP's all-reduces: over NCCL only
+            g = sync_group(m)
+            if g is not None and torch.distributed.get_backend(g) != "nccl":
+                raise ValueError(f"GraphedTrainStep: synchronised BatchNorm needs an NCCL process group to be captured, "
+                                 f"got {torch.distributed.get_backend(g)}")
         self.ts = ts
         dev = torch.device(device)
         self.rgb = torch.zeros(B, 3, H, W, dtype=torch.uint8, device=dev)

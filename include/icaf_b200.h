@@ -329,6 +329,26 @@ int icaf_bn_act_fwd(const void* x, const float* gamma, const float* beta, float*
 int icaf_bn_act_bwd(const void* x, const void* dy, const float* gamma, const float* beta, const float* save_mean, const float* save_invstd,
                     void* dx, float* dgamma, float* dbeta, int64_t rows, int C, int act, float grad_scale, int accumulate, float* workspace,
                     size_t workspace_bytes, void* stream);
+/* The same two calls in two phases each, for a BatchNorm synchronised over ranks (torch.nn.SyncBatchNorm).  The caller sums
+ * the exchange buffer over the ranks between the phases (all-reduce).  Fed phase 1's buffer unchanged, phase 2 gives what
+ * icaf_bn_act_fwd / icaf_bn_act_bwd give, bit for bit, for rows <= 2^24.
+ * Forward phase 1: stats (fp32 [2C + 1]) = (sum x [C], sum x^2 [C], rows).  The count travels as fp32: above 2^24 rows it is
+ * rounded, a relative error of at most 6e-8, below the error of the fp32 sums themselves.
+ * Forward phase 2: mean, invstd and the running-statistics update (unbiased with the summed count) from the summed stats, then
+ * y as icaf_bn_act_fwd.  The count is read from device memory: ranks may hold different row counts and no host read is needed.
+ * Backward phase 1: dgamma / dbeta of this rank's rows as icaf_bn_act_bwd (DDP averages them), and sums (fp32 [2C]) =
+ * (sum dz, sum dz * xhat).  Backward phase 2: dx from the summed sums and the forward's summed count (count = stats + 2C).
+ * rows: this rank's rows.  workspace: icaf_train_workspace_bytes(C) each. */
+int icaf_bn_act_fwd_stats(const void* x, int64_t rows, int C, float* stats, float* workspace, size_t workspace_bytes, void* stream);
+int icaf_bn_act_fwd_apply(const void* x, const float* gamma, const float* beta, float* run_mean, float* run_var, const float* stats, void* y,
+                          float* save_mean, float* save_invstd, int64_t rows, int C, float eps, float momentum, int act, float* workspace,
+                          size_t workspace_bytes, void* stream);
+int icaf_bn_act_bwd_sums(const void* x, const void* dy, const float* gamma, const float* beta, const float* save_mean, const float* save_invstd,
+                         float* dgamma, float* dbeta, float* sums, int64_t rows, int C, int act, float grad_scale, int accumulate, float* workspace,
+                         size_t workspace_bytes, void* stream);
+int icaf_bn_act_bwd_apply(const void* x, const void* dy, const float* gamma, const float* beta, const float* save_mean, const float* save_invstd,
+                          const float* sums, const float* count, void* dx, int64_t rows, int C, int act, float* workspace, size_t workspace_bytes,
+                          void* stream);
 /* Element-wise over n fp16 values (n % 8 == 0): mode 0 y = GELU_erf(x) (common.py:706); 1 y = dy * GELU'(x);
  * 2 y = dropout(x, p) with a counter-based mask keyed by (element index, seed) -- calling it on dy with the same seed is the backward. */
 int icaf_eltwise(int mode, const void* x, const void* dy, void* y, int64_t n, float p, uint32_t seed, void* stream);
