@@ -87,6 +87,9 @@ SIGNATURES = {
     "icaf_nms_multi_label": [_vp, _i, _i, _i, _f, _f, _i, C.c_uint64, _i, _vp, _vp, _vp, C.c_size_t, _vp],
     "icaf_match_detections_workspace_bytes": [_i],
     "icaf_match_detections": [_vp, _vp, _i, _i, _vp, _i, _vp, _i, _i, _vp, _i, _i, _vp, _vp, _vp, C.c_size_t, _vp],
+    "icaf_kaist_mr_workspace_bytes": [_i, _i, _i],
+    "icaf_kaist_mr": [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp, C.c_size_t, _vp],
+    "icaf_kaist_round_detections": [_vp, _vp, _vp, _vp, _i, _i, _i, _vp, _vp, _vp],
     "icaf_loss_workspace_bytes": [_i, _i, _i, C.POINTER(C.c_int), C.POINTER(C.c_int), _i, _i],
     "icaf_compute_loss_fwd": [C.POINTER(C.c_void_p), _i, _i, C.POINTER(C.c_int), C.POINTER(C.c_int), _i, _i, _i, _i, _vp, _i,
                               C.POINTER(C.c_float), C.POINTER(LossHyp), _vp, _vp, C.c_size_t, _vp],
@@ -144,6 +147,7 @@ def lib() -> C.CDLL:
                           "icaf_nms_workspace_bytes": C.c_size_t, "icaf_loss_workspace_bytes": C.c_size_t,
                           "icaf_nms_multi_label_workspace_bytes": C.c_size_t,
                           "icaf_match_detections_workspace_bytes": C.c_size_t,
+                          "icaf_kaist_mr_workspace_bytes": C.c_size_t,
                           "icaf_conv2d_wgrad_workspace_bytes": C.c_size_t, "icaf_train_workspace_bytes": C.c_size_t,
                           "icaf_cross_attention_bwd_workspace_bytes": C.c_size_t,
                           "icaf_augment_params_bytes": C.c_size_t}.get(name, C.c_int)

@@ -683,6 +683,66 @@ def match_detections(det: torch.Tensor, count: torch.Tensor, targets: torch.Tens
     return correct, native
 
 
+KAIST_MAX_DET = 1000      # the reference's maxDets: beyond it its evaluateImg indexes past its IoU rows
+
+
+def kaist_mr(gt, rows: torch.Tensor, span: torch.Tensor, max_per_image: int, day_images: int = 1455, curves: bool = False,
+             workspace: Optional[torch.Tensor] = None):
+    """The nine KAIST miss-rate evaluations of evaluation_script.evaluate on the device (icaf_kaist_mr).  gt: the device
+    arrays of a :class:`~icafusion_b200.kaist_eval.KaistAnnotations` (attributes box, height, occlusion, ignore, id, offset).
+    rows: float64 (N, 5) detections x, y, w, h, score; span: int32 (images, 2) (offset, count) per image, counts at most
+    ``max_per_image`` (<= 1000).  Returns (ys float64 (9, 9), counts int32 (9, 3) [kept, tp, npig], curves float64
+    (9, 2, N) fppi / miss rate or None); no host sync."""
+    images = int(gt.offset.numel()) - 1
+    if not 0 <= int(max_per_image) <= KAIST_MAX_DET:
+        raise ValueError(f"kaist_mr: more than {KAIST_MAX_DET} detections in one image ({max_per_image}); the reference's "
+                         "evaluateImg fails there")
+    if rows.dim() != 2 or rows.shape[1] != 5 or rows.dtype != torch.float64 or not rows.is_contiguous() or not on_device(rows):
+        raise ValueError(f"kaist_mr: rows must be contiguous CUDA float64 (N, 5), got {rows.dtype} {tuple(rows.shape)}")
+    if tuple(span.shape) != (images, 2) or span.dtype != torch.int32 or not span.is_contiguous():
+        raise ValueError(f"kaist_mr: span must be contiguous int32 {(images, 2)}")
+    N, G = int(rows.shape[0]), int(gt.id.numel())
+    dev = rows.device
+    ys = torch.empty(9, 9, dtype=torch.float64, device=dev)
+    counts = torch.empty(9, 3, dtype=torch.int32, device=dev)
+    cv = torch.empty(9, 2, N, dtype=torch.float64, device=dev) if curves else None
+    need = 256 if _DRY is not None else int(_lib.lib().icaf_kaist_mr_workspace_bytes(images, G, N))
+    if need == 0:
+        raise _lib.IcafError(f"icaf_kaist_mr_workspace_bytes failed: {_lib.lib().icaf_last_error().decode()}")
+    if workspace is None or workspace.numel() < need + 256:
+        workspace = torch.empty(need + 256, dtype=torch.uint8, device=dev)
+    base = (-workspace.data_ptr()) % 256 if _DRY is None else 0     # the kernel wants a 256-byte aligned workspace
+    ws = workspace[base:base + need]
+    _call("icaf_kaist_mr", _lib.lib().icaf_kaist_mr,
+          (_ptr(gt.box), _ptr(gt.height), _ptr(gt.occlusion), _ptr(gt.ignore), _ptr(gt.id), _ptr(gt.offset), images, G,
+           int(day_images), _ptr(rows), _ptr(span), N, int(max_per_image), _ptr(ys), _ptr(counts), _ptr(cv), _ptr(ws),
+           C.c_size_t(need)),
+          {"bytes": float(N * 40 + G * 40)})
+    return ys, counts, cv
+
+
+def kaist_round_detections(native: torch.Tensor, det: torch.Tensor, count: torch.Tensor, image: torch.Tensor,
+                           rows: torch.Tensor, span: torch.Tensor):
+    """test.py's ``%g`` result lines of one batch, in memory (icaf_kaist_round_detections): for image b, p = image[b],
+    rows (images * max_det, 5) float64 at p * max_det + i get float('%g' % v) of the fp32 x1, y1, w, h, score, and
+    span[p] = (p * max_det, count[b]).  native: fp32 (B, max_det, 4); det / count: what :func:`nms` returns; image: int32
+    (B,) dataset indices on the device.  No host sync."""
+    B, max_det = int(det.shape[0]), int(det.shape[1])
+    images = int(span.shape[0])
+    if tuple(native.shape) != (B, max_det, 4) or native.dtype != torch.float32 or not native.is_contiguous():
+        raise ValueError(f"kaist_round_detections: native must be contiguous fp32 {(B, max_det, 4)}")
+    if det.dim() != 3 or det.shape[2] != 6 or det.dtype != torch.float32 or not det.is_contiguous():
+        raise ValueError("kaist_round_detections: det must be contiguous fp32 (B, max_det, 6)")
+    if tuple(count.shape) != (B,) or count.dtype != torch.int32 or tuple(image.shape) != (B,) or image.dtype != torch.int32:
+        raise ValueError("kaist_round_detections: count and image must be int32 (B,)")
+    if tuple(rows.shape) != (images * max_det, 5) or rows.dtype != torch.float64 or span.dtype != torch.int32 or \
+            span.dim() != 2 or span.shape[1] != 2:
+        raise ValueError(f"kaist_round_detections: rows must be float64 {(images * max_det, 5)} and span int32 (images, 2)")
+    _call("icaf_kaist_round_detections", _lib.lib().icaf_kaist_round_detections,
+          (_ptr(native), _ptr(det), _ptr(count), _ptr(image), B, max_det, images, _ptr(rows), _ptr(span)),
+          {"bytes": float(B * max_det * (16 + 4 + 40))})
+
+
 # ---------------------------------------------------------------------------------------------------------------
 # Training-step building blocks (operator level; see include/icaf_b200.h).  Gradients of Conv2d / Linear layers.
 def conv2d_wgrad(x: torch.Tensor, dy: torch.Tensor, kh: int, kw: int, stride: int, pad: int, scale: float = 1.0,

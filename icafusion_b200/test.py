@@ -8,8 +8,13 @@ batch, to gather the statistics in the order the reference appends them and to c
 
 Not built: the command-line path (``weights=`` without ``model=``: attempt_load and a loader made from ``opt``), the
 pycocotools JSON (``save_json`` / ``is_coco``), autolabelling (``save_hybrid``), augmented inference, plots and the
-confusion matrix (``plots=True`` logs a warning and draws nothing; it never changes the metrics), W&B media and the KAIST
-miss-rate evaluation, which the reference comments out (``MRresult`` is its ten zeros).
+confusion matrix (``plots=True`` logs a warning and draws nothing; it never changes the metrics) and W&B media.
+
+The KAIST miss rate, which the reference comments out (``MRresult`` is its ten zeros), runs on the device when
+``mr_annotations=`` names the annotation file (or a :class:`~icafusion_b200.kaist_eval.KaistAnnotations`): one rounding
+launch per batch turns the detections into the doubles the reference reads back from its ``result.txt`` (icaf_kaist_round_
+detections), and one icaf_kaist_mr after the last batch evaluates them.  ``MRresult`` is then [MR_all, ..., MR_heavy,
+recall_all] as the commented reference code computes them from evaluate() on that ``result.txt``.
 """
 from __future__ import annotations
 
@@ -78,9 +83,34 @@ def write_result_txt(labels_dir):
         f.writelines(lines)
 
 
-def summarise(stats, nc, names, seen, verbose=False):
+def mr_positions(kaist, labels_list, paths, seen):
+    """int32 (B,) annotation-image positions of a batch's images (image id = the label file's index in labels_list, as
+    test.py's result lines number them); each image may come once."""
+    pos = []
+    for p in paths:
+        i = labels_list.index(Path(p).stem + ".txt")
+        if i not in kaist.position:
+            raise ValueError(f"test: image {Path(p).name} (id {i}) is not in the KAIST annotations {kaist.path}")
+        if i in seen:
+            raise ValueError(f"test: image {Path(p).name} (id {i}) is validated twice; the miss rate takes each image once")
+        seen.add(i)
+        pos.append(kaist.position[i])
+    return torch.tensor(pos, dtype=torch.int32)
+
+
+def kaist_mr_result(ys, counts):
+    """MRresult of the reference's commented KAIST code: [MR_all, ..., MR_heavy, recall_all], recall_all 0.0 where `all`
+    keeps no detection (the reference's line raises there)."""
+    from .kaist_eval import SETUP_OF, log_average, recall_all
+    mrs = [float(log_average(ys[e])) for e in range(len(SETUP_OF))]
+    r = recall_all(ys, counts)
+    return mrs + [0.0 if r is None else r]
+
+
+def summarise(stats, nc, names, seen, verbose=False, mr_result=(0.0,) * 10):
     """test.py:287-312 on the gathered statistics [(correct bool (n, niou), conf fp32 (n), pcls fp32 (n), tcls list)] of the
-    images the reference appends.  Returns (tp, fp, fn, f1, mp, mr, map50, map, maps) as the reference computes them."""
+    images the reference appends.  Returns (tp, fp, fn, f1, mp, mr, map50, map, maps) as the reference computes them.
+    mr_result: the ten MRresult values the log line prints (x 100)."""
     p = r = f1 = mp = mr = map50 = map75 = 0.0
     mean_ap = 0
     tp, fp, fn = 0, 0, 0
@@ -103,7 +133,7 @@ def summarise(stats, nc, names, seen, verbose=False):
         logger.info(pf % ("all", seen, nt.sum(), tp, fp, fn, f1, mp, mr, map50, mean_ap))
     logger.info(("%20s" + "%11s" * 9) % ("MR-all", "MR-day", "MR-night", "MR-near", "MR-medium", "MR-far", "MR-none",
                                          "MR-partial", "MR-heavy", "Recall-all"))
-    logger.info(("%20.2f" + "%11.2f" * 9) % ((0.0,) * 10))
+    logger.info(("%20.2f" + "%11.2f" * 9) % tuple(v * 100 for v in mr_result))
     if verbose and nc > 1 and len(stats):
         for i, c in enumerate(ap_class):
             logger.info(pf % (names[c], seen, nt[c], p[i], r[i], ap50[i], ap75[i], ap[i]))
@@ -135,9 +165,11 @@ def test(data,
          half_precision=True,
          is_coco=False,
          opt=None,
-         labels_list=None):
+         labels_list=None,
+         mr_annotations=None):
     """reference: test.py:23-367, the path train.py takes (``model=`` an eval-mode CUDA Model, ``dataloader=`` batches of
-    (img uint8 (B, 6, H, W), targets (T, 6), paths, shapes)).  The model is not cast: it runs in the precision it has."""
+    (img uint8 (B, 6, H, W), targets (T, 6), paths, shapes)).  The model is not cast: it runs in the precision it has.
+    mr_annotations: a KAIST annotation file or KaistAnnotations; image i of labels_list is the file's image id i."""
     if model is None or dataloader is None:
         raise NotImplementedError("test: only the train.py path (model= and dataloader=) is built; the command-line path "
                                   "(weights=, attempt_load, a loader made from opt) is not")
@@ -150,8 +182,18 @@ def test(data,
     if plots:
         logger.warning("test: plots=True draws nothing here (no plots, no confusion matrix); the metrics are unaffected")
     device = next(model.parameters()).device
-    if device.type != "cuda":
+    if device.type != "cuda" and not (ops.dry_running() and device.type == "meta"):
         raise RuntimeError("icafusion_b200 runs on CUDA tensors only (no CPU fallback)")
+    kaist = None
+    if mr_annotations is not None:
+        from .kaist_eval import KaistAnnotations
+        if labels_list is None:
+            raise ValueError("test: mr_annotations= needs labels_list (a detection's image id is its label file's index)")
+        kaist = mr_annotations if isinstance(mr_annotations, KaistAnnotations) else KaistAnnotations(mr_annotations, device)
+        if kaist.device != device:
+            raise ValueError(f"test: mr_annotations are on {kaist.device}, the model on {device}")
+        mr_rows = mr_span = None
+        mr_seen = set()
     save_dir = Path(save_dir)
     (save_dir / "labels" if save_txt else save_dir).mkdir(parents=True, exist_ok=True)
     labels_dir = increment_path(save_dir / "labels" / "pred", exist_ok=False, mkdir=True) if save_txt else None
@@ -182,11 +224,24 @@ def test(data,
             det, count = ops.nms(z.contiguous(), conf_thres, iou_thres, agnostic=single_cls, multi_label=True)
             ev[3].record()
             ratio_pad = ratio_pad_rows(shapes).pin_memory().to(device, non_blocking=True)
-            native = torch.empty(nb, det.shape[1], 4, dtype=torch.float32, device=device) if save_txt else None
+            need_native = save_txt or kaist is not None
+            native = torch.empty(nb, det.shape[1], 4, dtype=torch.float32, device=device) if need_native else None
             correct, _ = ops.match_detections(det, count, targets_dev, ratio_pad, height, width, iouv, single_cls,
                                               native=native)
+            if kaist is not None:
+                if mr_rows is None:
+                    mr_rows = torch.empty(kaist.images * det.shape[1], 5, dtype=torch.float64, device=device)
+                    mr_span = torch.zeros(kaist.images, 2, dtype=torch.int32, device=device)
+                image = mr_positions(kaist, labels_list, paths, mr_seen)
+                ops.kaist_round_detections(native, det, count, image.pin_memory().to(device, non_blocking=True), mr_rows,
+                                           mr_span)
         timers.append(ev)
-        batches.append((det, count, correct, native, [Path(p) for p in paths], label_classes(targets, nb)))
+        batches.append((det, count, correct, native if save_txt else None, [Path(p) for p in paths],
+                        label_classes(targets, nb)))
+    mr_out = None
+    if kaist is not None and mr_rows is not None:
+        from .kaist_eval import DAY_IMAGES
+        mr_out = ops.kaist_mr(kaist, mr_rows, mr_span, int(mr_rows.shape[0] // kaist.images), DAY_IMAGES)
 
     torch.cuda.synchronize()
     t0 = sum(e[0].elapsed_time(e[1]) for e in timers) / 1e3
@@ -209,7 +264,9 @@ def test(data,
     if save_txt:
         write_result_txt(labels_dir)
 
-    results, maps = summarise(stats, nc, names, seen, verbose)
     mr_result = [0.0] * 10
+    if mr_out is not None:
+        mr_result = kaist_mr_result(mr_out[0].cpu().numpy(), mr_out[1].cpu().numpy())
+    results, maps = summarise(stats, nc, names, seen, verbose, mr_result)
     t = tuple(x / max(seen, 1) * 1e3 for x in (t0, t1, t0 + t1)) + (imgsz, imgsz, batch_size)
     return (*results, *(loss.cpu() / len(dataloader)).tolist()), maps, mr_result, t

@@ -261,6 +261,33 @@ int icaf_match_detections(const float* det, const int* count, int B, int max_det
                           const float* ratio_pad, int height, int width, const float* iouv, int niou, int single_cls,
                           unsigned char* correct, float* native, void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- KAIST log-average miss rate (evaluation_script/evaluation_script.py: evaluate) -------------------------------------
+ * The nine evaluations of evaluate() (all, day, night on setup 0 over all / the first day_images / the other images; near,
+ * medium, far, none, partial, heavy on setups 1-6 over all images) in one call: per (setup, image) the reference's greedy
+ * matching at IoU 0.5 (its quirks included: the score sort applied twice to the IoU rows, a match on annotation id 0 counts
+ * as a false positive), then one stable sort of all detections by descending score and one accumulation per evaluation.
+ * gts, in CSR per image (images in ascending id order; gt_offset: int (images + 1)), in annotation-file order within an
+ * image: gt_box float64 (gts, 4) x, y, w, h; gt_height float64 (gts); gt_occlusion, gt_ignore (the file's flag) int (gts);
+ * gt_id int64 (gts), the annotation ids.  Detections: dt_rows float64 (rows, 5) x, y, w, h, score; dt_span int (images, 2)
+ * (offset, count) per image, rows in file order, spans disjoint and in image order; every count <= max_per_image <= 1000.
+ * Out: ys float64 (9, 9), the recall at each fppi threshold (-1 where the reference leaves -1: no image with detections or
+ * no regular gt among them); counts int (9, 3): kept detections (the curve's length), their true positives, npig;
+ * curves (optional) float64 (9, 2, rows): fppi and 1 - recall over the kept detections.  No host synchronisation.
+ * workspace: icaf_kaist_mr_workspace_bytes(images, gts, rows) bytes, 256-byte aligned (0 = bad sizes, or no CUDA device
+ * to size the radix sort's storage on).
+ * ------------------------------------------------------------------------------------------- */
+size_t icaf_kaist_mr_workspace_bytes(int images, int gts, int rows);
+int icaf_kaist_mr(const double* gt_box, const double* gt_height, const int* gt_occlusion, const int* gt_ignore,
+                  const long long* gt_id, const int* gt_offset, int images, int gts, int day_images, const double* dt_rows,
+                  const int* dt_span, int rows, int max_per_image, double* ys, int* counts, double* curves, void* workspace,
+                  size_t workspace_bytes, void* stream);
+/* test.py's result lines in memory: for image b of a batch (B, max_det) and p = image[b] (its dataset index, < images),
+ * rows[p * max_det + i] = float64 of `%g` of the fp32 x1, y1, x2 - x1, y2 - y1 of native[b, i] and the score det[b, i, 4]
+ * (what float() reads back from the line), and span[p] = (p * max_det, count[b]): the dense layout of icaf_kaist_mr.  Exact
+ * for values 0 and 1e-7 <= |v| < 1e6. */
+int icaf_kaist_round_detections(const float* native, const float* det, const int* count, const int* image, int B, int max_det,
+                                int images, double* rows, int* span, void* stream);
+
 /* ---------------------------------------------------------------------------------------------
  * Detection loss, forward only (the validation loss test.py:132-133 accumulates; the training backward is not built):
  * utils/loss.py:325-463 ComputeLoss.__call__ + build_targets -- anchor-ratio matching with the four half-cell neighbour
