@@ -399,6 +399,7 @@ struct ConvPlan {
   int tiles, m_tiles, n_tiles;    // output tiles of the launch (icaf_conv_plan.work_items) = m_tiles * n_tiles * problems
   int sms;                        // SM count the plan was made for
   bool persist;                   // conv_gemm_persist_kernel: `ctas` CTAs walk the grid_x * grid_y * grid_z tiles
+  bool stem;                      // conv_stem_kernel: one tile per CTA, 16-channel 3x3 stride-1 gather launches at BN = 64
   bool xm;                        // LayerNorm-fold / row-statistics epilogue: the XM instantiation of either kernel
   int ctas;                       // CTAs the launch starts
 };

@@ -33,6 +33,9 @@
 // to fp32 summation order), and every other epilogue piece (conv_common.cuh):
 // register epilogue (fragment_row_bias, epi_tile_fragments, tma_store_tile, tma_load_tile), staged rows (staged_row,
 // epi_staged_chunk) and the mode selection (epi_mode_act).
+// conv_stem_kernel: the gather launches with 16 input channels, 3x3, stride 1, pad 1 and BN = 64 (the yolov5m/l image
+// stems over the space-to-depth frame): one 128-row tile per CTA as above, but its input pixels are gathered once into a
+// halo that feeds all nine taps, and only the nine k16 steps that carry data are issued (see its own comment below).
 #include <cstdlib>
 #include <cstring>
 
@@ -673,6 +676,159 @@ conv_gemm_persist_kernel(const ConvParams P, const __grid_constant__ ConvMaps ma
 }
 
 // ---------------------------------------------------------------------------------------------------
+// conv_stem_kernel: 16 input channels, 3x3, stride 1, pad 1, one 128 x 64 output tile per CTA (plan_conv sends the BN = 64
+// gather launches of that geometry here when TMA can store the output and there is no residual).  On the one-tile
+// kernel such a launch gathers A once per tap, so every input pixel crosses from L2 nine times, and pads K from 144 to
+// 192, so three of its twelve k16 steps multiply zeros.  Here one warpgroup does everything:
+//   filter : the packed filter's first three 64-column K blocks by TMA, 128B-swizzled as on the one-tile kernel (24 KB,
+//            one mbarrier); K columns 144-191 are loaded but never read;
+//   halo   : the tile's 128 consecutive output rows (b, y, x) fall into runs of one output row each -- at most two when
+//            Wo >= 128, up to StemLayout::runs(Wo) on narrow maps.  Run j (from output pixel (g0 + j, xs), len pixels)
+//            needs the input rows y - 1 ... y + 1, pixels xs - 1 ... xs + len, cp.async'd (zero-filled outside the map:
+//            the padding; and past M) into halo rows 3 j + ty of `pitch` pixels each, the same pitch for every run, so
+//            tile row (j, p) at tap (ty, tx) is halo pixel (3 j + ty) pitch + p + tx.  A pixel is 32 bytes (two 16-byte
+//            chunks); chunk c of halo pixel h sits at chunk c ^ ((h >> 2) & 1), so the eight rows of an ldmatrix phase
+//            (consecutive pixels) hit eight distinct bank groups;
+//   MMA    : per tap, the two 64-row blocks' A fragments by ldmatrix and two m64n64k16 wgmma RS: 18 MMAs, tap-major like
+//            the one-tile kernel's K order, so each accumulator sums the same nine products in the same order (the one-tile
+//            kernel's three padded steps add +0).  Fragments rotate through three register sets, two taps in flight;
+//   output : the halo becomes the output tile: epi_tile_fragments and a TMA store of the 2-D [M][N] box, as on the
+//            one-tile kernel's register epilogue.
+// Shared memory (51 KB at Wo >= 128) and registers (at most 128 per thread) let four CTAs share an SM, so one CTA's
+// filter load and gather overlap the others' MMAs, epilogues and stores.
+constexpr int kStemThreads = 128;
+struct StemLayout {
+  static constexpr int kFilterBytes = 3 * SmemLayout<64>::kBBytes;   // three 64 x 64 K filter boxes
+  static constexpr int kBiasOff = kFilterBytes;                // 64 fp32
+  static constexpr int kBarOff = kBiasOff + 64 * 4;
+  static constexpr int kHaloOff = kFilterBytes + 1024;         // 1024-byte aligned: the output tile (128B swizzle) reuses it
+  __host__ __device__ static int pitch(int Wo) { return (Wo < BM ? Wo : BM) + 2; }   // pixels per halo row
+  __host__ __device__ static int runs(int Wo) { return 1 + (BM - 1 + Wo - 1) / Wo; }  // most runs a tile can span
+  // [filter][bias, mbarrier][halo, or the output tile] ; + 1024 B alignment slack
+  static int total(int Wo) {
+    const int halo = runs(Wo) * 3 * pitch(Wo) * 32;
+    return kHaloOff + (halo > kOutHalfBytes ? halo : kOutHalfBytes) + 1024;
+  }
+};
+
+__global__ void __launch_bounds__(kStemThreads, 4)
+conv_stem_kernel(const ConvParams P, const __grid_constant__ ConvMaps maps) {
+  extern __shared__ uint8_t smem_raw[];
+  using SL = StemLayout;
+  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  uint8_t* smem_gen = smem_raw + (smem_base - smem_u32(smem_raw));
+  const uint32_t bar = smem_base + SL::kBarOff;
+  const uint32_t halo = smem_base + SL::kHaloOff;
+  float* sbias = reinterpret_cast<float*>(smem_gen + SL::kBiasOff);
+
+  pdl_launch_dependents();
+  const int t = threadIdx.x, w = t >> 5, l = t & 31;
+  const int bz = blockIdx.z, n0 = blockIdx.y * 64;
+  const ConvProblem pr = pick_problem(P, bz);
+  const TileOrigin o{int(blockIdx.x) * BM, 0, 0, 0};
+  // the tile's runs: the first from output pixel (g0, ox0) of the (b, y) row index g0, the others from x = 0
+  const int g0 = o.m0 / P.Wo, ox0 = o.m0 - g0 * P.Wo;
+  const int len0 = min(P.Wo - ox0, BM);
+  const int nruns = 1 + (BM - len0 + P.Wo - 1) / P.Wo;
+  const int pitch = SL::pitch(P.Wo);
+  // halo pixel at tap (0, 0) of the tile row this lane addresses in ldmatrix, for the 64-row blocks 0 and 1 (matrix l / 8
+  // of an x4 covers rows 8 ((l / 8) % 2) ... of the warp's 16, chunk l / 16 of the tap's 16 channels)
+  int lane_hp[2];
+#pragma unroll
+  for (int hm = 0; hm < 2; ++hm) {
+    const int r = 64 * hm + 16 * w + (l & 7) + 8 * ((l >> 3) & 1);
+    int j = 0, p = r;
+    if (r >= len0) {
+      const int q = (r - len0) / P.Wo;
+      j = 1 + q;
+      p = r - len0 - q * P.Wo;
+    }
+    lane_hp[hm] = 3 * j * pitch + p;
+  }
+  if (t == 0) {
+    mbar_init(bar, 1);
+    fence_mbar_init();
+  }
+  if (t == 32) {
+    tma_prefetch_desc(bz ? &maps.w[1] : &maps.w[0]);
+    tma_prefetch_desc(bz ? &maps.y[1] : &maps.y[0]);
+  }
+  __syncthreads();
+  pdl_wait();   // prologue (barrier, descriptor prefetch, lane addresses) overlapped the previous kernel
+
+  if (t == 0) {
+    // K blocks 0-2 of the packed filter (K = tap * 16 + channel), output channels n0 ... n0 + 63
+    const CUtensorMap* mw = bz ? &maps.w[1] : &maps.w[0];
+    mbar_arrive_expect_tx(bar, SL::kFilterBytes);
+#pragma unroll 1
+    for (int kb = 0; kb < 3; ++kb) tma_load_2d(smem_base + uint32_t(kb * SmemLayout<64>::kBBytes), mw, bar, kb * BK, n0);
+  }
+  if (t < 64) sbias[t] = (pr.bias && !(P.epi & ICAF_EPI_BIAS_ROW) && n0 + t < P.N) ? __ldg(pr.bias + n0 + t) : 0.f;
+  float rb[4] = {0.f, 0.f, 0.f, 0.f};
+  fragment_row_bias(rb, P, pr, o, w, l);
+
+  // ---- halo: thread t copies chunk t % 2 of pixels t / 2, t / 2 + 64, ... of every halo row
+  const int c = t & 1;
+#pragma unroll 1
+  for (int j = 0; j < nruns; ++j) {
+    const int g = g0 + j;
+    const int xs = j ? 0 : ox0;
+    const int len = j ? min(P.Wo, BM - len0 - (j - 1) * P.Wo) : len0;
+    const int b = g / P.Ho, oy = g - b * P.Ho;
+    const bool gv = g < P.B * P.Ho;
+#pragma unroll
+    for (int ty = 0; ty < 3; ++ty) {
+      const int iy = oy + ty - 1;
+      const bool rv = gv && (unsigned)iy < (unsigned)P.Hi;
+      const __half* src = pr.x + (rv ? (size_t(b) * P.Hi + iy) * P.Wi * pr.x_ld : 0) + 8 * c;
+      const int h0 = (3 * j + ty) * pitch;
+      for (int px = t >> 1; px < len + 2; px += kStemThreads / 2) {
+        const int ix = xs - 1 + px, h = h0 + px;
+        const bool ok = rv && (unsigned)ix < (unsigned)P.Wi;
+        cp_async16(halo + uint32_t(h) * 32u + (uint32_t(c ^ ((h >> 2) & 1)) << 4), ok ? src + size_t(ix) * pr.x_ld : pr.x, ok);
+      }
+    }
+  }
+  cp_async_commit();
+  cp_async_wait<0>();
+  __syncthreads();                                            // halo and bias complete
+  mbar_wait_quiet(bar, 0);                                    // filter landed
+
+  // ---- nine taps x two 64-row blocks of m64n64k16 wgmma RS
+  float acc0[32], acc1[32];
+#pragma unroll
+  for (int i = 0; i < 32; ++i) { acc0[i] = 0.f; acc1[i] = 0.f; }
+  uint32_t fa[3][2][4];
+#pragma unroll
+  for (int tap = 0; tap < 9; ++tap) {
+    const int f = tap % 3;                                    // free once the group of tap - 3 has retired
+    const int off = (tap / 3) * pitch + tap % 3;
+#pragma unroll
+    for (int hm = 0; hm < 2; ++hm) {
+      const int h = lane_hp[hm] + off;
+      ldmatrix_x4(fa[f][hm], halo + uint32_t(h) * 32u + (uint32_t((l >> 4) ^ ((h >> 2) & 1)) << 4));
+    }
+    wgmma_fence();
+    const uint64_t bd = gmma_desc_sw128(smem_base + uint32_t((tap >> 2) * SmemLayout<64>::kBBytes + 32 * (tap & 3)));
+    wgmma_rs<0>(acc0, fa[f][0], bd, tap != 0);
+    wgmma_rs<0>(acc1, fa[f][1], bd, tap != 0);
+    wgmma_commit();
+    wgmma_wait<2>();
+  }
+  wgmma_wait<0>();
+  __syncthreads();                                            // every warp's fragments are in: the halo is free
+
+  // ---- epilogue on the accumulators into the output tile (where the halo was), TMA store
+  epi_tile_fragments<32>(epi_mode_act<false>(P, false), acc0, acc1, halo, sbias, rb, 0.f, 1.f, w, l);
+  fence_proxy_async_smem();                                   // the tile is visible to the TMA unit ...
+  __syncthreads();                                            // ... once every thread has written its part
+  if (t == 0) {
+    tma_store_tile<64>(P, bz ? &maps.y[1] : &maps.y[0], halo, n0, o);
+    bulk_wait_group<0>();                                     // complete before the grid is (PDL dependents read it)
+  }
+}
+
+// ---------------------------------------------------------------------------------------------------
 // CUDA-core reference with the identical contract (tests only).
 struct SimtParams { ConvParams P; const __half* w[2]; };
 __global__ void conv_gemm_simt_kernel(const SimtParams S) {
@@ -892,13 +1048,16 @@ static int launch_conv(const ConvParams& P, const ConvPlan& pl, const __half* co
                        cudaStream_t st) {
   void (*kernel)(ConvParams, ConvMaps) = pl.xm ? conv_gemm_tc_kernel<BN, true> : conv_gemm_tc_kernel<BN, false>;
   if (pl.persist) kernel = pl.xm ? conv_gemm_persist_kernel<true> : conv_gemm_persist_kernel<false>;
-  static bool configured[2][2][kMaxDevices] = {};
-  if (int rc = configure_smem(kernel, 227 * 1024, configured[pl.persist][pl.xm], "conv2d: cudaFuncSetAttribute")) return rc;
+  if (pl.stem) kernel = conv_stem_kernel;
+  static bool configured[3][2][kMaxDevices] = {};
+  const int family = pl.stem ? 2 : (pl.persist ? 1 : 0);
+  if (int rc = configure_smem(kernel, 227 * 1024, configured[family][pl.xm], "conv2d: cudaFuncSetAttribute")) return rc;
   ConvMaps maps;
   if (int rc = encode_maps<BN>(P, w, g, n_io, P.tma_epi != 0, maps)) return rc;
-  // the one-tile kernel takes the tile grid (split-K: in clusters along x); the persistent one `ctas` CTAs
+  // the one-tile kernels take the tile grid (split-K: in clusters along x); the persistent one `ctas` CTAs
   const dim3 grid = pl.persist ? dim3(unsigned(pl.ctas)) : dim3(pl.grid_x, pl.grid_y, pl.grid_z);
-  return launch_kc("conv2d_fwd", kernel, grid, dim3(pl.persist ? kPersistThreads : kThreads), (size_t)pl.smem, st, pl.cluster, P, maps);
+  const int threads = pl.persist ? kPersistThreads : (pl.stem ? kStemThreads : kThreads);
+  return launch_kc("conv2d_fwd", kernel, grid, dim3(threads), (size_t)pl.smem, st, pl.cluster, P, maps);
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -926,7 +1085,17 @@ static int plan_conv(const icaf_conv_geom* g, int n_io, int sms, bool tma_out, C
       // the persistent kernel stores its non-XM tiles by TMA; a launch whose outputs TMA cannot write stays one-tile
       if (!rc && (pl.xm || tma_out) && P.a_mode != A_GATHER && P.splits == 1 && pl.tiles > sms) rc = plan_persist(P, pl);
       break;
-    case 64: rc = plan_tc<64>(P, n_io, pl); break;
+    case 64:
+      rc = plan_tc<64>(P, n_io, pl);
+      // 16-channel stride-1 3x3 gather launches (the yolov5m/l image stems) run on conv_stem_kernel, whose epilogue is
+      // the register one with a TMA store and has no residual
+      if (!rc && !pl.xm && tma_out && P.a_mode == A_GATHER && P.splits == 1 && P.Cin == 16 && P.kh == 3 && P.kw == 3 &&
+          P.stride == 1 && P.pad == 1 && !(P.epi & (ICAF_EPI_ADD_RES | ICAF_EPI_SCALED_RES))) {
+        P.stages = 1;                                   // one filter load and one halo per tile, no ring
+        pl.stem = true;
+        pl.smem = StemLayout::total(P.Wo);
+      }
+      break;
     default: rc = plan_tc<32>(P, n_io, pl); break;
   }
   if (rc) return rc;
