@@ -1,6 +1,9 @@
 // Detection loss, forward (utils/loss.py:325-463 ComputeLoss.__call__ + build_targets): target assignment, CIoU box loss,
 // objectness BCE against IoU-valued targets, class BCE -- three launches, no host round trip, deterministic (no floating
 // point atomics: objectness targets meet in an integer atomicMax, every sum is reduced in a fixed order).
+// Both BCE terms are optionally wrapped in the focal loss of utils/loss.py:37-64 (hyp fl_gamma > 0, loss.py:341-344): the
+// candidate and objectness kernels, forward and backward, take it as a template argument, so the plain BCE path compiles to
+// the code it has without it.
 //   1. loss_candidates_kernel: one thread per (level, target, anchor, offset) candidate of build_targets (:405-463):
 //      anchor-ratio match, the four half-cell neighbour offsets, grid cell, CIoU of the decoded prediction against the
 //      target box (general.py:410-447), its (1 - iou) and class-BCE terms, objectness target into tobj by atomicMax
@@ -35,6 +38,7 @@ struct LossParams {
   float* cand_box; float* cand_cls; int* cand_valid;     // [nl][nt][na][5]
   float* obj_part;                      // [nl][kLossObjBlocks]
   float* out;                           // 5 floats
+  float fl_gamma;                       // focal-loss gamma (only read by the kFocal instantiations)
 };
 
 __device__ __forceinline__ float loss_ld(const void* p, int fp32, long long i) {
@@ -45,6 +49,36 @@ __device__ __forceinline__ float sigmoid_f(float v) { return 1.f / (1.f + expf(-
 __device__ __forceinline__ float bce_logits(float x, float y, float pw) {
   const float lw = 1.f + (pw - 1.f) * y;
   return (1.f - y) * x + lw * (log1pf(expf(-fabsf(x))) + fmaxf(-x, 0.f));
+}
+
+// FocalLoss(BCEWithLogitsLoss, gamma, alpha = 0.25), utils/loss.py:37-64, per element:
+//   bce(x, y) * (y a + (1 - y)(1 - a)) * (1 - p_t)^gamma,   p_t = y sigmoid(x) + (1 - y)(1 - sigmoid(x)).
+constexpr float kFocalAlpha = 0.25f;
+template <bool kFocal>
+__device__ __forceinline__ float bce_elem(float x, float y, float pw, float gamma) {
+  float l = bce_logits(x, y, pw);
+  if constexpr (kFocal) {
+    const float s = sigmoid_f(x);
+    const float pt = y * s + (1.f - y) * (1.f - s);
+    l *= (y * kFocalAlpha + (1.f - y) * (1.f - kFocalAlpha)) * powf(1.f - pt, gamma);
+  }
+  return l;
+}
+// d bce_elem / dx.  Plain: (1 - y) - (1 + (pw - 1) y)(1 - sigmoid(x)).  Focal: the product rule over the three factors, with
+// d(1 - p_t)/dx = (1 - 2y) s (1 - s) -- the derivative autograd takes through the reference's FocalLoss.forward.
+template <bool kFocal>
+__device__ __forceinline__ float bce_elem_grad(float x, float y, float pw, float gamma) {
+  const float lw = 1.f + (pw - 1.f) * y;
+  if constexpr (!kFocal) {
+    return (1.f - y) - lw * (1.f - sigmoid_f(x));
+  } else {
+    const float s = sigmoid_f(x);
+    const float q = 1.f - (y * s + (1.f - y) * (1.f - s));
+    const float af = y * kFocalAlpha + (1.f - y) * (1.f - kFocalAlpha);
+    const float dbce = (1.f - y) - lw * (1.f - s);
+    const float dq = (1.f - 2.f * y) * s * (1.f - s);
+    return af * (dbce * powf(q, gamma) + bce_logits(x, y, pw) * gamma * powf(q, gamma - 1.f) * dq);
+  }
 }
 
 // Forward-mode value with the four partial derivatives w.r.t. the raw box logits: the backward pass evaluates the very same
@@ -136,6 +170,7 @@ __device__ __forceinline__ bool cand_setup(const LossParams& P, long long idx, C
   return true;
 }
 
+template <bool kFocal>
 __global__ void loss_candidates_kernel(const LossParams P) {
   pdl_launch_dependents();
   pdl_wait();
@@ -157,7 +192,7 @@ __global__ void loss_candidates_kernel(const LossParams P) {
   float lc = 0.f;
   if (P.no - 5 > 1) {                                                               // :380-383
     for (int j = 0; j < P.no - 5; ++j)
-      lc += bce_logits(loss_ld(pl, P.p_fp32, pb + 5 + j), (j == K.c) ? P.cp : P.cn, P.cls_pw);
+      lc += bce_elem<kFocal>(loss_ld(pl, P.p_fp32, pb + 5 + j), (j == K.c) ? P.cp : P.cn, P.cls_pw, P.fl_gamma);
   }
   P.cand_cls[idx] = lc;
   P.cand_valid[idx] = 1;
@@ -167,6 +202,7 @@ __global__ void loss_candidates_kernel(const LossParams P) {
 
 // Backward, 1 of 2: box and class gradients of every matched candidate, accumulated in fp32 per (cell, channel) -- several
 // candidates can meet in one cell.  (fp32 atomics: the sum order is not fixed; the result is rounded to the dtype of p.)
+template <bool kFocal>
 __global__ void loss_candidates_bwd_kernel(const LossParams P) {
   pdl_launch_dependents();
   pdl_wait();
@@ -194,13 +230,13 @@ __global__ void loss_candidates_bwd_kernel(const LossParams P) {
     const float kc = g * P.cls / (float(n) * float(P.no - 5));
     for (int j = 0; j < P.no - 5; ++j) {
       const float x = loss_ld(pl, P.p_fp32, K.pb + 5 + j), y = (j == K.c) ? P.cp : P.cn;
-      const float lw = 1.f + (P.cls_pw - 1.f) * y;
-      atomicAdd(acc + 5 + j, kc * ((1.f - y) - lw * (1.f - sigmoid_f(x))));
+      atomicAdd(acc + 5 + j, kc * bce_elem_grad<kFocal>(x, y, P.cls_pw, P.fl_gamma));
     }
   }
 }
 
 // Backward, 2 of 2: objectness gradient of every cell, plus the accumulated candidate gradients, written as dp.
+template <bool kFocal>
 __global__ void __launch_bounds__(256) loss_obj_bwd_kernel(const LossParams P) {
   pdl_launch_dependents();
   pdl_wait();
@@ -216,16 +252,16 @@ __global__ void __launch_bounds__(256) loss_obj_bwd_kernel(const LossParams P) {
     const long long pb = cell_offset(P, lvl, b, a, gj, gi);
     const float* acc = P.dacc + (P.cell_off[lvl] + c) * P.no;
     const float x = loss_ld(P.p[lvl], P.p_fp32, pb + 4), y = P.tobj[P.cell_off[lvl] + c];
-    const float lw = 1.f + (P.obj_pw - 1.f) * y;
     for (int j = 0; j < P.no; ++j) {
       float v = acc[j];
-      if (j == 4) v += g * ((1.f - y) - lw * (1.f - sigmoid_f(x)));
+      if (j == 4) v += g * bce_elem_grad<kFocal>(x, y, P.obj_pw, P.fl_gamma);
       if (P.p_fp32) reinterpret_cast<float*>(P.dp[lvl])[pb + j] = v;
       else reinterpret_cast<__half*>(P.dp[lvl])[pb + j] = __float2half(v);
     }
   }
 }
 
+template <bool kFocal>
 __global__ void __launch_bounds__(256) loss_obj_kernel(const LossParams P) {
   pdl_launch_dependents();
   pdl_wait();
@@ -245,7 +281,7 @@ __global__ void __launch_bounds__(256) loss_obj_kernel(const LossParams P) {
       const int gj = int(t % ny); t /= ny;
       pb = cell_offset(P, lvl, int(t / P.na), int(t % P.na), gj, gi);
     }
-    s += bce_logits(loss_ld(P.p[lvl], P.p_fp32, pb + 4), tobj[c], P.obj_pw);
+    s += bce_elem<kFocal>(loss_ld(P.p[lvl], P.p_fp32, pb + 4), tobj[c], P.obj_pw, P.fl_gamma);
   }
   red[threadIdx.x] = s;
   __syncthreads();
@@ -319,7 +355,6 @@ static int loss_setup(const char* what, const void* const* p, int p_fp32, int p_
   if (nl < 1 || nl > kLossMaxLevels || B < 1 || na < 1 || na > 8 || no < 6 || nt < 0 || (nt > 0 && !targets))
     return set_error(ICAF_ERR_BAD_ARG, "compute_loss: bad shape (nl <= 5, na <= 8)");
   if (p_ld != 0 && p_ld < na * no) return set_error(ICAF_ERR_BAD_ARG, "compute_loss: p_ld is 0 ((B,na,ny,nx,no) contiguous) or the pixel pitch of the (B,ny,nx,na*no) head map");
-  if (hyp->fl_gamma > 0.f) return set_error(ICAF_ERR_UNSUPPORTED, "compute_loss: focal loss (fl_gamma > 0) is not built");
   if (workspace_bytes < icaf_loss_workspace_bytes(B, na, nt, ny, nx, nl, bwd ? no : 0) || (reinterpret_cast<uintptr_t>(workspace) & 255))
     return set_error(ICAF_ERR_BAD_ARG, "compute_loss: workspace too small (icaf_loss_workspace_bytes) or not 256-byte aligned");
   (void)what;
@@ -335,6 +370,7 @@ static int loss_setup(const char* what, const void* const* p, int p_fp32, int p_
   P.p_fp32 = p_fp32; P.nhwc = p_ld; P.nl = nl; P.B = B; P.na = na; P.no = no; P.nt = nt;
   P.box = hyp->box; P.obj = hyp->obj; P.cls = hyp->cls; P.cls_pw = hyp->cls_pw; P.obj_pw = hyp->obj_pw;
   P.anchor_t = hyp->anchor_t; P.gr = hyp->gr; P.cp = hyp->cp; P.cn = hyp->cn;
+  P.fl_gamma = hyp->fl_gamma;                                                        // <= 0: plain BCE (loss.py:342 `if g > 0`)
   P.targets = targets;
   cand = (size_t)nl * (nt > 0 ? nt : 1) * na * 5;
   char* w = (char*)workspace;
@@ -357,15 +393,18 @@ extern "C" int icaf_compute_loss_fwd(const void* const* p, int p_fp32, int p_ld,
   if (int rc = loss_setup("compute_loss", p, p_fp32, p_ld, ny, nx, nl, B, na, no, targets, nt, anchors_host, hyp, workspace, workspace_bytes, false, P, cells, cand))
     return rc;
   P.out = out;
+  const bool focal = P.fl_gamma > 0.f;
   cudaStream_t st = (cudaStream_t)stream;
   cudaError_t e = cudaMemsetAsync(P.tobj, 0, cells * 4, st);                        // tobj = zeros_like(pi[..., 0])   :351
   if (e == cudaSuccess) e = cudaMemsetAsync(P.cand_valid, 0, cand * 4, st);
   if (e != cudaSuccess) return set_cuda_error(e, "compute_loss: cudaMemsetAsync");
   if (nt > 0) {
     const long long total = (long long)nl * nt * na * 5;
-    if (int rc = launch_k("compute_loss(candidates)", loss_candidates_kernel, dim3(blocks_for(total, 128)), dim3(128), 0, st, P)) return rc;
+    if (int rc = launch_k("compute_loss(candidates)", focal ? loss_candidates_kernel<true> : loss_candidates_kernel<false>,
+                          dim3(blocks_for(total, 128)), dim3(128), 0, st, P)) return rc;
   }
-  if (int rc = launch_k("compute_loss(objectness)", loss_obj_kernel, dim3(kLossObjBlocks, nl), dim3(256), 0, st, P)) return rc;
+  if (int rc = launch_k("compute_loss(objectness)", focal ? loss_obj_kernel<true> : loss_obj_kernel<false>, dim3(kLossObjBlocks, nl),
+                        dim3(256), 0, st, P)) return rc;
   return launch_k("compute_loss(finalize)", loss_finalize_kernel, dim3(1), dim3(256), 0, st, P);
 }
 
@@ -382,12 +421,15 @@ extern "C" int icaf_compute_loss_bwd(const void* const* p, int p_fp32, int p_ld,
     P.dp[i] = dp[i];
   }
   P.gout = grad_out;
+  const bool focal = P.fl_gamma > 0.f;
   cudaStream_t st = (cudaStream_t)stream;
   cudaError_t e = cudaMemsetAsync(P.dacc, 0, cells * no * 4, st);
   if (e != cudaSuccess) return set_cuda_error(e, "compute_loss_bwd: cudaMemsetAsync");
   if (nt > 0) {
     const long long total = (long long)nl * nt * na * 5;
-    if (int rc = launch_k("compute_loss_bwd(candidates)", loss_candidates_bwd_kernel, dim3(blocks_for(total, 128)), dim3(128), 0, st, P)) return rc;
+    if (int rc = launch_k("compute_loss_bwd(candidates)", focal ? loss_candidates_bwd_kernel<true> : loss_candidates_bwd_kernel<false>,
+                          dim3(blocks_for(total, 128)), dim3(128), 0, st, P)) return rc;
   }
-  return launch_k("compute_loss_bwd(objectness)", loss_obj_bwd_kernel, dim3(kLossObjBlocks, nl), dim3(256), 0, st, P);
+  return launch_k("compute_loss_bwd(objectness)", focal ? loss_obj_bwd_kernel<true> : loss_obj_bwd_kernel<false>,
+                  dim3(kLossObjBlocks, nl), dim3(256), 0, st, P);
 }

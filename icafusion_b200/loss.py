@@ -4,6 +4,7 @@
 the use test.py:132-133 (validation loss) and train.py:338-344 (training loss + backward) make of it: when a prediction
 requires grad the returned loss carries an autograd node whose backward launches icaf_compute_loss_bwd.  Target assignment,
 CIoU, both BCE terms, the reductions and their gradients run as kernels of libicaf_b200 (csrc/loss.cu) with no host sync.
+``hyp['fl_gamma'] > 0`` wraps both BCE terms in the reference's FocalLoss (alpha 0.25, loss.py:37-64, 341-344) on the device.
 """
 from __future__ import annotations
 
@@ -26,8 +27,6 @@ class ComputeLoss:
             raise NotImplementedError("ComputeLoss: autobalance needs a host read per level and step; not built")
         m = model.module if hasattr(model, "module") else model
         h = m.hyp                                            # train.py:229 attaches the hyper-parameter dict to the model
-        if h.get("fl_gamma", 0.0) > 0:
-            raise NotImplementedError("ComputeLoss: focal loss (fl_gamma > 0) is not built")
         det = m.model[-1]
         self.na, self.nc, self.nl = det.na, det.nc, det.nl
         self.anchors = det.anchors.detach().float().cpu().reshape(-1).tolist()      # grid units, (nl, na, 2)

@@ -1,4 +1,5 @@
-"""The training step of train.py:117-349 around the icafusion_b200 model: optimiser groups, DDP wrap, GradScaler, one step.
+"""The training step of train.py:117-352 around the icafusion_b200 model: optimiser groups, DDP wrap, GradScaler, one step,
+and gradient accumulation over train.py's nominal batch of 64.
 
 This is the caller side of the hot path (SURVEY.md section 8e): what the reference's ``train_rgb_ir`` does between building
 the model and ``ema.update`` -- minus data loading, logging, checkpoints and evaluation.  The model's forward and backward are
@@ -17,6 +18,7 @@ from __future__ import annotations
 
 from typing import Dict, List, Optional
 
+import numpy as np
 import torch
 import torch.nn as nn
 
@@ -100,23 +102,39 @@ class ModelEMA:
 
 
 class TrainStep:
-    """model -> (optional DDP) -> loss -> scaled backward -> optimiser step, per call (train.py:334-349).
+    """model -> (optional DDP) -> loss -> scaled backward -> optimiser step, per call (train.py:334-352).
+
+    Gradient accumulation (train.py:123-125, 314-320, 346-352): the reference steps the optimiser once per nominal batch of
+    64 images, every ``accumulate`` batches.  ``__call__(..., optimizer_step=False)`` runs forward, loss and the scaled
+    backward and leaves the gradients in ``.grad`` for the next call to add to; a train.py-shaped loop reads
+
+        step(rgb, ir, targets, optimizer_step=(ni % step.accumulate_at(ni, nw) == 0))
+
+    and calls ``step.zero_grad()`` at the start of each epoch (train.py:291).  Under DDP every backward all-reduces, as in the
+    reference (no ``no_sync``): the bucket views accumulate the per-micro-batch averages.
+
+    adam (train.py --adam): ``optim.Adam(pg0, lr=lr0, betas=(momentum, 0.999))`` instead of nesterov SGD, same three groups.
 
     sync_bn (train.py --sync-bn): with world_size > 1, every BatchNorm2d is converted to nn.SyncBatchNorm after the optimiser
     groups are built and before the DDP wrap (train.py:195-198), so BatchNorm normalises over the batch of all ranks.  At
     world size 1 the model is left as it is.  A model the caller converted beforehand trains synchronised as well."""
 
     def __init__(self, model: nn.Module, hyp: Optional[Dict[str, float]] = None, total_batch_size: int = 64, world_size: int = 1,
-                 local_rank: Optional[int] = None, imgsz: int = 640, amp_scale: bool = True, ema: bool = False, sync_bn: bool = False):
+                 local_rank: Optional[int] = None, imgsz: int = 640, amp_scale: bool = True, ema: bool = False, sync_bn: bool = False,
+                 adam: bool = False):
         hyp = dict(HYP_SCRATCH if hyp is None else hyp)
         det = model.model[-1]
         nl, nc = det.nl, det.nc
         nbs = 64
         accumulate = max(round(nbs / total_batch_size), 1)
         hyp["weight_decay"] *= total_batch_size * accumulate / nbs                    # train.py:121
+        self.nbs, self.total_batch_size, self.accumulate = nbs, total_batch_size, accumulate
         self.dead = freeze_dead_parameters(model)
         pg0, pg1, pg2 = param_groups(model)
-        self.optimizer = torch.optim.SGD(pg0, lr=hyp["lr0"], momentum=hyp["momentum"], nesterov=True)      # train.py:136
+        if adam:
+            self.optimizer = torch.optim.Adam(pg0, lr=hyp["lr0"], betas=(hyp["momentum"], 0.999))            # train.py:133-134
+        else:
+            self.optimizer = torch.optim.SGD(pg0, lr=hyp["lr0"], momentum=hyp["momentum"], nesterov=True)  # train.py:136
         self.optimizer.add_param_group({"params": pg1, "weight_decay": hyp["weight_decay"]})
         self.optimizer.add_param_group({"params": pg2})
         hyp["box"] *= 3.0 / nl                                                        # train.py:238-240
@@ -138,19 +156,28 @@ class TrainStep:
         self.hyp = hyp
         self.ema = ModelEMA(self.raw_model) if ema else None                          # train.py:154 (rank 0 / single GPU in the reference)
 
-    def __call__(self, rgb: torch.Tensor, ir: torch.Tensor, targets: torch.Tensor):
+    def accumulate_at(self, ni: int, nw: int) -> int:
+        """Batches per optimiser step at integrated batch ``ni`` with ``nw`` warm-up batches: train.py:317's ramp from 1 to
+        64 / total_batch_size during warm-up, ``accumulate`` (train.py:124) after it."""
+        if ni <= nw:
+            return int(max(1, np.interp(ni, [0, nw], [1, self.nbs / self.total_batch_size]).round()))
+        return self.accumulate
+
+    def __call__(self, rgb: torch.Tensor, ir: torch.Tensor, targets: torch.Tensor, optimizer_step: bool = True):
         """rgb / ir: (B,3,H,W) uint8 (scaled by 1/255 inside the stem staging, train.py:297-298) or float images on the device;
-        targets (nt, 6).  Returns (loss, loss_items) of this rank."""
+        targets (nt, 6).  optimizer_step=False: only add this batch's scaled gradients to ``.grad`` (train.py:346 with
+        ``ni % accumulate != 0``).  Returns (loss, loss_items) of this rank."""
         pred = self.model(rgb, ir)                                                    # train.py:336
         loss, items = self.compute_loss(pred, targets)                                # train.py:337
         if self.world_size > 1:
             loss = loss * self.world_size                                             # train.py:339
         self.scaler.scale(loss).backward()                                            # train.py:344
-        self.scaler.step(self.optimizer)                                              # train.py:348-350
-        self.scaler.update()
-        self.zero_grad()
-        if self.ema is not None:
-            self.ema.update(self.raw_model)                                           # train.py:351-352
+        if optimizer_step:
+            self.scaler.step(self.optimizer)                                          # train.py:347-350
+            self.scaler.update()
+            self.zero_grad()
+            if self.ema is not None:
+                self.ema.update(self.raw_model)                                       # train.py:351-352
         return loss.detach(), items
 
     def zero_grad(self) -> None:
@@ -166,6 +193,12 @@ class GraphedTrainStep:
     build_targets rejects).  The optimiser step and GradScaler.update stay eager (train.py:348-350; GradScaler reads its
     inf flag on the host).  Dropout masks: the kernels add a device-side step counter to their seeds (icaf_set_seed_offset),
     incremented inside the graph, so every replay draws new masks.
+
+    Gradient accumulation: the graph above (the "fresh" one) writes the gradients into the static ``.grad`` tensors.  The
+    first call with ``optimizer_step=False`` captures a second, "accumulating" graph on the same inputs and memory pool while
+    ``.grad`` is defined, so autograd adds into those tensors in place.  The fresh graph serves the first micro-batch after
+    construction, an optimiser step or ``zero_grad()``; the accumulating one every other micro-batch.  A run that steps on
+    every call never captures it.
 
     DDP (world_size > 1): construct the TrainStep inside ``torch.cuda.stream(side)`` and set TORCH_NCCL_ASYNC_ERROR_HANDLING=0
     before init_process_group, as torch's CUDA-graph notes require; 11 eager iterations run before the capture."""
@@ -202,24 +235,32 @@ class GraphedTrainStep:
         with torch.no_grad():
             for k, v in ts.raw_model.state_dict().items():
                 v.copy_(saved[k])                        # in place: the graph will be captured on these very tensors
-            for st in ts.optimizer.state.values():
-                if st.get("momentum_buffer") is not None:
-                    st["momentum_buffer"].zero_()        # == the state before the first step (SGD seeds the buffer with the gradient)
+            for st in ts.optimizer.state.values():   # == the state before the first step: SGD seeds its momentum buffer with
+                for v in st.values():                # the gradient; Adam starts from step 0 and zero moments
+                    if torch.is_tensor(v):
+                        v.zero_()
         if saved_scaler:
             ts.scaler.load_state_dict(saved_scaler)
         self.seed_ctr.zero_()
         ts.zero_grad()
         self.graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(self.graph):
+        self.loss, self.items = self._capture(self.graph)
+        self.acc_graph = None                            # the accumulating graph, captured on first use
+        self.fresh = True                                # the next replay starts a new accumulation window
+
+    def _capture(self, graph, pool=None):
+        ts = self.ts
+        with torch.cuda.graph(graph, pool=pool):
             self.seed_ctr += 1
             pred = ts.model(self.rgb, self.ir)
-            loss, self.items = ts.compute_loss(pred, self.tg)
+            loss, items = ts.compute_loss(pred, self.tg)
             if ts.world_size > 1:
                 loss = loss * ts.world_size
-            self.loss = loss
             ts.scaler.scale(loss).backward()
+        return loss, items
 
-    def __call__(self, rgb: torch.Tensor, ir: torch.Tensor, targets: torch.Tensor):
+    def __call__(self, rgb: torch.Tensor, ir: torch.Tensor, targets: torch.Tensor, optimizer_step: bool = True):
+        """As TrainStep.__call__; optimizer_step=False adds this batch's gradients to the static ``.grad`` tensors."""
         nt = int(targets.shape[0])
         if nt > self.max_targets:
             raise ValueError(f"GraphedTrainStep: {nt} label rows, captured for at most {self.max_targets}")
@@ -228,12 +269,27 @@ class GraphedTrainStep:
         self.tg[:nt].copy_(targets, non_blocking=True)
         if nt < self.max_targets:
             self.tg[nt:, 0] = -1.0
-        self.graph.replay()
-        self.ts.scaler.step(self.ts.optimizer)            # gradients live in static buffers the next replay overwrites
-        self.ts.scaler.update()
-        if self.ts.ema is not None:
-            self.ts.ema.update(self.ts.raw_model)
-        return self.loss.detach(), self.items
+        if self.fresh:
+            self.graph.replay()
+            loss, items = self.loss, self.items
+        else:
+            if self.acc_graph is None:                   # .grad holds this window's gradients: the capture adds into them
+                self.acc_graph = torch.cuda.CUDAGraph()
+                self.acc_loss, self.acc_items = self._capture(self.acc_graph, pool=self.graph.pool())
+            self.acc_graph.replay()
+            loss, items = self.acc_loss, self.acc_items
+        self.fresh = optimizer_step
+        if optimizer_step:
+            self.ts.scaler.step(self.ts.optimizer)        # gradients live in static buffers the next fresh replay overwrites
+            self.ts.scaler.update()
+            if self.ts.ema is not None:
+                self.ts.ema.update(self.ts.raw_model)
+        return loss.detach(), items
+
+    def zero_grad(self) -> None:
+        """Start a new accumulation window (train.py:291): the next call replays the fresh graph, which overwrites ``.grad``.
+        The gradient tensors stay allocated, because both graphs write them in place."""
+        self.fresh = True
 
     def close(self) -> None:
         _lib.lib().icaf_set_seed_offset(None)

@@ -294,14 +294,15 @@ int icaf_kaist_round_detections(const float* native, const float* det, const int
  * offsets, CIoU box loss, objectness BCE against IoU-valued targets (largest IoU wins a contested cell), class BCE.
  * p: nl device pointers to the Detect training outputs (B, na, ny[i], nx[i], no), fp16 (p_fp32 = 0) or fp32 (1); arithmetic
  * in fp32.  targets: device fp32 (nt, 6) rows [image, class, x, y, w, h] normalised to [0, 1].  anchors_host: nl*na*2 floats
- * in grid units (Detect.anchors).  out: 5 device floats [loss * batch, lbox, lobj, lcls, 0].  fl_gamma must be 0.
+ * in grid units (Detect.anchors).  out: 5 device floats [loss * batch, lbox, lobj, lcls, 0].  fl_gamma > 0 wraps both BCE
+ * terms in FocalLoss(gamma, alpha = 0.25) (loss.py:37-64, 341-344), in the forward and the backward; <= 0 keeps plain BCE.
  * Deterministic: no floating-point atomics.  workspace: icaf_loss_workspace_bytes(...) bytes, 256-byte aligned.
  * ------------------------------------------------------------------------------------------- */
 typedef struct {
   float box, obj, cls;   /* loss gains hyp['box'], hyp['obj'], hyp['cls'] (already scaled as train.py:226-228 does) */
   float cls_pw, obj_pw;  /* BCE positive weights                                                                   */
   float anchor_t;        /* anchor-multiple threshold                                                              */
-  float fl_gamma;        /* focal-loss gamma; only 0 is supported                                                  */
+  float fl_gamma;        /* focal-loss gamma; > 0 turns the focal loss on for the class and objectness BCE         */
   float gr;              /* model.gr: objectness target = (1 - gr) + gr * iou                                      */
   float cp, cn;          /* smoothed positive / negative class targets (smooth_BCE, loss.py:15-17)                 */
   float balance[5];      /* per-level objectness weights: {4, 1, 0.4} for three levels (loss.py:346)               */
