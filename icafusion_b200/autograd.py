@@ -418,8 +418,8 @@ def _layernorm(ln: nn.LayerNorm, x):
     return LayerNormFn.apply(x, ln.weight, ln.bias, ln.eps)
 
 
-# Head dims icaf_cross_attention_bwd is built for.  The forward runs every multiple of 8 up to 128, so a model can run in
-# eval() with a head dim (yolov5m: 24 / 48 / 96) that it cannot train with.
+# Head dims icaf_cross_attention_bwd is built for.  The forward runs every multiple of 8 up to 128, and 160, so a model can
+# run in eval() with a head dim (yolov5m: 24 / 48 / 96, yolov5x: 40 / 80 / 160) that it cannot train with.
 ATTN_BWD_HEAD_DIMS = (8, 16, 32, 64, 128)
 
 

@@ -35,10 +35,11 @@ struct AttnParams {
 
 // ---------------------------------------------------------------------------------------------------
 // 288 threads: warps 0-7 two consumer warpgroups (queries 0-63 / 64-127 of the tile), warp 8 TMA producer.
-// A head dim d (any multiple of 8 up to 128) runs the kernel of width D = 16 / 32 / 64 / 128, the smallest >= d.  Every
-// tile comes through a 3-D map that gives each head its own extent of d columns:
-//   Q / K tiles: (d, k*heads, B*Npad) view of the projection matrix (k = 2 split, 3 fused), box (min(D,64), 1, rows)
-//                -> K-major rows of 32 / 64 / 128 bytes with the matching swizzle (D = 128: two 64-column blocks)
+// A head dim d (any multiple of 8 up to 128) runs the kernel of width D = 16 / 32 / 64 / 128, the smallest >= d; d = 160
+// runs its own width D = 160.  Every tile comes through a 3-D map that gives each head its own extent of d columns:
+//   Q / K tiles: (d, k*heads, B*Npad) view of the projection matrix (k = 2 split, 3 fused), box (W, 1, rows) with
+//                W = min(D, 64), or 32 at D = 160 -> K-major rows of 32 / 64 / 128 bytes with the matching swizzle, D / W
+//                column blocks (D = 128: two 64-column blocks; D = 160: five 32-column blocks, 64-byte rows)
 //   V tiles    : (VF, fused [q|k|v] rows) boxes like K's at projection 2 -> rows = keys, i.e. an MN-major B operand
 //   V^T tiles  : (B*Npad, d, heads) view of the (C, B*Npad) matrix, box (64, D, 1) -> K-major SW128 (keys are the K dim
 //                of PV)
@@ -46,23 +47,28 @@ struct AttnParams {
 // masked in the softmax.  The zero columns add exactly 0 to S = Q K^T and produce zero columns of O = P V, which are not
 // stored.
 struct AttnMaps {
-  CUtensorMap qk[2];   // [0] = vis, [1] = ir : box (min(D,64), 1, 128) -- Q tiles
-  CUtensorMap kv[2];   // same views, box (min(D,64), 1, KV) -- K tiles (and V tiles in the fused form)
+  CUtensorMap qk[2];   // [0] = vis, [1] = ir : box (W, 1, 128) -- Q tiles
+  CUtensorMap kv[2];   // same views, box (W, 1, KV) -- K tiles (and V tiles in the fused form)
   CUtensorMap vt[2];   // split form: V^T view, box (64, D, 1)
 };
 
 // KV = keys per tile (N of S, K of PV).  Head dims up to 32 run 64-key tiles (less masked work at the DMFF token counts).
 // The dropout kernel at D = 128 spills 48 bytes with 128-key tiles; 64-key tiles would change the rounding of yolov5l's
-// P5 training attention (d = 128).
+// P5 training attention (d = 128).  D = 160 runs 64-key tiles: with 128 its 80 accumulator registers, S and P spill
+// 256 bytes under the 168-register cap of 288 threads.
 template <int D>
 struct AttnCfg {
-  static constexpr int kKV = D <= 32 ? 64 : 128;
+  static constexpr int kKV = D <= 32 || D == 160 ? 64 : 128;
 };
 
 template <int D, int KV>
 struct AttnSmemT {
-  static constexpr int kKB = (D + 63) / 64;                 // 64-wide column blocks of the head dim
-  static constexpr int kRowB = D >= 64 ? 128 : D * 2;       // bytes per staged Q / K row (= swizzle span)
+  // head-dim columns per TMA box and staged row: 160 = 5 x 32 keeps one swizzle mode (64 B) across the whole head, so
+  // P V runs as one N = 160 wgmma on a uniform MN-major V tile
+  static constexpr int kBoxW = D % 64 == 0 ? 64 : (D >= 32 ? 32 : D);
+  static constexpr int kKB = D / kBoxW;                     // column blocks of the head dim
+  static constexpr int kRowB = kBoxW * 2;                   // bytes per staged Q / K row (= swizzle span)
+  static constexpr int kKS = kRowB / 32;                    // k16 steps per column block
   static constexpr int kQBytes = kKB * kQT * kRowB;
   static constexpr int kKBytes = kKB * KV * kRowB;          // per buffer
   static constexpr int kVBytes = (KV / 64) * D * 128;       // per buffer: 64-key blocks of D rows (= KV rows of D halfs)
@@ -71,6 +77,7 @@ struct AttnSmemT {
   static constexpr int kVOff = kKOff + 2 * kKBytes;
   static constexpr int kBarOff = kVOff + 2 * kVBytes;
   static constexpr int kTotal = kBarOff + 128 + 1024;       // + alignment slack
+  static_assert(D % kBoxW == 0 && kBoxW % 16 == 0, "the head dim must split into whole column blocks of k16 steps");
   static_assert(kQBytes % 1024 == 0 && kKBytes % 1024 == 0 && kVBytes % 1024 == 0, "tiles must keep 1024-byte alignment");
 };
 
@@ -78,6 +85,14 @@ __device__ __forceinline__ float fast_exp2_t(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
+}
+
+// Barrier waits of the width-D kernel.  D = 160 waits without the deadlock report (mbar_wait_quiet): a printf reachable
+// anywhere in a kernel makes ptxas serialise all of its wgmmas (warning C7510).  The other widths keep the reporting wait.
+template <int D>
+__device__ __forceinline__ void attn_wait(uint32_t bar, uint32_t parity) {
+  if constexpr (D == 160) mbar_wait_quiet(bar, parity);
+  else mbar_wait(bar, parity);
 }
 
 // TRAIN: dropout on the attention probabilities (the row sum still runs over the un-dropped values, like
@@ -126,18 +141,19 @@ __global__ void __launch_bounds__(288, 1) cross_attn_tma_kernel(const AttnParams
     float o[D / 2];
 #pragma unroll
     for (int i = 0; i < D / 2; ++i) o[i] = 0.f;
-    mbar_wait(q_full, 0);
+    attn_wait<D>(q_full, 0);
     for (int j = 0; j < nkv; ++j) {
       const int buf = j & 1;
       const int kv0 = j * kKV;
-      mbar_wait(kv_full(buf), (j >> 1) & 1);
+      attn_wait<D>(kv_full(buf), (j >> 1) & 1);
       // ---- S = Q K^T (64 x KV per warpgroup) ----
       float s[kKV / 2];
       wgmma_fence();
 #pragma unroll
       for (int k = 0; k < D / 16; ++k) {
-        const uint64_t ad = gmma_desc_kmajor(sbase + L::kQOff + (k >> 2) * (kQT * 128) + 64 * g * L::kRowB + (k & 3) * 32, L::kRowB);
-        const uint64_t bd = gmma_desc_kmajor(sbase + L::kKOff + buf * L::kKBytes + (k >> 2) * (kKV * 128) + (k & 3) * 32, L::kRowB);
+        const int kb = k / L::kKS, ko = (k % L::kKS) * 32;    // column block, byte offset of the k16 step in its rows
+        const uint64_t ad = gmma_desc_kmajor(sbase + L::kQOff + kb * (kQT * L::kRowB) + 64 * g * L::kRowB + ko, L::kRowB);
+        const uint64_t bd = gmma_desc_kmajor(sbase + L::kKOff + buf * L::kKBytes + kb * (kKV * L::kRowB) + ko, L::kRowB);
         wgmma_ss<0, 0>(s, ad, bd, k != 0);
       }
       wgmma_commit();
@@ -188,7 +204,7 @@ __global__ void __launch_bounds__(288, 1) cross_attn_tma_kernel(const AttnParams
 #pragma unroll
       for (int k = 0; k < kKV / 16; ++k) {
         if (VF) {
-          wgmma_rs<1>(o, pa[k], gmma_desc_mnmajor(sbase + L::kVOff + buf * L::kVBytes + k * 16 * L::kRowB, L::kRowB, kKV * 128), true);
+          wgmma_rs<1>(o, pa[k], gmma_desc_mnmajor(sbase + L::kVOff + buf * L::kVBytes + k * 16 * L::kRowB, L::kRowB, kKV * L::kRowB), true);
         } else {
           wgmma_rs<0>(o, pa[k], gmma_desc_sw128(sbase + L::kVOff + buf * L::kVBytes + (k >> 2) * (D * 128) + (k & 3) * 32), true);
         }
@@ -224,23 +240,23 @@ __global__ void __launch_bounds__(288, 1) cross_attn_tma_kernel(const AttnParams
     const int row_b = b * n_pad;
     // a tile = (column block kb of projection k's head `head`, rows r0 ..)
     auto load_tile = [&](uint32_t dst, const CUtensorMap* m, uint32_t bar, int k, int kb, int r0) {
-      tma_load_3d(dst, m, bar, kb * 64, k * P.heads + head, r0);
+      tma_load_3d(dst, m, bar, kb * L::kBoxW, k * P.heads + head, r0);
     };
     mbar_arrive_expect_tx(q_full, L::kQBytes);      // overhanging boxes count in full: the zero fill arrives as bytes too
 #pragma unroll
     for (int kb = 0; kb < L::kKB; ++kb)
-      load_tile(sbase + L::kQOff + kb * (kQT * 128), mq, q_full, 0, kb, row_b + q0);
+      load_tile(sbase + L::kQOff + kb * (kQT * L::kRowB), mq, q_full, 0, kb, row_b + q0);
     for (int j = 0; j < nkv; ++j) {
       const int buf = j & 1;
-      if (j >= 2) mbar_wait(kv_empty(buf), ((j >> 1) & 1) ^ 1);     // PV(j-2) has drained this buffer
+      if (j >= 2) attn_wait<D>(kv_empty(buf), ((j >> 1) & 1) ^ 1);     // PV(j-2) has drained this buffer
       mbar_arrive_expect_tx(kv_full(buf), L::kKBytes + L::kVBytes);
 #pragma unroll
       for (int kb = 0; kb < L::kKB; ++kb)
-        load_tile(sbase + L::kKOff + buf * L::kKBytes + kb * (kKV * 128), mk, kv_full(buf), 1, kb, row_b + j * kKV);
+        load_tile(sbase + L::kKOff + buf * L::kKBytes + kb * (kKV * L::kRowB), mk, kv_full(buf), 1, kb, row_b + j * kKV);
       if (VF) {
 #pragma unroll
         for (int kb = 0; kb < L::kKB; ++kb)
-          load_tile(sbase + L::kVOff + buf * L::kVBytes + kb * (kKV * 128), mk, kv_full(buf), 2, kb, row_b + j * kKV);
+          load_tile(sbase + L::kVOff + buf * L::kVBytes + kb * (kKV * L::kRowB), mk, kv_full(buf), 2, kb, row_b + j * kKV);
       } else {
 #pragma unroll
         for (int kb = 0; kb < kKV / 64; ++kb)
@@ -296,13 +312,16 @@ __global__ void cross_attn_simt_kernel(const AttnParams P) {
   for (int i = 0; i < d; ++i) o[i] = __float2half_rn(acc[i] / l);
 }
 
+// d160: the caller has a kernel for head dim 160 (the tensor-core forward; not the CUDA-core or dropout kernels)
 static int fill_attn(const void* qk_vis, const void* qk_ir, const void* vt_vis, const void* vt_ir, void* out_vis,
-                     void* out_ir, int B, int N, int n_pad, int C, int heads, AttnParams& P) {
+                     void* out_ir, int B, int N, int n_pad, int C, int heads, AttnParams& P, bool d160 = false) {
   // vt_* both NULL: the fused form, qk_* are (B, Npad, 3C) [q | k | v] matrices
   if (!qk_vis || !qk_ir || (!vt_vis != !vt_ir) || !out_vis || !out_ir) return set_error(ICAF_ERR_BAD_ARG, "cross_attention: null pointer");
   if (B < 1 || N < 1 || n_pad < N || n_pad % 8 || heads < 1 || C % heads) return set_error(ICAF_ERR_BAD_ARG, "cross_attention: bad shape");
   int d = C / heads;
-  if (d % 8 || d < 8 || d > 128) return set_error(ICAF_ERR_UNSUPPORTED, "cross_attention: head dim must be a multiple of 8 in [8, 128]");
+  if (d % 8 || d < 8 || (d > 128 && !(d160 && d == 160)))
+    return set_error(ICAF_ERR_UNSUPPORTED, d160 ? "cross_attention: head dim must be a multiple of 8 in [8, 128], or 160"
+                                                : "cross_attention: head dim must be a multiple of 8 in [8, 128]");
   P.qk[0] = (const __half*)qk_vis; P.qk[1] = (const __half*)qk_ir;
   P.vt[0] = (const __half*)vt_vis; P.vt[1] = (const __half*)vt_ir;
   P.out[0] = (__half*)out_vis; P.out[1] = (__half*)out_ir;
@@ -323,7 +342,7 @@ static int launch_attn_tma(const AttnParams& P, cudaStream_t st) {
   memset(&maps, 0, sizeof(maps));
   const uint64_t rows = uint64_t(P.B) * P.n_pad;
   const uint64_t d = uint64_t(P.d);
-  const uint32_t bw = D < 64 ? D : 64;
+  const uint32_t bw = L::kBoxW;
   const uint64_t dims[3] = {d, uint64_t(P.ld / d), rows};       // (head column, projection * heads + head, token)
   const uint64_t vdims[3] = {rows, d, uint64_t(P.heads)};       // (token, head row, head)
   for (int i = 0; i < 2; ++i) {
@@ -336,14 +355,20 @@ static int launch_attn_tma(const AttnParams& P, cudaStream_t st) {
   return launch_k("cross_attention", cross_attn_tma_kernel<D, VF, TRAIN>, dim3(grid), dim3(288), L::kTotal, st, P, maps);
 }
 
-// A head dim d runs the kernel of the smallest width D >= d; columns d .. D-1 are zero-filled (see AttnMaps).
+// A head dim d up to 128 runs the kernel of the smallest width D >= d; columns d .. D-1 are zero-filled (see AttnMaps).
+// d = 160 (yolov5x's P5 block) runs at its exact width: padded to 256 it would cost 60 % more MMA work and a 128-register
+// accumulator.  It has no dropout instantiation: the training entry point refuses it (there is no backward either).
 template <bool VF, bool TRAIN = false>
 static int dispatch_attn(const AttnParams& P, cudaStream_t st) {
   const int d = P.d;
   if (d <= 16) return launch_attn_tma<16, VF, TRAIN>(P, st);
   if (d <= 32) return launch_attn_tma<32, VF, TRAIN>(P, st);
   if (d <= 64) return launch_attn_tma<64, VF, TRAIN>(P, st);
-  return launch_attn_tma<128, VF, TRAIN>(P, st);
+  if (d <= 128) return launch_attn_tma<128, VF, TRAIN>(P, st);
+  if constexpr (!TRAIN) {
+    if (d == 160) return launch_attn_tma<160, VF>(P, st);
+  }
+  return set_error(ICAF_ERR_UNSUPPORTED, "cross_attention: no kernel for this head dim");
 }
 
 }  // namespace icaf
@@ -353,7 +378,7 @@ using namespace icaf;
 extern "C" int icaf_cross_attention(const void* qk_vis, const void* qk_ir, const void* vt_vis, const void* vt_ir,
                                     void* out_vis, void* out_ir, int B, int N, int n_pad, int C, int heads, void* stream) {
   AttnParams P;
-  int rc = fill_attn(qk_vis, qk_ir, vt_vis, vt_ir, out_vis, out_ir, B, N, n_pad, C, heads, P);
+  int rc = fill_attn(qk_vis, qk_ir, vt_vis, vt_ir, out_vis, out_ir, B, N, n_pad, C, heads, P, true);
   if (rc) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   if ((uint64_t(B) * n_pad * 2) % 16 || (reinterpret_cast<uintptr_t>(vt_vis) & 15) || (reinterpret_cast<uintptr_t>(qk_vis) & 15) ||

@@ -198,11 +198,12 @@ int icaf_row_stats(const void* x0, const void* x1, float* stats0, float* stats1,
  *   fused  (vt_vis == vt_ir == NULL): qk_* are fp16 (B, Npad, 3C) rows [q | k | v] exactly as ONE fused projection GEMM
  *          emits them; the V tiles feed the tensor core as MN-major operands, no transpose anywhere;
  *   split  : qk_* fp16 (B, Npad, 2C) rows [q | k], vt_* fp16 (C, B*Npad) value projection stored transposed.
- * out_*: fp16 (B, Npad, C) heads merged (the layout out_proj consumes).  Every tile is staged by TMA. */
+ * out_*: fp16 (B, Npad, C) heads merged (the layout out_proj consumes).  Every tile is staged by TMA.
+ * Head dim C / heads: a multiple of 8 in [8, 128], or 160; others return ICAF_ERR_UNSUPPORTED. */
 int icaf_cross_attention(const void* qk_vis, const void* qk_ir, const void* vt_vis, const void* vt_ir, void* out_vis,
                          void* out_ir, int B, int N, int n_pad, int C, int heads, void* stream);
 
-/* Test-only CUDA-core reference of icaf_cross_attention (same contract). */
+/* Test-only CUDA-core reference of icaf_cross_attention (same contract, head dims up to 128 only). */
 int icaf_cross_attention_simt(const void* qk_vis, const void* qk_ir, const void* vt_vis, const void* vt_ir,
                               void* out_vis, void* out_ir, int B, int N, int n_pad, int C, int heads, void* stream);
 
@@ -421,7 +422,7 @@ int icaf_set_seed_offset(const void* device_u32);
 
 /* Training-mode forward of the fused form: like icaf_cross_attention(qkv_vis, qkv_ir, NULL, NULL, ...) plus dropout with
  * probability p_drop on the attention probabilities (common.py:677,680; counter-based mask keyed by `seed`, reproduced by the
- * backward below). */
+ * backward below).  Head dims up to 128 only: 160 has no dropout kernel and no backward. */
 int icaf_cross_attention_train(const void* qkv_vis, const void* qkv_ir, void* out_vis, void* out_ir, int B, int N, int n_pad, int C, int heads,
                                float p_drop, uint32_t seed, void* stream);
 

@@ -1,15 +1,15 @@
-"""Forward step times of the four detector sizes, and the cross-attention launch time per DMFF head dim.
+"""Forward step times of the five detector sizes, and the cross-attention launch time per DMFF head dim.
 
-For yolov5{n,s,m,l}_Transfusion_FLIR at batch 1 and 16, 512 x 640 RGB+IR (seeded synthetic weights, BN folded, fp16), the way
+For yolov5{n,s,m,l,x}_Transfusion_FLIR at batch 1 and 16, 512 x 640 RGB+IR (seeded synthetic weights, BN folded, fp16), the way
 bench.py builds its detector:
   - step: CUDA-graph replay of the forward (GraphedDetector), device-resident uint8 inputs, one CUDA event pair per step, the
     L2 flushed (256 MiB memset) between steps; the median and the spread over the timed steps are printed.
   - attention: eager forwards on one stream with a CUDA event after every library launch (ops.profile), each pass queued
     behind a spin kernel and after an L2 flush; every icaf_cross_attention launch keeps its fastest pass.  Head dims:
-    n 8/16/32, s 16/32/64, m 24/48/96, l 32/64/128 (DMFF C / 8 heads at P3 / P4 / P5).
+    n 8/16/32, s 16/32/64, m 24/48/96, l 32/64/128, x 40/80/160 (DMFF C / 8 heads at P3 / P4 / P5).
 The card name, power limit and the SM clocks nvidia-smi reports during the timed steps are printed with the numbers.
 
-    python scripts/model_size_times.py [--sizes n,s,m,l] [--batches 1,16] [--steps 50] [--warmup 10] [--passes 5]
+    python scripts/model_size_times.py [--sizes n,s,m,l,x] [--batches 1,16] [--steps 50] [--warmup 10] [--passes 5]
 """
 from __future__ import annotations
 
@@ -92,7 +92,7 @@ def measure(size, B, steps, warmup, passes, dev, flush):
 
 def main():
     ap = argparse.ArgumentParser(description=__doc__.split("\n\n")[0])
-    ap.add_argument("--sizes", default="n,s,m,l")
+    ap.add_argument("--sizes", default="n,s,m,l,x")
     ap.add_argument("--batches", default="1,16")
     ap.add_argument("--steps", type=int, default=50)
     ap.add_argument("--warmup", type=int, default=10)
