@@ -1,0 +1,74 @@
+"""The launch census without a GPU: every entry point the detectors issue is either replayed or listed with a reason, the
+census spans every conv plan family, and each replay builder re-issues exactly the launch it replays (tests/census.py)."""
+import collections
+
+import pytest
+
+import census
+
+
+@pytest.fixture(scope="module")
+def walks():
+    return {c.id: census.walk_config(c) for c in census.CONFIGS}
+
+
+@pytest.fixture(scope="module")
+def records(walks):
+    """Unique records over all configurations, {key: record}."""
+    out = {}
+    for recs in walks.values():
+        for k, r in census.unique(recs).items():
+            out.setdefault(k, r)
+    return out
+
+
+def test_configurations():
+    ids = [c.id for c in census.CONFIGS]
+    assert len(ids) == len(set(ids)) == 5 * 2 * 2 + 3 * 2
+    assert "yolov5x-kaist-512x640-b16-infer" in ids and "yolov5l-kaist-512x640-b16-train" in ids
+
+
+def test_every_entry_point_is_accounted_for(walks):
+    """A C-ABI call a detector issues is replayed or listed with a reason, and neither map names a call no walk issues."""
+    assert not set(census.REPLAYED) & set(census.NOT_REPLAYED)
+    issued = {name for recs in walks.values() for name, _, _ in recs}
+    accounted = set(census.REPLAYED) | set(census.NOT_REPLAYED)
+    assert issued - accounted == set(), f"entry points the census neither replays nor excuses: {sorted(issued - accounted)}"
+    # all_reduce is issued only when SyncBatchNorm runs under a process group
+    assert accounted - issued <= {"all_reduce"}, f"entry points no walk issues: {sorted(accounted - issued)}"
+
+
+def test_census_covers_every_conv_plan_family(records):
+    from icafusion_b200 import _lib
+    convs = [r for k, r in records.items() if k[0] == "icaf_conv2d_fwd"]
+    wgrads = [r for k, r in records.items() if k[0] == "icaf_conv2d_wgrad"]
+    slices = [r for r in convs if any(io.x_ld > r[1][0]._obj.Cin or io.y_ld > r[1][0]._obj.Cout for io in r[1][1])]
+    bns, modes, kinds, splits = collections.Counter(), collections.Counter(), collections.Counter(), collections.Counter()
+    for _, args, _ in convs:
+        pl = census.conv_plan(args[0]._obj, args[2], 132)
+        assert pl is not None and pl.kernel == _lib.KERNEL_TC, census.describe((None, args, None))
+        bns[pl.bn] += 1
+        modes[pl.a_mode] += 1
+        kinds["persistent" if pl.ctas < pl.grid_x * pl.grid_y * pl.grid_z else "one-tile"] += 1
+        splits[pl.splits] += 1
+    print(f"\n{len(convs)} conv, {len(wgrads)} wgrad, {len(slices)} slice launches; bn {dict(bns)} a_mode {dict(modes)} {dict(kinds)} "
+          f"splits {dict(sorted(splits.items()))}")
+    assert len(convs) >= 1400 and len(wgrads) >= 225 and len(slices) >= 400
+    assert {32, 64, 128} <= set(bns) and {0, 1, 2} <= set(modes) and {"persistent", "one-tile"} <= set(kinds)
+    assert {2, 3, 4, 5, 6, 8} <= set(splits)
+
+
+def test_builders_reissue_the_recorded_launch(records):
+    """Each builder, run on meta tensors under a dry run, issues a call with the same key as the record it replays: the replay
+    hits the product's geometry, channel pitches, epilogue flags and scales."""
+    from icafusion_b200 import ops
+    done = collections.Counter()
+    for k, rec in records.items():
+        if k[0] not in census.REPLAYED:
+            continue
+        with ops.dry_run() as dr:
+            assert census.replay(rec, "meta") == []
+        issued = {census.key(r) for r in dr.records}
+        assert k in issued, f"{census.describe(rec)}: the replay issued {sorted(issued, key=str)[:4]}"
+        done[k[0]] += 1
+    assert set(done) == set(census.REPLAYED)
