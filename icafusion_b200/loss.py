@@ -77,7 +77,7 @@ class ComputeLoss:
         if nl != self.nl:
             raise ValueError(f"ComputeLoss: {nl} prediction levels, Detect has {self.nl}")
         dev = p[0].device
-        if dev.type != "cuda":
+        if not ops.on_device(p[0]):
             raise RuntimeError("icafusion_b200 runs on CUDA tensors only (no CPU fallback)")
         dt = p[0].dtype
         if dt not in (torch.float16, torch.float32) or any(t.dtype != dt for t in p):

@@ -19,6 +19,7 @@ import zlib
 from dataclasses import dataclass
 from typing import Callable, List, Union
 
+import numpy as np
 import torch
 import torch.nn.functional as F
 
@@ -42,12 +43,23 @@ class Config:
 
 
 CONFIGS = [Config("infer", s, ds, B, H, W) for s in "nsmlx" for ds, H, W in (("kaist", 512, 640), ("FLIR", 320, 320)) for B in (1, 16)] + \
-          [Config("train", s, "kaist", B, 512, 640) for s in "nsl" for B in (2, 16)]
+          [Config("train", s, "kaist", B, 512, 640) for s in "nsl" for B in (2, 16)] + \
+          [Config("infer", s, "FLIR", B, 512, 640) for s in "nsmlx" for B in (1, 16)] + \
+          [Config("infer", s, ds, B, 544, 672) for s in "nsmlx" for ds in ("kaist", "FLIR") for B in (1, 32)] + \
+          [Config("train", s, "kaist", B, 640, 640) for s in "nsl" for B in (8, 16, 3)] + \
+          [Config("train", "s", "FLIR", 8, 640, 640)]
+# Inference: detect.py letterboxes the 512x640 frames of both datasets to 512x640; test.py's rectangular batches
+# (rect=True, pad=0.5) make them 544x672, at test.py's batch 32 and train.py's validation batch 1.  Training: train.py's mosaic
+# batches are img_size x img_size = 640x640 at its default batch 8, at 16 and with a ragged last batch of 3.
 # Training of yolov5m / yolov5x is not built: the attention backward has no head dim 24 / 48 / 96 / 160.
+
+TARGETS_PER_IMAGE = 16      # a mosaic stitches four frames of a few pedestrians each
 
 
 def walk(kind: str, cfg: str, B: int, H: int, W: int):
-    """Records [(entry point, ctypes args, work)] of one dry-run walk of model `cfg` (e.g. 'yolov5s_Transfusion_kaist')."""
+    """Records [(entry point, ctypes args, work)] of one dry-run walk of model `cfg` (e.g. 'yolov5s_Transfusion_kaist').
+    A training walk is TrainStep's: forward, ComputeLoss with train.py's hyper-parameters as TrainStep scales them, and the
+    backward from the loss."""
     from icafusion_b200 import Model
     rgb = torch.empty(B, 3, H, W, dtype=torch.uint8, device="meta")
     if kind == "infer":
@@ -55,10 +67,14 @@ def walk(kind: str, cfg: str, B: int, H: int, W: int):
         with torch.no_grad(), ops.dry_run() as dr:
             m(rgb, rgb)
     elif kind == "train":
-        m = Model(cfg).to("meta").train()
+        from icafusion_b200.trainer import TrainStep
+        m = Model(cfg).train()
+        step = TrainStep(m, imgsz=max(H, W), amp_scale=False)       # ComputeLoss reads the anchors before the move to meta
+        m.to("meta")
+        targets = torch.empty(TARGETS_PER_IMAGE * B, 6, device="meta")
         with ops.dry_run() as dr:
-            pred = m(rgb, rgb)
-            torch.autograd.backward(pred, [torch.empty_like(p) for p in pred])
+            loss, _ = step.compute_loss(m(rgb, rgb), targets)
+            loss.backward()
     else:
         raise ValueError(kind)
     return dr.records
@@ -72,13 +88,19 @@ def walk_config(c: Config):
 # ---------------------------------------------------------------------------------------------------------------
 # Dedupe key
 # Arguments that are not geometry: the dropout probability and mask seed of the training attention.  The census replays
-# those launches at p = 0 (a plain reference cannot reproduce a counter-based mask), so they are left out of the key.
-_NOT_KEYED = {"icaf_cross_attention_train": (9, 10), "icaf_cross_attention_bwd": (13, 14)}
+# those launches at p = 0 (a plain reference cannot reproduce a counter-based mask), so they are left out of the key.  The
+# mask seed of the element-wise dropout is drawn per call: keying it would make two walks of one configuration differ.
+_NOT_KEYED = {"icaf_cross_attention_train": (9, 10), "icaf_cross_attention_bwd": (13, 14), "icaf_eltwise": (6,)}
+
+
+def _value(v):
+    """A struct field as a plain value: nested arrays (LossHyp.balance) as tuples, which compare by content."""
+    return tuple(v) if isinstance(v, C.Array) else v
 
 
 def _fields(s):
-    """The non-pointer fields of a ConvIO / BottleneckIO: channel pitches, ln_parts, ln_eps."""
-    return tuple(getattr(s, f) for f, t in s._fields_ if t is not C.c_void_p)
+    """The non-pointer fields of a struct: ConvGeom; ConvIO / BottleneckIO channel pitches, ln_parts, ln_eps; LossHyp."""
+    return tuple(_value(getattr(s, f)) for f, t in s._fields_ if t is not C.c_void_p)
 
 
 def key(rec) -> tuple:
@@ -95,11 +117,12 @@ def key(rec) -> tuple:
         elif isinstance(a, C.Array):
             if issubclass(a._type_, C.Structure):
                 out.append(tuple(_fields(s) for s in a))
+            elif a._type_ is C.c_void_p:                  # per-level pointers (compute_loss): not geometry
+                continue
             else:
                 out.append(tuple(a))
-        elif type(a).__name__ == "CArgObject":           # byref(ConvGeom)
-            s = a._obj
-            out.append(tuple(getattr(s, f) for f, _ in s._fields_))
+        elif type(a).__name__ == "CArgObject":           # byref(ConvGeom), byref(LossHyp)
+            out.append(_fields(a._obj))
         else:
             raise TypeError(f"{name}: argument {i} of type {type(a).__name__} has no key form")
     return tuple(out)
@@ -183,6 +206,7 @@ class Operands:
     def __init__(self, device, seed: int):
         self.dev = torch.device(device)
         self.meta = self.dev.type == "meta"
+        self.seed = seed
         self.gen = None if self.meta else torch.Generator(device=self.dev).manual_seed(seed)
 
     def randn(self, *shape, dtype=torch.float16, scale=1.0):
@@ -793,8 +817,195 @@ def _maxpool5_bwd(rec, R: Operands) -> List[Check]:
     return [Check("dx", dx, ref, 1e-3, "l2")]
 
 
+def _f32_hit(f, x0: float, want: float, side: str) -> np.float32:
+    """The fp32 x next to x0 at which the monotone fp32 function f reaches `want`: side 'at' f(x) == want exactly, 'below'
+    the largest x with f(x) < want, 'above' the smallest x with f(x) > want."""
+    up = lambda v: np.nextafter(v, np.float32(np.inf))        # noqa: E731
+    down = lambda v: np.nextafter(v, np.float32(-np.inf))     # noqa: E731
+    want = np.float32(want)
+    x = np.float32(x0)
+    while f(x) < want:
+        x = up(x)
+    while f(down(x)) >= want:
+        x = down(x)
+    if side == "at":
+        assert f(x) == want, (x0, want)
+        return x
+    if side == "below":
+        return down(x)
+    while f(x) <= want:
+        x = up(x)
+    return x
+
+
+def _grid(n: int):
+    """fp32 normalised coordinate -> grid coordinate, as build_targets scales it (targets * gain, loss.py:425-426)."""
+    n = np.float32(n)
+    return lambda x: np.float32(x) * n
+
+
+def _loss_targets(rng, nt: int, B: int, nc: int, ny, nx, anchors):
+    """(nt, 6) fp32 targets [image, class, x, y, w, h] that hit the edges of build_targets (loss.py:405-463) on every level,
+    then random boxes.  The last image of a batch of two or more gets none.  Rows 0-3: two pairs of targets contesting one
+    (image, anchor, cell) of the coarsest level, the better-fitting one first in one pair and second in the other (their
+    predictions are set by _contest_logits)."""
+    rows = []
+    L = len(ny) - 1
+    aw, ah = anchors[L][0]
+    for k, (gi, gj) in enumerate(((1, 1), (nx[L] - 3, ny[L] - 2))):
+        fit = [gi + 0.3, gj + 0.3, 1.2 * aw, 1.2 * ah]
+        off = [gi + 0.3, gj + 0.3, 2.0 * aw, 0.8 * ah]
+        for box in ((fit, off) if k == 0 else (off, fit)):
+            rows.append([0, 0, box[0] / nx[L], box[1] / ny[L], box[2] / nx[L], box[3] / ny[L]])
+    edges = []                     # per kind, per level
+    for lvl in range(len(ny)):
+        gx, gy = _grid(nx[lvl]), _grid(ny[lvl])
+        a_w, a_h = anchors[lvl][0]
+        w, h = a_w / nx[lvl], a_h / ny[lvl]
+        kx, ky = nx[lvl] // 3, ny[lvl] // 3
+        sx, sy = (kx + 0.25) / nx[lvl], (ky + 0.25) / ny[lvl]            # a plain coordinate on the other axis
+        kinds = []
+        for n, f, safe, k, put in ((nx[lvl], gx, sy, kx, lambda v, s: (v, s)), (ny[lvl], gy, sx, ky, lambda v, s: (s, v))):
+            for want, side in ((k + 0.5, "at"), (k + 0.5, "below"),               # fractional part at / just below 0.5
+                               (1.0, "at"), (1.0, "above"),                          # g at / just above 1
+                               (n - 1.0, "at"), (n - 1.0, "below"),                  # n - g at / just above 1
+                               (n - k - 0.5, "above")):                              # n - g: fractional part just below 0.5
+                kinds.append((*put(float(_f32_hit(f, want / n, want, side)), safe), w, h))
+        kinds += [(1.0, sy, w, h), (sx, 1.0, w, h), (1.0, 1.0, w, h), (0.0, 0.0, w, h)]     # image border: gi / gj clamp
+        ratio = lambda v, s=a_w, f=gx: np.float32(f(v) / np.float32(s))                   # noqa: E731  gw / anchor_w
+        for side in ("at", "below", "above"):                                             # gw / aw at / around anchor_t = 4
+            kinds.append((sx, sy, float(_f32_hit(ratio, 4 * w, 4.0, side)), h))
+        hr = lambda v, s=a_h, f=gy: np.float32(f(v) / np.float32(s))                      # noqa: E731  gh / ah = 1 / 4
+        kinds.append((sx, sy, w, float(_f32_hit(hr, h / 4, 0.25, "at"))))
+        edges.append(kinds)
+    for kind in zip(*edges):
+        for x, y, w, h in kind:
+            rows.append([0, 0, x, y, w, h])
+    n_img = max(B - 1, 1)
+    for i in range(4, len(rows)):
+        rows[i][0] = i % n_img
+        rows[i][1] = i % nc
+    t = np.zeros((nt, 6), dtype=np.float32)
+    t[:min(nt, len(rows))] = np.array(rows[:nt], dtype=np.float32)
+    r = nt - len(rows)
+    if r > 0:
+        t[len(rows):, 0] = rng.integers(0, n_img, r)
+        t[len(rows):, 1] = rng.integers(0, nc, r)
+        t[len(rows):, 2:4] = rng.uniform(0.0, 1.0, (r, 2))
+        t[len(rows):, 4:6] = np.exp(rng.uniform(np.log(0.005), np.log(0.4), (r, 2)))
+    return t
+
+
+def _contest_logits(buf, t, ny, nx, anchors):
+    """Anchor 0's box logits of the coarsest level at the cell of the better-fitting target of each contested pair (rows 0
+    and 3), decoding to that target's box, so that the two targets of a pair have clearly different IoUs there (loss.py:355-361
+    decode, inverted)."""
+    L = len(ny) - 1
+    aw, ah = anchors[L][0]
+    logit = lambda s: math.log(s / (1 - s))       # noqa: E731
+    for row in (0, 3):
+        if row >= len(t):
+            break
+        x, y, w, h = (float(v) for v in t[row, 2:6])
+        gx, gy = x * nx[L], y * ny[L]
+        gi, gj = int(gx), int(gy)
+        sx, sy = (gx - gi + 0.5) / 2, (gy - gj + 0.5) / 2
+        sw, sh = math.sqrt(w * nx[L] / aw) / 2, math.sqrt(h * ny[L] / ah) / 2
+        v = torch.tensor([logit(sx), logit(sy), logit(sw), logit(sh)], dtype=buf.dtype)
+        buf[int(t[row, 0]), gj, gi, 0:4] = v.to(buf.device)
+
+
+def _loss(rec, R: Operands) -> List[Check]:
+    """icaf_compute_loss_fwd and _bwd of one record (the builder issues both, like the training step): fp16 head maps in
+    the record's NHWC layout with pitch p_ld (pad channels NaN: the kernels must not read them), targets on the edges of
+    build_targets, against the oracle's ComputeLoss (oracle/focal_loss.py) in float64 on the fp16 predictions, with fp32
+    targets and anchors so that candidate selection is the reference's fp32 arithmetic.  Replayed at the record's fl_gamma,
+    at the other of 0 / 1.5, and once with no targets."""
+    import types
+    from icafusion_b200.loss import ComputeLoss
+    _, args, _ = rec
+    p_ld, ny, nx, nl, B, na, no, nt = args[2], list(args[3]), list(args[4]), args[5], args[6], args[7], args[8], args[10]
+    nc = no - 5
+    anchors = torch.tensor(list(args[11]), dtype=torch.float32).view(nl, na, 2)
+    h = args[12]._obj
+    hyp = dict(box=h.box, obj=h.obj, cls=h.cls, cls_pw=h.cls_pw, obj_pw=h.obj_pw, anchor_t=h.anchor_t, fl_gamma=h.fl_gamma,
+               label_smoothing=2.0 * h.cn)
+    rng = np.random.Generator(np.random.PCG64(R.seed))
+    tg = _loss_targets(rng, nt, B, nc, ny, nx, anchors.tolist())
+    bufs, views = [], []
+    for lvl in range(nl):
+        buf = R.nan(B, ny[lvl], nx[lvl], p_ld)
+        logits = R.randn(B, ny[lvl], nx[lvl], na, no, dtype=torch.float32)
+        if not R.meta:
+            logits[..., 4] = 1.5 * logits[..., 4] - 4.0                    # objectness: mostly background
+        buf[..., :na * no] = logits.view(B, ny[lvl], nx[lvl], na * no).half()
+        bufs.append(buf)
+        views.append(buf.as_strided((B, na, ny[lvl], nx[lvl], no), (ny[lvl] * nx[lvl] * p_ld, no, nx[lvl] * p_ld, p_ld, 1)))
+    if not R.meta:
+        _contest_logits(bufs[-1], tg, ny, nx, anchors.tolist())
+    checks = []
+    other = 1.5 if not h.fl_gamma > 0 else 0.0
+    for gamma, t in ((h.fl_gamma, tg), (other, tg), (h.fl_gamma, tg[:0])):
+        hp = dict(hyp, fl_gamma=gamma)
+        det = types.SimpleNamespace(na=na, nc=nc, nl=nl, anchors=anchors)
+        crit = ComputeLoss(types.SimpleNamespace(hyp=hp, gr=h.gr, model=[det]))
+        checks += _loss_case(crit, R, views, bufs, p_ld, torch.from_numpy(t).to(R.dev), anchors, hp, h.gr,
+                             f"fl_gamma {gamma:g} nt {len(t)}")
+    return checks
+
+
+LOSS_GRAD_OUT = 256.0      # d/d(loss * bs) fed to the backward: keeps the fp16 gradient of every level in the normal range
+
+
+def _loss_case(crit, R: Operands, views, bufs, p_ld, tg, anchors, hyp, gr, tag) -> List[Check]:
+    from oracle import focal_loss
+    crit.with_backward = True
+    ld, ps = crit._layout(views)
+    assert ld == p_ld, (ld, p_ld)
+    B = views[0].shape[0]
+    na, no = views[0].shape[1], views[0].shape[4]
+    out, out2 = R.nan(5, dtype=torch.float32), R.nan(5, dtype=torch.float32)
+    ws = crit._launch(ps, p_ld, tg, out=out)
+    crit._launch(ps, p_ld, tg, out=out2)
+    dbufs, dps = [], []
+    for v in views:
+        _, _, ny, nx, _ = v.shape
+        d = R.nan(B + 2, ny, nx, p_ld)                        # images 0 and B + 1: NaN neighbours the backward must not touch
+        d[1:B + 1, ..., na * no:] = 0                         # pad channels zeroed, as _LossFn.backward allocates them
+        dbufs.append(d)
+        dps.append(d[1:B + 1].as_strided(v.shape, v.stride()))
+    gout = torch.full((1,), LOSS_GRAD_OUT, dtype=torch.float32, device=R.dev)
+    crit._launch(ps, p_ld, tg, ws=ws, grad_out=gout, dps=dps)
+    if R.meta:
+        return []
+
+    @functools.lru_cache(None)
+    def ref():
+        pr = [v.detach().double().cpu().requires_grad_(True) for v in views]
+        lo, items = focal_loss.compute_loss(pr, tg.cpu(), anchors, hyp, gr)
+        (lo * LOSS_GRAD_OUT).backward()
+        return torch.cat([lo.detach().view(1), items.detach()]), [p.grad for p in pr]
+
+    checks = [Check(f"{tag}: loss, lbox, lobj, lcls", lambda: out.cpu(), lambda: ref()[0], 1.0, "close", (2e-6, 3e-5)),
+              Check(f"{tag}: forward repeat", out2, out, 0.0, "exact")]
+    for lvl, (dp, d) in enumerate(zip(dps, dbufs)):
+        # 2e-5 of the level's largest gradient, plus the half ulp of the kernel's final rounding to fp16 (2^-11 of the value)
+        scale = lambda lvl=lvl: float(ref()[1][lvl].abs().max())                              # noqa: E731
+        checks.append(Check(f"{tag}: dp[{lvl}]", lambda dp=dp, s=scale: dp.double().cpu() / s(),
+                            lambda lvl=lvl, s=scale: ref()[1][lvl] / s(), 1.0, "close", (2e-5, 2.0 ** -11)))
+        if p_ld > na * no:
+            checks.append(Check(f"{tag}: dp[{lvl}] pad channels", lambda d=d: d[1:B + 1, ..., na * no:],
+                                lambda d=d: torch.zeros_like(d[1:B + 1, ..., na * no:]), 0.0, "exact"))
+        nb = lambda d=d: torch.cat([d[0].reshape(-1), d[B + 1].reshape(-1)])                   # noqa: E731
+        checks.append(Check(f"{tag}: dp[{lvl}] neighbours unchanged", nb,
+                            lambda nb=nb: torch.full(nb().shape, NAN16, dtype=torch.int16, device=R.dev).view(torch.float16), 0.0, "exact"))
+    return checks
+
+
 REPLAYED = {
     "icaf_conv2d_fwd": _conv_fwd,
+    "icaf_compute_loss_fwd": _loss,           # both builders issue the forward and the backward
+    "icaf_compute_loss_bwd": _loss,
     "icaf_bottleneck_fwd": _bottleneck,
     "icaf_conv2d_wgrad": _wgrad,            # and the data gradient of the same layer
     "icaf_pack_weight_pair": _pack_pair,

@@ -24,8 +24,24 @@ def records(walks):
 
 def test_configurations():
     ids = [c.id for c in census.CONFIGS]
-    assert len(ids) == len(set(ids)) == 5 * 2 * 2 + 3 * 2
+    assert len(ids) == len(set(ids)) == 5 * 2 * 2 + 3 * 2 + 5 * 2 + 5 * 2 * 2 + 3 * 3 + 1
     assert "yolov5x-kaist-512x640-b16-infer" in ids and "yolov5l-kaist-512x640-b16-train" in ids
+    # train.py's mosaic batches (640x640, batch 8 by default) and test.py's rectangular validation batches (544x672)
+    for s in "nsl":
+        assert {f"yolov5{s}-kaist-640x640-b{B}-train" for B in (8, 16, 3)} <= set(ids)
+    assert "yolov5s-flir-640x640-b8-train" in ids
+    assert {f"yolov5{s}-{ds}-544x672-b{B}-infer" for s in "nsmlx" for ds in ("kaist", "flir") for B in (1, 32)} <= set(ids)
+    assert {f"yolov5{s}-flir-512x640-b{B}-infer" for s in "nsmlx" for B in (1, 16)} <= set(ids)
+
+
+def test_keys_are_pointer_free():
+    """Two walks of one configuration give the same key set: no pointer, seed or per-call object reaches a key (the loss
+    records pass per-level pointer arrays and byref(LossHyp))."""
+    c = census.Config("train", "n", "kaist", 3, 640, 640)
+    a, b = (census.walk(c.kind, f"yolov5{c.size}_Transfusion_{c.dataset}", c.B, c.H, c.W) for _ in range(2))
+    ka, kb = set(census.unique(a)), set(census.unique(b))
+    assert ka == kb
+    assert {"icaf_compute_loss_fwd", "icaf_compute_loss_bwd"} <= {k[0] for k in ka}
 
 
 def test_every_entry_point_is_accounted_for(walks):
@@ -53,7 +69,7 @@ def test_census_covers_every_conv_plan_family(records):
         splits[pl.splits] += 1
     print(f"\n{len(convs)} conv, {len(wgrads)} wgrad, {len(slices)} slice launches; bn {dict(bns)} a_mode {dict(modes)} {dict(kinds)} "
           f"splits {dict(sorted(splits.items()))}")
-    assert len(convs) >= 1400 and len(wgrads) >= 225 and len(slices) >= 400
+    assert len(convs) >= 2450 and len(wgrads) >= 525 and len(slices) >= 625
     assert {32, 64, 128} <= set(bns) and {0, 1, 2} <= set(modes) and {"persistent", "one-tile"} <= set(kinds)
     assert {2, 3, 4, 5, 6, 8} <= set(splits)
 
@@ -71,4 +87,5 @@ def test_builders_reissue_the_recorded_launch(records):
         issued = {census.key(r) for r in dr.records}
         assert k in issued, f"{census.describe(rec)}: the replay issued {sorted(issued, key=str)[:4]}"
         done[k[0]] += 1
+    print("\ndistinct launches replayed per entry point: " + ", ".join(f"{n} {c}" for n, c in sorted(done.items())))
     assert set(done) == set(census.REPLAYED)

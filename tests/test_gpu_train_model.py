@@ -41,7 +41,13 @@ def _step(cuda_device, m, d):
 
 
 def test_training_step_yolov5s_320(cuda_device):
-    m, d = load_golden("train_yolov5s_320")
+    check_training_step(cuda_device, "train_yolov5s_320")
+
+
+def check_training_step(cuda_device, name):
+    """One step of the golden's case against fp32 autograd through the oracle and the reference's own step, each bar taken
+    relative to the reference's fp16-autocast regime."""
+    m, d = load_golden(name)
     model, pred, loss, items, (rl, ri, rg, rp, rstate), (_, _, ag, ap, _) = _step(cuda_device, m, d)
     got = torch.cat([loss.detach(), items]).cpu().numpy()
     want = np.concatenate([rl.numpy().reshape(1), ri.numpy()])
