@@ -55,6 +55,11 @@ class AugSample(C.Structure):
                [("lut", C.c_uint8 * (2 * 3 * 256))]
 
 
+class ValSample(C.Structure):
+    _fields_ = [("rgb", C.c_void_p), ("ir", C.c_void_p)] + \
+               [(n, C.c_int) for n in ("H0", "W0", "h", "w", "top", "left", "mode", "xtab", "ytab", "sx", "sy", "reserved")]
+
+
 KERNEL_TC = 0
 
 _vp, _i, _i64, _f = C.c_void_p, C.c_int, C.c_int64, C.c_float
@@ -123,6 +128,8 @@ SIGNATURES = {
     "icaf_detect_decode": [_vp, _i64, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _f, C.POINTER(C.c_float), _vp],
     "icaf_augment_params_bytes": [_i, _i, _i],
     "icaf_augment": [_vp, C.c_size_t, _i, _i, _i, _vp, _vp, _vp],
+    "icaf_val_stage_params_bytes": [_i, _i],
+    "icaf_val_stage": [_vp, C.c_size_t, _i, _i, _i, _i, _vp, _vp],
 }
 
 _lib = None
@@ -150,7 +157,7 @@ def lib() -> C.CDLL:
                           "icaf_kaist_mr_workspace_bytes": C.c_size_t,
                           "icaf_conv2d_wgrad_workspace_bytes": C.c_size_t, "icaf_train_workspace_bytes": C.c_size_t,
                           "icaf_cross_attention_bwd_workspace_bytes": C.c_size_t,
-                          "icaf_augment_params_bytes": C.c_size_t}.get(name, C.c_int)
+                          "icaf_augment_params_bytes": C.c_size_t, "icaf_val_stage_params_bytes": C.c_size_t}.get(name, C.c_int)
         _lib = L
     return _lib
 

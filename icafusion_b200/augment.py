@@ -24,7 +24,7 @@ import numpy as np
 import torch
 
 from . import _lib, ops
-from .datasets import letterbox_geometry, resize_taps
+from .datasets import frames_on_device, letterbox_geometry, resize_taps
 
 PAD = 114
 AB_BITS, INTER_BITS = 10, 5                 # cv2 imgwarp.cpp: AB_SCALE = 1 << 10, INTER_TAB_SIZE = 32
@@ -413,37 +413,6 @@ class Augment:
     def draw(self, indices: Sequence[int]) -> List[SampleDraw]:
         return [draw_sample(int(i), len(self.labels), self.img_size, self.hyp) for i in indices]
 
-    def _frames_on_device(self, needed: Sequence[int]):
-        """index -> ((rgb, ir) device uint8 frames, (H0, W0)); host frames go up in one pinned copy."""
-        got, host = {}, []
-        for idx in needed:
-            rgb, ir = self.frames(idx)
-            for f in (rgb, ir):
-                if f.dtype not in (np.uint8, torch.uint8) or f.ndim != 3 or f.shape[2] != 3:
-                    raise ValueError(f"augment: frame {idx} must be uint8 (H0, W0, 3) BGR, got {f.dtype} {tuple(f.shape)}")
-            if tuple(rgb.shape) != tuple(ir.shape):
-                raise ValueError(f"augment: RGB and IR frames of index {idx} differ in size: {tuple(rgb.shape)} vs {tuple(ir.shape)}")
-            got[idx] = [rgb, ir]
-            for m, f in enumerate((rgb, ir)):
-                if isinstance(f, torch.Tensor):
-                    if not ops.on_device(f):
-                        f = f.numpy()
-                    else:
-                        got[idx][m] = f.contiguous()
-                        continue
-                host.append((idx, m, np.ascontiguousarray(f)))
-        if host:
-            sizes = [a.nbytes for _, _, a in host]
-            offs = np.concatenate([[0], np.cumsum([(n + 255) // 256 * 256 for n in sizes])]).astype(np.int64)
-            buf = torch.empty(int(offs[-1]), dtype=torch.uint8, pin_memory=not ops.dry_running())
-            bn = buf.numpy()
-            for (idx, m, a), o in zip(host, offs):
-                bn[o:o + a.nbytes] = a.reshape(-1)
-            dev = buf.to(self.device, non_blocking=True)
-            for (idx, m, a), o in zip(host, offs):
-                got[idx][m] = dev[o:o + a.nbytes].view(a.shape)
-        return {k: (v[0], v[1]) for k, v in got.items()}
-
     def __call__(self, indices: Sequence[int], out: Optional[Tuple[torch.Tensor, torch.Tensor]] = None):
         import time
         t0 = time.perf_counter()
@@ -452,7 +421,7 @@ class Augment:
             raise ValueError("augment: empty batch")
         draws = self.draw(indices)
         needed = sorted({i for d in draws for i in d.indices})
-        frames = self._frames_on_device(needed)
+        frames = frames_on_device(self.frames, needed, self.device, "augment")
         shapes = {i: (int(frames[i][0].shape[0]), int(frames[i][0].shape[1])) for i in needed}
         samples = (_lib.AugSample * B)()
         warp = np.zeros((B, 4, s), dtype=np.int32)

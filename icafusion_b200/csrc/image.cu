@@ -88,6 +88,120 @@ __global__ void letterbox_kernel(const LetterboxParams P) {
   d[0] = (unsigned char)v2; d[hw] = (unsigned char)v1; d[2 * hw] = (unsigned char)v0;
 }
 
+// ------------------------------------------------------------------------------------------------
+// Validation batch staging (utils/datasets.py:948-1024, augment=False, rect=True): one thread per 4 adjacent output pixels of
+// one sample, both frames; each of the 6 output planes gets one 32-bit store.  A pixel inside the load_image rectangle is
+// cv2.resize of the decoded frame -- copy, INTER_LINEAR (the letterbox arithmetic above) or INTER_AREA (resizeAreaFast's
+// block sums, or resizeArea_'s float taps with every product and sum rounded in cv2's order) -- and 114 outside it.
+constexpr int kValThreads = 256;
+constexpr int kValPad = 114;
+
+struct ValStageParams {
+  const icaf_val_sample* samples; const int* tab;
+  unsigned char* out;
+  int H, W;
+};
+
+__device__ __forceinline__ unsigned char sat_u8(float v) { return (unsigned char)min(255, max(0, __float2int_rn(v))); }
+
+// Pixel (x, y) of the load_image-resized pair: v[0..2] = RGB frame B, G, R; v[3..5] = IR frame.
+__device__ __forceinline__ void val_pixel(const icaf_val_sample& S, const int* __restrict__ tab, int x, int y, int (&v)[6]) {
+  const unsigned char* fr[2] = {static_cast<const unsigned char*>(S.rgb), static_cast<const unsigned char*>(S.ir)};
+  const long long row = (long long)S.W0 * 3;
+  if (S.mode == ICAF_VAL_COPY) {
+#pragma unroll
+    for (int m = 0; m < 2; ++m) {
+      const unsigned char* p = fr[m] + y * row + x * 3;
+      v[3 * m] = p[0]; v[3 * m + 1] = p[1]; v[3 * m + 2] = p[2];
+    }
+  } else if (S.mode == ICAF_VAL_LINEAR) {
+    const int4 tx = reinterpret_cast<const int4*>(tab + S.xtab)[x], ty = reinterpret_cast<const int4*>(tab + S.ytab)[y];
+#pragma unroll
+    for (int m = 0; m < 2; ++m) {
+      const unsigned char* r0 = fr[m] + ty.x * row;
+      const unsigned char* r1 = fr[m] + ty.y * row;
+#pragma unroll
+      for (int c = 0; c < 3; ++c) {
+        const int h0 = r0[tx.x * 3 + c] * tx.z + r0[tx.y * 3 + c] * tx.w;
+        const int h1 = r1[tx.x * 3 + c] * tx.z + r1[tx.y * 3 + c] * tx.w;
+        v[3 * m + c] = (((ty.z * (h0 >> 4)) >> 16) + ((ty.w * (h1 >> 4)) >> 16) + 2) >> 2;
+      }
+    }
+  } else if (S.mode == ICAF_VAL_AREA_FAST) {
+    int sum[6] = {0, 0, 0, 0, 0, 0};
+    for (int dy = 0; dy < S.sy; ++dy)
+      for (int dx = 0; dx < S.sx; ++dx) {
+        const long long o = (long long)(y * S.sy + dy) * row + (x * S.sx + dx) * 3;
+#pragma unroll
+        for (int m = 0; m < 2; ++m) {
+          sum[3 * m] += fr[m][o]; sum[3 * m + 1] += fr[m][o + 1]; sum[3 * m + 2] += fr[m][o + 2];
+        }
+      }
+    if (S.sx == 2 && S.sy == 2) {
+#pragma unroll
+      for (int c = 0; c < 6; ++c) v[c] = (sum[c] + 2) >> 2;
+    } else {
+      const float scale = __fdiv_rn(1.0f, (float)(S.sx * S.sy));
+#pragma unroll
+      for (int c = 0; c < 6; ++c) v[c] = sat_u8(__fmul_rn((float)sum[c], scale));
+    }
+  } else {
+    const int2 hx = reinterpret_cast<const int2*>(tab + S.xtab)[x], hy = reinterpret_cast<const int2*>(tab + S.ytab)[y];
+    const int2* tx = reinterpret_cast<const int2*>(tab + S.xtab + hx.x);
+    const int2* ty = reinterpret_cast<const int2*>(tab + S.ytab + hy.x);
+    float acc[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+    for (int j = 0; j < hy.y; ++j) {
+      const int2 t = ty[j];
+      const float beta = __int_as_float(t.y);
+      float buf[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+      for (int k = 0; k < hx.y; ++k) {
+        const int2 s = tx[k];
+        const float alpha = __int_as_float(s.y);
+        const long long o = t.x * row + s.x * 3;
+#pragma unroll
+        for (int m = 0; m < 2; ++m)
+#pragma unroll
+          for (int c = 0; c < 3; ++c) buf[3 * m + c] = __fadd_rn(buf[3 * m + c], __fmul_rn((float)fr[m][o + c], alpha));
+      }
+#pragma unroll
+      for (int c = 0; c < 6; ++c) acc[c] = __fadd_rn(acc[c], __fmul_rn(beta, buf[c]));
+    }
+#pragma unroll
+    for (int c = 0; c < 6; ++c) v[c] = sat_u8(acc[c]);
+  }
+}
+
+__global__ void __launch_bounds__(kValThreads) val_stage_kernel(const ValStageParams P) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const int b = blockIdx.y;
+  const int W4 = P.W >> 2;
+  const int q = blockIdx.x * blockDim.x + threadIdx.x;
+  if (q >= P.H * W4) return;
+  const int y = q / W4, x0 = (q - y * W4) * 4;
+  const icaf_val_sample& S = P.samples[b];
+  uint32_t word[6] = {0, 0, 0, 0, 0, 0};
+  const int yy = y - S.top;
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const int xx = x0 + i - S.left;
+    int v[6] = {kValPad, kValPad, kValPad, kValPad, kValPad, kValPad};
+    if (yy >= 0 && yy < S.h && xx >= 0 && xx < S.w) val_pixel(S, P.tab, xx, yy, v);
+#pragma unroll
+    for (int m = 0; m < 2; ++m) {                           // planar RGB: channel 0 = R = source channel 2
+      word[3 * m] |= uint32_t(v[3 * m + 2]) << (8 * i);
+      word[3 * m + 1] |= uint32_t(v[3 * m + 1]) << (8 * i);
+      word[3 * m + 2] |= uint32_t(v[3 * m]) << (8 * i);
+    }
+  }
+  const long long plane = (long long)P.H * P.W;
+  uint32_t* d = reinterpret_cast<uint32_t*>(P.out + (long long)b * 6 * plane + (long long)y * P.W + x0);
+#pragma unroll
+  for (int c = 0; c < 6; ++c) d[c * (plane >> 2)] = word[c];
+}
+
+static size_t val_align16(size_t n) { return (n + 15) & ~size_t(15); }
+
 }  // namespace icaf
 
 using namespace icaf;
@@ -131,4 +245,25 @@ extern "C" int icaf_letterbox(const void* src, int B, int H0, int W0, void* dst,
   P.src = (const unsigned char*)src; P.dst = (unsigned char*)dst; P.xtab = resize ? xtab : nullptr; P.ytab = resize ? ytab : nullptr;
   P.B = B; P.H0 = H0; P.W0 = W0; P.H = H; P.W = W; P.top = top; P.left = left; P.new_h = new_h; P.new_w = new_w; P.pad = pad_value;
   return launch_k("letterbox", letterbox_kernel, dim3(blocks_for((long long)B * H * W, 256)), dim3(256), 0, (cudaStream_t)stream, P);
+}
+
+extern "C" size_t icaf_val_stage_params_bytes(int B, int n_words) {
+  if (B < 1 || B > 65535 || n_words < 0 || (n_words & 3)) return 0;
+  return val_align16((size_t)B * sizeof(icaf_val_sample)) + (size_t)n_words * sizeof(int);
+}
+
+extern "C" int icaf_val_stage(const void* params, size_t params_bytes, int B, int H, int W, int n_words, void* out, void* stream) {
+  if (!params || !out) return set_error(ICAF_ERR_BAD_ARG, "val_stage: null pointer");
+  if (H < 1 || W < 4 || (W & 3) || (long long)H * W > (1ll << 30)) return set_error(ICAF_ERR_BAD_ARG, "val_stage: H x W must be positive with W % 4 == 0");
+  const size_t need = icaf_val_stage_params_bytes(B, n_words);
+  if (!need || params_bytes < need) return set_error(ICAF_ERR_BAD_ARG, "val_stage: bad batch or parameter block smaller than icaf_val_stage_params_bytes");
+  if ((reinterpret_cast<uintptr_t>(params) & 15) || (reinterpret_cast<uintptr_t>(out) & 3))
+    return set_error(ICAF_ERR_BAD_ARG, "val_stage: parameter block not 16-byte aligned or output not 4-byte aligned");
+  ValStageParams P;
+  P.samples = static_cast<const icaf_val_sample*>(params);
+  P.tab = reinterpret_cast<const int*>(static_cast<const char*>(params) + val_align16((size_t)B * sizeof(icaf_val_sample)));
+  P.out = static_cast<unsigned char*>(out);
+  P.H = H; P.W = W;
+  const dim3 grid(blocks_for((long long)H * (W / 4), kValThreads), (unsigned)B);
+  return launch_k("val_stage", val_stage_kernel, grid, dim3(kValThreads), 0, (cudaStream_t)stream, P);
 }

@@ -8,7 +8,7 @@ staging kernel (/255 -> fp16, space-to-depth) consumes."""
 from __future__ import annotations
 
 import functools
-from typing import Tuple
+from typing import Callable, Sequence, Tuple
 
 import numpy as np
 import torch
@@ -51,6 +51,39 @@ def _device_taps(src: int, dst: int, vertical: bool, device) -> torch.Tensor:
     if t is None:
         t = _TAPS_ON_DEVICE[key] = torch.from_numpy(resize_taps(src, dst, vertical)).to(device)
     return t
+
+
+def frames_on_device(frames: Callable[[int], Tuple[object, object]], needed: Sequence[int], device, what: str):
+    """index -> (rgb, ir) device uint8 frames for the decoded BGR uint8 (H0, W0, 3) pairs frames(index) returns (numpy arrays
+    or tensors); host frames go up in one pinned copy.  `what` names the caller in error messages."""
+    got, host = {}, []
+    for idx in needed:
+        rgb, ir = frames(idx)
+        for f in (rgb, ir):
+            if f.dtype not in (np.uint8, torch.uint8) or f.ndim != 3 or f.shape[2] != 3:
+                raise ValueError(f"{what}: frame {idx} must be uint8 (H0, W0, 3) BGR, got {f.dtype} {tuple(f.shape)}")
+        if tuple(rgb.shape) != tuple(ir.shape):
+            raise ValueError(f"{what}: RGB and IR frames of index {idx} differ in size: {tuple(rgb.shape)} vs {tuple(ir.shape)}")
+        got[idx] = [rgb, ir]
+        for m, f in enumerate((rgb, ir)):
+            if isinstance(f, torch.Tensor):
+                if not ops.on_device(f):
+                    f = f.numpy()
+                else:
+                    got[idx][m] = f.contiguous()
+                    continue
+            host.append((idx, m, np.ascontiguousarray(f)))
+    if host:
+        sizes = [a.nbytes for _, _, a in host]
+        offs = np.concatenate([[0], np.cumsum([(n + 255) // 256 * 256 for n in sizes])]).astype(np.int64)
+        buf = torch.empty(int(offs[-1]), dtype=torch.uint8, pin_memory=not ops.dry_running())
+        bn = buf.numpy()
+        for (idx, m, a), o in zip(host, offs):
+            bn[o:o + a.nbytes] = a.reshape(-1)
+        dev = buf.to(device, non_blocking=True)
+        for (idx, m, a), o in zip(host, offs):
+            got[idx][m] = dev[o:o + a.nbytes].view(a.shape)
+    return {k: (v[0], v[1]) for k, v in got.items()}
 
 
 def letterbox_geometry(shape: Tuple[int, int], new_shape=(640, 640), scaleup: bool = True):

@@ -150,6 +150,36 @@ int icaf_pack_image(const void* src, int src_dtype, float scale, int B, int H, i
 int icaf_letterbox(const void* src, int B, int H0, int W0, void* dst, int H, int W, int top, int left, int new_h, int new_w,
                    const int* xtab, const int* ytab, int pad_value, void* stream);
 
+/* Validation batch staging: LoadMultiModalImagesAndLabels.__getitem__ (utils/datasets.py:948-1024) with augment=False,
+ * rect=True -- load_image_rgb_ir's resize (:1097-1125: a copy at r = 1, cv2.resize INTER_LINEAR at r > 1, INTER_AREA at
+ * r < 1), letterbox to the batch shape (scaleup=False: a border only), BGR->RGB, HWC->CHW -- and collate_fn's stack of the
+ * 6-channel images, for a batch, one launch, bit-exact against cv2.  Geometry and tables are the host's
+ * (icafusion_b200/valdata.py). */
+#define ICAF_VAL_COPY 0        /* (h, w) == (H0, W0)                                                                     */
+#define ICAF_VAL_LINEAR 1      /* INTER_LINEAR: xtab / ytab = int4 {i0, i1, w0, w1} rows [w] / [h] as for icaf_letterbox */
+#define ICAF_VAL_AREA_FAST 2   /* INTER_AREA, integer scales sx, sy: block sums; 2 x 2 rounds (s + 2) >> 2, else
+                                  saturate_cast<uchar>(s * (1.f / (sx sy)))                                                */
+#define ICAF_VAL_AREA 3        /* INTER_AREA, other scales: xtab / ytab = [dst] int2 {first tap word (from the table),
+                                  count} + int2 {si, alpha float bits} taps in cv2's order (computeResizeAreaTab)          */
+typedef struct {
+  const void* rgb; const void* ir;  /* device uint8 (H0, W0, 3) BGR frames of this sample                              */
+  int H0, W0;                       /* decoded size                                                                    */
+  int h, w;                         /* load_image size (int(h0 r), int(w0 r))                                          */
+  int top, left;                    /* its place in the (H, W) batch image; the rest is 114                            */
+  int mode;                         /* ICAF_VAL_*                                                                      */
+  int xtab, ytab;                   /* word offsets of the column / row tables in the table region (16-byte aligned)   */
+  int sx, sy;                       /* ICAF_VAL_AREA_FAST scales                                                        */
+  int reserved;
+} icaf_val_sample;
+
+/* Bytes of the parameter block for B samples with n_words table words.  Layout: icaf_val_sample [B] at 0, int32 tables
+ * [n_words] at align16(B * sizeof(icaf_val_sample)).  0 for a bad argument. */
+size_t icaf_val_stage_params_bytes(int B, int n_words);
+
+/* params: device block laid out as above (16-byte aligned); out: uint8 (B, 6, H, W) -- RGB frame in channels 0-2, IR frame
+ * in 3-5, each R, G, B.  W % 4 == 0 (batch shapes are stride multiples). */
+int icaf_val_stage(const void* params, size_t params_bytes, int B, int H, int W, int n_words, void* out, void* stream);
+
 /* Same staging, space-to-depth layout: dst is (B, H/2, W/2, 16) fp16 with channel (dy*2+dx)*4 + c (c = r,g,b,0).
  * A 6x6 / stride 2 / pad 2 stem convolution over the image (yolov5 "P1/2" row of the model YAML) is then exactly a
  * 3x3 / stride 1 / pad 1 convolution over this tensor (ky = 2*ty+dy, kx = 2*tx+dx), which runs on the TMA path. H, W even. */
