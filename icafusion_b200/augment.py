@@ -24,7 +24,7 @@ import numpy as np
 import torch
 
 from . import _lib, ops
-from .datasets import frames_on_device, letterbox_geometry, resize_taps
+from .datasets import ParamBlock, frames_on_device, letterbox_geometry, resize_taps
 
 PAD = 114
 AB_BITS, INTER_BITS = 10, 5                 # cv2 imgwarp.cpp: AB_SCALE = 1 << 10, INTER_TAB_SIZE = 32
@@ -425,19 +425,8 @@ class Augment:
         shapes = {i: (int(frames[i][0].shape[0]), int(frames[i][0].shape[1])) for i in needed}
         samples = (_lib.AugSample * B)()
         warp = np.zeros((B, 4, s), dtype=np.int32)
-        taps, tap_rows, n_taps = {}, [], 0
+        block = ParamBlock()
         per_labels = []
-
-        def tap(src, dst, vertical):
-            nonlocal n_taps
-            key = (src, dst, vertical)
-            if key not in taps:
-                t = resize_taps(src, dst, vertical)
-                taps[key] = n_taps
-                tap_rows.append(t)
-                n_taps += t.shape[0]
-            return taps[key]
-
         for b, d in enumerate(draws):
             tiles, canvas, lbox = sample_layout(d, shapes, s)
             S = samples[b]
@@ -448,25 +437,19 @@ class Augment:
                 T.rgb, T.ir = ops._addr(frames[idx][0]), ops._addr(frames[idx][1])
                 T.H0, T.W0, T.h, T.w = H0, W0, h, w
                 T.x1a, T.y1a, T.x2a, T.y2a, T.x1b, T.y1b = x1a, y1a, x2a, y2a, x1b, y1b
-                if (h, w) != (H0, W0):
-                    T.xtab, T.ytab = tap(W0, w, False), tap(H0, h, True)
+                if (h, w) != (H0, W0):                # offsets in int4 rows: every resize_taps row is 4 words
+                    T.xtab = block.table((W0, w, False), lambda: resize_taps(W0, w)) // 4
+                    T.ytab = block.table((H0, h, True), lambda: resize_taps(H0, h, vertical=True)) // 4
             lut = np.stack([hsv_luts(g) for g in d.gains])
             C.memmove(C.addressof(S.lut), lut.ctypes.data, lut.nbytes)
             if d.mosaic:
                 warp[b] = warp_tables(d.M, s)
             per_labels.append(sample_labels(d, self.labels, tiles, lbox, s))
+        n_taps = block.n_words // 4
         nbytes = int(_lib.lib().icaf_augment_params_bytes(B, s, n_taps))
         if nbytes == 0:
             raise ValueError(f"augment: unsupported batch {B} / size {s}")
-        blob = torch.zeros(nbytes, dtype=torch.uint8, pin_memory=not ops.dry_running())
-        bn = blob.numpy()
-        off_warp = (C.sizeof(samples) + 15) // 16 * 16
-        bn[:C.sizeof(samples)] = np.frombuffer(samples, dtype=np.uint8)
-        bn[off_warp:off_warp + warp.nbytes] = warp.view(np.uint8).reshape(-1)
-        if tap_rows:
-            t = np.concatenate(tap_rows).astype(np.int32)
-            bn[off_warp + warp.nbytes:off_warp + warp.nbytes + t.nbytes] = t.view(np.uint8).reshape(-1)
-        params = blob.to(self.device, non_blocking=True)
+        params = block.upload(samples, (warp,), nbytes, self.device)
         self.params = params                         # the latest batch's parameter block (re-launched by scripts/augment_times.py)
         targets = torch.from_numpy(collate_targets(per_labels)).to(self.device, non_blocking=True)
         if out is None:

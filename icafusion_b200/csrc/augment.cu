@@ -7,11 +7,10 @@
 //   augment_hsv: BGR->HSV with cv2's integer tables (hsv_shift 12), the three LUTs, HSV->BGR in float32 as cv2's
 //     vectorised path computes it (the two inner products fused, result x 255 truncated);
 //   flipud / fliplr (output index only), BGR->RGB, HWC->CHW.
-#include "icaf_internal.cuh"
+#include "staging.cuh"
 
 namespace icaf {
 
-constexpr int kAugPad = 114;
 constexpr int kAugThreads = 256;
 
 struct AugmentParams {
@@ -24,25 +23,10 @@ struct AugmentParams {
 __device__ __forceinline__ void tile_pixel(const icaf_aug_tile& T, const int4* __restrict__ taps, int tx, int ty, int (&v)[6]) {
   const unsigned char* fr[2] = {static_cast<const unsigned char*>(T.rgb), static_cast<const unsigned char*>(T.ir)};
   if (T.h == T.H0 && T.w == T.W0) {
-#pragma unroll
-    for (int m = 0; m < 2; ++m) {
-      const unsigned char* p = fr[m] + ((long long)ty * T.W0 + tx) * 3;
-      v[3 * m] = p[0]; v[3 * m + 1] = p[1]; v[3 * m + 2] = p[2];
-    }
+    copy_pixel(fr, T.W0, tx, ty, v);
     return;
   }
-  const int4 cx = taps[T.xtab + tx], cy = taps[T.ytab + ty];
-#pragma unroll
-  for (int m = 0; m < 2; ++m) {
-    const unsigned char* r0 = fr[m] + (long long)cy.x * T.W0 * 3;
-    const unsigned char* r1 = fr[m] + (long long)cy.y * T.W0 * 3;
-#pragma unroll
-    for (int c = 0; c < 3; ++c) {
-      const int h0 = r0[cx.x * 3 + c] * cx.z + r0[cx.y * 3 + c] * cx.w;
-      const int h1 = r1[cx.x * 3 + c] * cx.z + r1[cx.y * 3 + c] * cx.w;
-      v[3 * m + c] = (((cy.z * (h0 >> 4)) >> 16) + ((cy.w * (h1 >> 4)) >> 16) + 2) >> 2;
-    }
-  }
+  linear_pixel(fr, T.W0, taps[T.xtab + tx], taps[T.ytab + ty], v);
 }
 
 // Canvas pixel (cx, cy): the last tile placed over it, or the 114 background (also outside the canvas).
@@ -57,7 +41,7 @@ __device__ __forceinline__ void canvas_pixel(const icaf_aug_sample& S, const int
     }
   }
 #pragma unroll
-  for (int c = 0; c < 6; ++c) v[c] = kAugPad;
+  for (int c = 0; c < 6; ++c) v[c] = kStagePad;
 }
 
 // cv2 COLOR_BGR2HSV (uint8, hrange 180) -> LUT -> COLOR_HSV2BGR, in place on (b, g, r).
@@ -136,12 +120,9 @@ __global__ void __launch_bounds__(kAugThreads) augment_kernel(const AugmentParam
   for (int m = 0; m < 2; ++m) {
     int bb = v[3 * m], gg = v[3 * m + 1], rr = v[3 * m + 2];
     hsv_jitter(bb, gg, rr, &S.lut[m][0][0], sdiv, hdiv);
-    unsigned char* d = outs[m] + (long long)b * 3 * plane + p;   // planar RGB: channel 0 = R
-    d[0] = (unsigned char)rr; d[plane] = (unsigned char)gg; d[2 * plane] = (unsigned char)bb;
+    store_planar_rgb(outs[m] + (long long)b * 3 * plane + p, plane, bb, gg, rr);
   }
 }
-
-static size_t align16(size_t n) { return (n + 15) & ~size_t(15); }
 
 }  // namespace icaf
 

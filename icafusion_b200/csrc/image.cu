@@ -1,6 +1,6 @@
 // Image staging of the inference path: planar input frames -> the fp16 NHWC image the stem convolution reads (plain or
 // space-to-depth), and the letterbox resize of uint8 frames.
-#include "icaf_internal.cuh"
+#include "staging.cuh"
 
 namespace icaf {
 
@@ -46,9 +46,8 @@ __global__ void pack_image_s2d_kernel(const T* __restrict__ src, float scale, in
 }
 
 // ------------------------------------------------------------------------------------------------
-// Letterbox (utils/datasets.py:1404-1427) + BGR->RGB + HWC->CHW (datasets.py:238) for a batch of frames:
-// cv2.resize(INTER_LINEAR) on uint8 is fixed-point -- horizontal taps a0, a1 (x 2048, from the host-built tables), vertical
-// dst = (((b0 * (r0 >> 4)) >> 16) + ((b1 * (r1 >> 4)) >> 16) + 2) >> 2 -- reproduced bit for bit; the border is `pad`.
+// Letterbox (utils/datasets.py:1404-1427) + BGR->RGB + HWC->CHW (datasets.py:238) for a batch of frames: the frame, copied or
+// through cv2.resize(INTER_LINEAR) (staging.cuh, host-built tables), at (top, left); the border is `pad`.
 struct LetterboxParams {
   const unsigned char* src; unsigned char* dst;
   const int* xtab; const int* ytab;     // [new_w][4] = {x0, x1, a0, a1}, [new_h][4] = {y0, y1, b0, b1}; NULL = no resize
@@ -64,37 +63,21 @@ __global__ void letterbox_kernel(const LetterboxParams P) {
   const long long r = i - b * hw;
   const int y = int(r / P.W), x = int(r - (long long)y * P.W);
   const int yy = y - P.top, xx = x - P.left;
-  int v0 = P.pad, v1 = P.pad, v2 = P.pad;               // B, G, R of the source order
+  int v[3] = {P.pad, P.pad, P.pad};                     // B, G, R of the source order
   if (yy >= 0 && yy < P.new_h && xx >= 0 && xx < P.new_w) {
     const unsigned char* S = P.src + (long long)b * P.H0 * P.W0 * 3;
-    if (!P.xtab) {
-      const unsigned char* s = S + ((long long)yy * P.W0 + xx) * 3;
-      v0 = s[0]; v1 = s[1]; v2 = s[2];
-    } else {
-      const int4 tx = reinterpret_cast<const int4*>(P.xtab)[xx], ty = reinterpret_cast<const int4*>(P.ytab)[yy];
-      const unsigned char* r0 = S + (long long)ty.x * P.W0 * 3;
-      const unsigned char* r1 = S + (long long)ty.y * P.W0 * 3;
-      int out[3];
-#pragma unroll
-      for (int c = 0; c < 3; ++c) {
-        const int h0 = r0[tx.x * 3 + c] * tx.z + r0[tx.y * 3 + c] * tx.w;
-        const int h1 = r1[tx.x * 3 + c] * tx.z + r1[tx.y * 3 + c] * tx.w;
-        out[c] = (((ty.z * (h0 >> 4)) >> 16) + ((ty.w * (h1 >> 4)) >> 16) + 2) >> 2;
-      }
-      v0 = out[0]; v1 = out[1]; v2 = out[2];
-    }
+    if (!P.xtab) copy_pixel(S, P.W0, xx, yy, v);
+    else linear_pixel(S, P.W0, reinterpret_cast<const int4*>(P.xtab)[xx], reinterpret_cast<const int4*>(P.ytab)[yy], v);
   }
-  unsigned char* d = P.dst + (long long)b * 3 * hw + r;  // planar RGB: channel 0 = R = source channel 2
-  d[0] = (unsigned char)v2; d[hw] = (unsigned char)v1; d[2 * hw] = (unsigned char)v0;
+  store_planar_rgb(P.dst + (long long)b * 3 * hw + r, hw, v[0], v[1], v[2]);
 }
 
 // ------------------------------------------------------------------------------------------------
 // Validation batch staging (utils/datasets.py:948-1024, augment=False, rect=True): one thread per 4 adjacent output pixels of
 // one sample, both frames; each of the 6 output planes gets one 32-bit store.  A pixel inside the load_image rectangle is
-// cv2.resize of the decoded frame -- copy, INTER_LINEAR (the letterbox arithmetic above) or INTER_AREA (resizeAreaFast's
-// block sums, or resizeArea_'s float taps with every product and sum rounded in cv2's order) -- and 114 outside it.
+// cv2.resize of the decoded frame -- copy, INTER_LINEAR (staging.cuh) or INTER_AREA (resizeAreaFast's block sums, or
+// resizeArea_'s float taps with every product and sum rounded in cv2's order) -- and 114 outside it.
 constexpr int kValThreads = 256;
-constexpr int kValPad = 114;
 
 struct ValStageParams {
   const icaf_val_sample* samples; const int* tab;
@@ -109,24 +92,9 @@ __device__ __forceinline__ void val_pixel(const icaf_val_sample& S, const int* _
   const unsigned char* fr[2] = {static_cast<const unsigned char*>(S.rgb), static_cast<const unsigned char*>(S.ir)};
   const long long row = (long long)S.W0 * 3;
   if (S.mode == ICAF_VAL_COPY) {
-#pragma unroll
-    for (int m = 0; m < 2; ++m) {
-      const unsigned char* p = fr[m] + y * row + x * 3;
-      v[3 * m] = p[0]; v[3 * m + 1] = p[1]; v[3 * m + 2] = p[2];
-    }
+    copy_pixel(fr, S.W0, x, y, v);
   } else if (S.mode == ICAF_VAL_LINEAR) {
-    const int4 tx = reinterpret_cast<const int4*>(tab + S.xtab)[x], ty = reinterpret_cast<const int4*>(tab + S.ytab)[y];
-#pragma unroll
-    for (int m = 0; m < 2; ++m) {
-      const unsigned char* r0 = fr[m] + ty.x * row;
-      const unsigned char* r1 = fr[m] + ty.y * row;
-#pragma unroll
-      for (int c = 0; c < 3; ++c) {
-        const int h0 = r0[tx.x * 3 + c] * tx.z + r0[tx.y * 3 + c] * tx.w;
-        const int h1 = r1[tx.x * 3 + c] * tx.z + r1[tx.y * 3 + c] * tx.w;
-        v[3 * m + c] = (((ty.z * (h0 >> 4)) >> 16) + ((ty.w * (h1 >> 4)) >> 16) + 2) >> 2;
-      }
-    }
+    linear_pixel(fr, S.W0, reinterpret_cast<const int4*>(tab + S.xtab)[x], reinterpret_cast<const int4*>(tab + S.ytab)[y], v);
   } else if (S.mode == ICAF_VAL_AREA_FAST) {
     int sum[6] = {0, 0, 0, 0, 0, 0};
     for (int dy = 0; dy < S.sy; ++dy)
@@ -185,7 +153,7 @@ __global__ void __launch_bounds__(kValThreads) val_stage_kernel(const ValStagePa
 #pragma unroll
   for (int i = 0; i < 4; ++i) {
     const int xx = x0 + i - S.left;
-    int v[6] = {kValPad, kValPad, kValPad, kValPad, kValPad, kValPad};
+    int v[6] = {kStagePad, kStagePad, kStagePad, kStagePad, kStagePad, kStagePad};
     if (yy >= 0 && yy < S.h && xx >= 0 && xx < S.w) val_pixel(S, P.tab, xx, yy, v);
 #pragma unroll
     for (int m = 0; m < 2; ++m) {                           // planar RGB: channel 0 = R = source channel 2
@@ -199,8 +167,6 @@ __global__ void __launch_bounds__(kValThreads) val_stage_kernel(const ValStagePa
 #pragma unroll
   for (int c = 0; c < 6; ++c) d[c * (plane >> 2)] = word[c];
 }
-
-static size_t val_align16(size_t n) { return (n + 15) & ~size_t(15); }
 
 }  // namespace icaf
 
@@ -249,7 +215,7 @@ extern "C" int icaf_letterbox(const void* src, int B, int H0, int W0, void* dst,
 
 extern "C" size_t icaf_val_stage_params_bytes(int B, int n_words) {
   if (B < 1 || B > 65535 || n_words < 0 || (n_words & 3)) return 0;
-  return val_align16((size_t)B * sizeof(icaf_val_sample)) + (size_t)n_words * sizeof(int);
+  return align16((size_t)B * sizeof(icaf_val_sample)) + (size_t)n_words * sizeof(int);
 }
 
 extern "C" int icaf_val_stage(const void* params, size_t params_bytes, int B, int H, int W, int n_words, void* out, void* stream) {
@@ -261,7 +227,7 @@ extern "C" int icaf_val_stage(const void* params, size_t params_bytes, int B, in
     return set_error(ICAF_ERR_BAD_ARG, "val_stage: parameter block not 16-byte aligned or output not 4-byte aligned");
   ValStageParams P;
   P.samples = static_cast<const icaf_val_sample*>(params);
-  P.tab = reinterpret_cast<const int*>(static_cast<const char*>(params) + val_align16((size_t)B * sizeof(icaf_val_sample)));
+  P.tab = reinterpret_cast<const int*>(static_cast<const char*>(params) + align16((size_t)B * sizeof(icaf_val_sample)));
   P.out = static_cast<unsigned char*>(out);
   P.H = H; P.W = W;
   const dim3 grid(blocks_for((long long)H * (W / 4), kValThreads), (unsigned)B);

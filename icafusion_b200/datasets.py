@@ -7,6 +7,7 @@ its tap tables are rebuilt on the host by :func:`resize_taps`).  The result is t
 staging kernel (/255 -> fp16, space-to-depth) consumes."""
 from __future__ import annotations
 
+import ctypes as C
 import functools
 from typing import Callable, Sequence, Tuple
 
@@ -39,6 +40,42 @@ def resize_taps(src: int, dst: int, vertical: bool = False) -> np.ndarray:
     i1 = np.clip(i0 + 1, 0, src - 1).astype(np.int32)
     i0 = np.clip(i0, 0, src - 1).astype(np.int32)
     return np.ascontiguousarray(np.stack([i0, i1, w0, w1], 1).astype(np.int32))
+
+
+def _align16(n: int) -> int:
+    return (n + 15) // 16 * 16
+
+
+class ParamBlock:
+    """The parameter block of one staging launch (icaf_val_stage, icaf_augment): a ctypes struct array at 0, then int32
+    regions, each 16-byte aligned; the last region holds the resize tables, interned by key."""
+
+    def __init__(self):
+        self.offsets, self.tables, self.n_words = {}, [], 0
+
+    def table(self, key, make: Callable[[], np.ndarray]) -> int:
+        """Offset in int32 words of the table `key` in the table region; make() builds it on the key's first use.  Every
+        table starts 16-byte aligned."""
+        if key not in self.offsets:
+            t = np.asarray(make(), dtype=np.int32).reshape(-1)
+            self.offsets[key] = self.n_words
+            self.tables.append(np.pad(t, (0, -t.size % 4)))
+            self.n_words += self.tables[-1].size
+        return self.offsets[key]
+
+    def upload(self, structs, regions: Sequence[np.ndarray], nbytes: int, device) -> torch.Tensor:
+        """The block on `device`: structs, then `regions` and the table region, assembled in a pinned buffer (plain host
+        memory in a dry run) of nbytes, the size the library computes for this layout."""
+        blob = torch.zeros(nbytes, dtype=torch.uint8, pin_memory=not ops.dry_running())
+        bn = blob.numpy()
+        bn[:C.sizeof(structs)] = np.frombuffer(structs, dtype=np.uint8)
+        off = _align16(C.sizeof(structs))
+        for r in (*regions, *self.tables):
+            bn[off:off + r.nbytes] = r.view(np.uint8).reshape(-1)
+            off = _align16(off + r.nbytes)
+        if off != nbytes:
+            raise ValueError(f"parameter block: the layout takes {off} bytes, the library expects {nbytes}")
+        return blob.to(device, non_blocking=True)
 
 
 _TAPS_ON_DEVICE = {}

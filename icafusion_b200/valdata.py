@@ -23,7 +23,6 @@ a geometry that would need it raises NotImplementedError.  Decoding stays with t
 scripts/val_loader_times.py)."""
 from __future__ import annotations
 
-import ctypes as C
 import functools
 import math
 import time
@@ -34,7 +33,7 @@ import torch
 
 from . import _lib, ops
 from .augment import load_size, resize_fixed, xywhn2xyxy, xyxy2xywh
-from .datasets import frames_on_device, letterbox_geometry, resize_taps
+from .datasets import ParamBlock, frames_on_device, letterbox_geometry, resize_taps
 
 PAD = 114
 MODE_COPY, MODE_LINEAR, MODE_AREA_FAST, MODE_AREA = 0, 1, 2, 3
@@ -263,19 +262,7 @@ class ValBatches:
         H, W = (int(v) for v in self.shape_of[ks[0]])
         frames = frames_on_device(self.frames, idx, self.device, "val")
         samples = (_lib.ValSample * B)()
-        tables, words, n_words = {}, [], 0
-
-        def table(key, make):
-            nonlocal n_words
-            if key not in tables:
-                t = make()
-                tables[key] = n_words
-                words.append(t)
-                n_words += (t.size + 3) // 4 * 4          # every table starts 16-byte aligned
-                if t.size % 4:
-                    words.append(np.zeros(4 - t.size % 4, np.int32))
-            return tables[key]
-
+        block = ParamBlock()
         per_labels, shapes = [], []
         for b, (k, i) in enumerate(zip(ks, idx)):
             h0, w0 = self.hw0[i]
@@ -288,24 +275,18 @@ class ValBatches:
             S.rgb, S.ir = ops._addr(rgb), ops._addr(ir)
             S.H0, S.W0, S.h, S.w, S.top, S.left, S.mode, S.sx, S.sy = h0, w0, h, w, top, left, mode, sx, sy
             if mode == MODE_LINEAR:
-                S.xtab = table(("linear", w0, w, False), lambda: resize_taps(w0, w).reshape(-1))
-                S.ytab = table(("linear", h0, h, True), lambda: resize_taps(h0, h, vertical=True).reshape(-1))
+                S.xtab = block.table(("linear", w0, w, False), lambda: resize_taps(w0, w))
+                S.ytab = block.table(("linear", h0, h, True), lambda: resize_taps(h0, h, vertical=True))
             elif mode == MODE_AREA:
-                S.xtab = table(("area", w0, w), lambda: area_table_words(w0, w))
-                S.ytab = table(("area", h0, h), lambda: area_table_words(h0, h))
+                S.xtab = block.table(("area", w0, w), lambda: area_table_words(w0, w))
+                S.ytab = block.table(("area", h0, h), lambda: area_table_words(h0, h))
             per_labels.append(sample_labels(self.labels[i], h, w, ratio, pad, H, W))
             shapes.append(((h0, w0), ((h / h0, w / w0), pad)))
+        n_words = block.n_words
         nbytes = int(_lib.lib().icaf_val_stage_params_bytes(B, n_words))
         if nbytes == 0:
             raise ValueError(f"val: unsupported batch {B} / {n_words} table words")
-        blob = torch.zeros(nbytes, dtype=torch.uint8, pin_memory=not ops.dry_running())
-        bn = blob.numpy()
-        bn[:C.sizeof(samples)] = np.frombuffer(samples, dtype=np.uint8)
-        if words:
-            off = (C.sizeof(samples) + 15) // 16 * 16
-            t = np.concatenate(words).astype(np.int32).view(np.uint8)
-            bn[off:off + t.size] = t
-        params = blob.to(self.device, non_blocking=True)
+        params = block.upload(samples, (), nbytes, self.device)
         self.params = params                         # the latest batch's parameter block (re-launched by scripts/val_loader_times.py)
         targets = collate(per_labels)
         if not ops.dry_running():
