@@ -87,9 +87,10 @@ def walk_config(c: Config):
 
 # ---------------------------------------------------------------------------------------------------------------
 # Dedupe key
-# Arguments that are not geometry: the dropout probability and mask seed of the training attention.  The census replays
-# those launches at p = 0 (a plain reference cannot reproduce a counter-based mask), so they are left out of the key.  The
-# mask seed of the element-wise dropout is drawn per call: keying it would make two walks of one configuration differ.
+# Arguments that are not geometry: the dropout probability and mask seed of the training attention, and the mask seed of the
+# element-wise dropout.  The replay chooses them itself: each dropout record is replayed at p = 0 and at its recorded p, with
+# a seed from its key, against the mask restated on the host (tests/dropout_mask.py).  A seed is drawn per call, so keying
+# it would also make two walks of one configuration differ.
 _NOT_KEYED = {"icaf_cross_attention_train": (9, 10), "icaf_cross_attention_bwd": (13, 14), "icaf_eltwise": (6,)}
 
 
@@ -596,23 +597,28 @@ def _dot(rec, R: Operands) -> List[Check]:
             Check("dot repeat", out2, out, 0.0, "exact")]
 
 
-def _attn_ref(q_src, kv_src, N, Cc, h):
-    """One direction of the cross-attention (common.py:670-684) in fp32: queries of one modality on the other's keys/values."""
+def _attn_ref(q_src, kv_src, N, Cc, h, mask=None, p=0.0):
+    """One direction of the cross-attention (common.py:670-684) in fp32: queries of one modality on the other's keys/values;
+    mask (B * h, N, N) = kept probabilities of the dropout with probability p."""
     B = q_src.shape[0]
     d = Cc // h
     q = q_src[:, :N, :Cc].reshape(B, N, h, d).permute(0, 2, 1, 3)
     k = kv_src[:, :N, Cc:2 * Cc].reshape(B, N, h, d).permute(0, 2, 1, 3)
     v = kv_src[:, :N, 2 * Cc:].reshape(B, N, h, d).permute(0, 2, 1, 3)
     att = torch.softmax(q @ k.transpose(-1, -2) / d ** 0.5, -1)
+    if mask is not None:
+        att = att * mask.view(B, h, N, N) / (1 - p)
     return (att @ v).permute(0, 2, 1, 3).reshape(B, N, Cc)
 
 
-def _attn_checks(out_v, out_i, qv, qi, N, Cc, h, tol):
-    ref_v = lambda: _attn_ref(qi.float(), qv.float(), N, Cc, h)      # noqa: E731  RGB output: IR queries on RGB keys / values
-    ref_i = lambda: _attn_ref(qv.float(), qi.float(), N, Cc, h)      # noqa: E731
-    checks = [Check("out_vis", lambda: out_v[:, :N], ref_v, tol), Check("out_ir", lambda: out_i[:, :N], ref_i, tol)]
+def _attn_checks(out_v, out_i, qv, qi, N, Cc, h, tol, mask=None, p=0.0, tag=""):
+    """mask: lazy (2, B * h, N, N) keep mask, direction 0 the RGB output."""
+    m = (lambda dir: mask()[dir]) if mask is not None else (lambda dir: None)      # noqa: E731
+    ref_v = lambda: _attn_ref(qi.float(), qv.float(), N, Cc, h, m(0), p)      # noqa: E731  RGB output: IR queries on RGB keys / values
+    ref_i = lambda: _attn_ref(qv.float(), qi.float(), N, Cc, h, m(1), p)      # noqa: E731
+    checks = [Check(tag + "out_vis", lambda: out_v[:, :N], ref_v, tol), Check(tag + "out_ir", lambda: out_i[:, :N], ref_i, tol)]
     if out_v.shape[1] > N:
-        checks.append(_zero("pad rows", lambda: torch.cat([out_v[:, N:], out_i[:, N:]])))
+        checks.append(_zero(tag + "pad rows", lambda: torch.cat([out_v[:, N:], out_i[:, N:]])))
     return checks
 
 
@@ -628,35 +634,101 @@ def _attention(rec, R: Operands) -> List[Check]:
     return [] if R.meta else _attn_checks(out_v, out_i, qv, qi, N, Cc, h, 1e-3)
 
 
+def _attn_mask(R: Operands, B, h, N, p):
+    """Lazy keep mask of a replay at dropout probability p, seeded by the replay's own seed."""
+    from dropout_mask import attn_keep_mask
+    return functools.lru_cache(None)(lambda: attn_keep_mask(R.seed, 0, B, h, N, p, R.dev))
+
+
 def _attention_train(rec, R: Operands) -> List[Check]:
+    """At p = 0 (the inference kernel) and, for a dropout record, at its recorded p (the dropout instantiation)."""
     _, args, _ = rec
-    B, N, n_pad, Cc, h = args[4:9]
+    B, N, n_pad, Cc, h, p = args[4:10]
     qv, qi = _qkv(R, B, n_pad, Cc)
     out_v, out_i = ops.cross_attention_train(qv, qi, B, N, n_pad, Cc, h, 0.0, 0)
-    return [] if R.meta else _attn_checks(out_v, out_i, qv, qi, N, Cc, h, 1e-3)
-
-
-def _attention_bwd(rec, R: Operands) -> List[Check]:
-    _, args, _ = rec
-    B, N, n_pad, Cc, h = args[8:13]
-    qv, qi = _qkv(R, B, n_pad, Cc)
-    out_v, out_i = (R.randn(B, n_pad, Cc) for _ in range(2)) if R.meta else ops.cross_attention_train(qv, qi, B, N, n_pad, Cc, h)
-    dov, doi = R.randn(B, n_pad, Cc, scale=0.1), R.randn(B, n_pad, Cc, scale=0.1)
-    dq_v, dq_i = ops.cross_attention_bwd(qv, qi, out_v, out_i, dov, doi, B, N, n_pad, Cc, h, 0.0, 0)
+    if p > 0:
+        dv, di = ops.cross_attention_train(qv, qi, B, N, n_pad, Cc, h, p, R.seed)
+        dv2, di2 = ops.cross_attention_train(qv, qi, B, N, n_pad, Cc, h, p, R.seed)
     if R.meta:
         return []
+    checks = _attn_checks(out_v, out_i, qv, qi, N, Cc, h, 1e-3)
+    if p > 0:
+        checks += _attn_checks(dv, di, qv, qi, N, Cc, h, 1.5e-3, _attn_mask(R, B, h, N, p), p, f"p {p:g}: ")
+        checks += [Check(f"p {p:g}: out_vis repeat", dv2, dv, 0.0, "exact"), Check(f"p {p:g}: out_ir repeat", di2, di, 0.0, "exact")]
+    return checks
+
+
+def _attention_bwd_case(qv, qi, dov, doi, B, N, n_pad, Cc, h, p, R: Operands) -> List[Check]:
+    seed = R.seed if p > 0 else 0
+    if R.meta:
+        out_v, out_i = (R.randn(B, n_pad, Cc) for _ in range(2))
+    else:
+        out_v, out_i = ops.cross_attention_train(qv, qi, B, N, n_pad, Cc, h, p, seed)
+    dq_v, dq_i = ops.cross_attention_bwd(qv, qi, out_v, out_i, dov, doi, B, N, n_pad, Cc, h, p, seed)
+    if p > 0:
+        dq_v2, dq_i2 = ops.cross_attention_bwd(qv, qi, out_v, out_i, dov, doi, B, N, n_pad, Cc, h, p, seed)
+    if R.meta:
+        return []
+    mask = _attn_mask(R, B, h, N, p) if p > 0 else None
 
     @functools.lru_cache(None)
     def ref():
         rv, ri = qv.float().requires_grad_(True), qi.float().requires_grad_(True)
-        (_attn_ref(ri, rv, N, Cc, h) * dov[:, :N].float()).sum().backward(retain_graph=True)
-        (_attn_ref(rv, ri, N, Cc, h) * doi[:, :N].float()).sum().backward()
+        m = (lambda dir: mask()[dir]) if mask is not None else (lambda dir: None)      # noqa: E731
+        (_attn_ref(ri, rv, N, Cc, h, m(0), p) * dov[:, :N].float()).sum().backward(retain_graph=True)
+        (_attn_ref(rv, ri, N, Cc, h, m(1), p) * doi[:, :N].float()).sum().backward()
         return rv.grad[:, :N], ri.grad[:, :N]
-    checks = [Check("dqkv_vis", lambda: dq_v[:, :N], lambda: ref()[0], 2e-3), Check("dqkv_ir", lambda: dq_i[:, :N], lambda: ref()[1], 2e-3)]
+    tag = f"p {p:g}: " if p > 0 else ""
+    checks = [Check(tag + "dqkv_vis", lambda: dq_v[:, :N], lambda: ref()[0], 2e-3),
+              Check(tag + "dqkv_ir", lambda: dq_i[:, :N], lambda: ref()[1], 2e-3)]
     if n_pad > N:
         pad = lambda: torch.cat([dq_v[:, N:], dq_i[:, N:]])      # noqa: E731
-        checks.append(_zero("pad rows", pad))
+        checks.append(_zero(tag + "pad rows", pad))
+    if p > 0:
+        checks += [Check(tag + "dqkv_vis repeat", dq_v2, dq_v, 0.0, "exact"), Check(tag + "dqkv_ir repeat", dq_i2, dq_i, 0.0, "exact")]
     return checks
+
+
+def _attention_bwd(rec, R: Operands) -> List[Check]:
+    """At p = 0 and, for a dropout record, at its recorded p; each on the forward output of the same p and seed."""
+    _, args, _ = rec
+    B, N, n_pad, Cc, h, p = args[8:14]
+    qv, qi = _qkv(R, B, n_pad, Cc)
+    dov, doi = R.randn(B, n_pad, Cc, scale=0.1), R.randn(B, n_pad, Cc, scale=0.1)
+    checks = _attention_bwd_case(qv, qi, dov, doi, B, N, n_pad, Cc, h, 0.0, R)
+    if p > 0:
+        checks += _attention_bwd_case(qv, qi, dov, doi, B, N, n_pad, Cc, h, p, R)
+    return checks
+
+
+ELTWISE_GUARD = 8          # NaN elements on each side of the output: a write past either end fails the check
+
+
+def _eltwise(rec, R: Operands) -> List[Check]:
+    """Mode 0 (GELU) against F.gelu and mode 1 (its gradient) against autograd, in fp32; mode 2 (dropout) bit-exact against
+    the mask restated on the host: fp16(fp32(x) / (1 - fp32(p))) where kept, 0 where dropped."""
+    _, args, _ = rec
+    mode, n, p = args[0], args[4], args[5]
+    x = R.randn(n, scale=2.0)
+    dy = R.randn(n, scale=0.1) if mode == 1 else None
+    ybuf = R.nan(n + 2 * ELTWISE_GUARD)
+    y = ybuf[ELTWISE_GUARD:ELTWISE_GUARD + n]
+    ops._call("icaf_eltwise", _lib.lib().icaf_eltwise,
+              (mode, ops._ptr(x), ops._ptr(dy), ops._ptr(y), n, p, C.c_uint32(R.seed)), {})
+    if R.meta:
+        return []
+    guard = lambda: torch.cat([ybuf[:ELTWISE_GUARD], ybuf[ELTWISE_GUARD + n:]])      # noqa: E731
+    checks = [Check("y neighbours unchanged", guard, lambda: R.nan(2 * ELTWISE_GUARD), 0.0, "exact")]
+    if mode == 0:
+        return checks + [Check("gelu", y, lambda: F.gelu(x.float()), 1e-3)]
+    if mode == 1:
+        def ref():
+            xr = x.float().requires_grad_(True)
+            F.gelu(xr).backward(dy.float())
+            return xr.grad
+        return checks + [Check("gelu'", y, ref, 1e-3)]
+    from dropout_mask import eltwise_dropout, eltwise_keep
+    return checks + [Check(f"dropout p {p:g}", y, lambda: eltwise_dropout(x, eltwise_keep(n, R.seed, 0, p, R.dev), p), 0.0, "exact")]
 
 
 def _pool_window(H, W, nh, nw):
@@ -1024,12 +1096,12 @@ REPLAYED = {
     "icaf_dmff_upsample_cat_bwd": _upsample_cat_bwd,
     "icaf_sppf_pool": _sppf,
     "icaf_maxpool5_bwd": _maxpool5_bwd,
+    "icaf_eltwise": _eltwise,
 }
 
 _ELEMENTWISE = "pure element-wise kernel with no shape-dependent plan"
 NOT_REPLAYED = {
     "icaf_axpby": _ELEMENTWISE,
-    "icaf_eltwise": _ELEMENTWISE,
     "icaf_copy_channels": _ELEMENTWISE,
     "icaf_upsample2x": _ELEMENTWISE,
     "icaf_upsample2x_bwd": _ELEMENTWISE,

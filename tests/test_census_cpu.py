@@ -74,11 +74,15 @@ def test_census_covers_every_conv_plan_family(records):
     assert {2, 3, 4, 5, 6, 8} <= set(splits)
 
 
+DROPOUT_P = {"icaf_cross_attention_train": 9, "icaf_cross_attention_bwd": 13, "icaf_eltwise": 5}     # argument index of p
+
+
 def test_builders_reissue_the_recorded_launch(records):
     """Each builder, run on meta tensors under a dry run, issues a call with the same key as the record it replays: the replay
-    hits the product's geometry, channel pitches, epilogue flags and scales."""
+    hits the product's geometry, channel pitches, epilogue flags and scales.  A dropout record (p > 0) is also replayed at its
+    recorded p, which the key leaves out."""
     from icafusion_b200 import ops
-    done = collections.Counter()
+    done, dropout = collections.Counter(), collections.Counter()
     for k, rec in records.items():
         if k[0] not in census.REPLAYED:
             continue
@@ -87,5 +91,14 @@ def test_builders_reissue_the_recorded_launch(records):
         issued = {census.key(r) for r in dr.records}
         assert k in issued, f"{census.describe(rec)}: the replay issued {sorted(issued, key=str)[:4]}"
         done[k[0]] += 1
+        if k[0] in DROPOUT_P and rec[1][DROPOUT_P[k[0]]] > 0:
+            i = DROPOUT_P[k[0]]
+            ps = {r[1][i] for r in dr.records if census.key(r) == k}
+            assert rec[1][i] in ps, f"{census.describe(rec)}: recorded p {rec[1][i]}, replayed at {sorted(ps)}"
+            dropout[k[0]] += 1
     print("\ndistinct launches replayed per entry point: " + ", ".join(f"{n} {c}" for n, c in sorted(done.items())))
+    print("of which replayed at their dropout probability: " + ", ".join(f"{n} {c}" for n, c in sorted(dropout.items())))
     assert set(done) == set(census.REPLAYED)
+    # training's dropout launches: 36 attention geometries (forward and backward) and 27 element-wise sizes, all at p = 0.1
+    assert dropout == {"icaf_cross_attention_train": 36, "icaf_cross_attention_bwd": 36, "icaf_eltwise": 27}, dropout
+    assert done["icaf_eltwise"] == 81

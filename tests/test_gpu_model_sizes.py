@@ -7,6 +7,7 @@ import numpy as np
 import pytest
 import torch
 
+import dropout_mask as DM
 from conftest import load_golden
 from helpers import err, load_synth
 from oracle import icaf_oracle as O
@@ -76,6 +77,8 @@ def test_cross_attention_dropout_padded(cuda_device, d):
     n = 2 * mask_v.numel()
     keep = float(torch.cat([mask_v, mask_i]).mean())
     assert abs(keep - (1 - p)) < 5 * math.sqrt(p * (1 - p) / n)
+    want = DM.attn_keep_mask(seed, 0, B, h, N, p).view(2, B, h, N, N)
+    assert torch.equal(mask_v.bool(), want[0]) and torch.equal(mask_i.bool(), want[1])
     out_v, out_i = ops.cross_attention_train(qv.to(cuda_device), qi.to(cuda_device), B, N, n_pad, C, h, p, seed)
     torch.cuda.synchronize()
     o_v, o_i = _attn_ref(qi.float(), qv.float(), N, C, h, mask_v, p), _attn_ref(qv.float(), qi.float(), N, C, h, mask_i, p)

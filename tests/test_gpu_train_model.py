@@ -191,33 +191,71 @@ def test_c3_sppf_fusion_block_nodes(cuda_device):
                  lambda m, a, b: A.fusion_block(m, a, b), [rgb, ir], 6e-3)
 
 
-def test_graphed_train_step_equals_eager(cuda_device):
+def test_graphed_train_step_equals_eager(cuda_device, monkeypatch):
     """GraphedTrainStep (forward + loss + backward replayed from a CUDA graph) takes the same optimiser steps as the eager
-    TrainStep: same losses and the same parameters / BatchNorm buffers after three steps on changing batches (dropout off:
-    its masks are keyed by a step counter that the two modes advance differently)."""
-    from icafusion_b200 import Model
+    TrainStep: same losses and the same parameters / BatchNorm buffers after three steps on changing batches, dropout off."""
+    check_graphed_train_step(cuda_device, monkeypatch, dropout=False)
+
+
+def test_graphed_train_step_with_dropout_equals_eager(cuda_device, monkeypatch):
+    """As above with the model's own dropout (p = 0.1).  Both runs draw the same per-site seeds (autograd.manual_seed before
+    each eager step and before the capture), and eager step r runs with the seed offset at r, as graph replay r does after
+    its in-graph increment: the masks then agree only if every replay draws new masks and every kernel adds the offset."""
+    check_graphed_train_step(cuda_device, monkeypatch, dropout=True)
+
+
+def check_graphed_train_step(cuda_device, monkeypatch, dropout: bool):
+    from icafusion_b200 import Model, _lib
+    from icafusion_b200 import autograd as A
     from icafusion_b200.trainer import GraphedTrainStep, TrainStep, dead_parameters
     m, d = load_golden("train_yolov5s_320")
     B, H, W = 2, 320, 320
+    S = 0x5EED
     batches = []
     for s in range(3):
         rgb, ir = synth.synth_images(B, H, W, 100 + s)
         t = torch.from_numpy(synth_targets(8 + s, B, 100 + s))
         batches.append(((rgb * 255).to(torch.uint8).to(cuda_device), (ir * 255).to(torch.uint8).to(cuda_device), t.to(cuda_device)))
+    for k in ("seed", "count"):                        # restored on exit: the mask seed state is process-global
+        monkeypatch.setitem(A._STATE, k, A._STATE[k])
+    capture = GraphedTrainStep._capture
+
+    def seeded_capture(self, graph, pool=None):
+        A.manual_seed(S)
+        return capture(self, graph, pool)
+    monkeypatch.setattr(GraphedTrainStep, "_capture", seeded_capture)
     runs = []
     for graphed in (False, True):
         model = Model("yolov5s_Transfusion_kaist")
         load_synth(model, m["seed"])
         model = model.to(cuda_device).train()
+        n_drop = 0
         for mod in model.modules():
             if isinstance(mod, torch.nn.Dropout):
-                mod.p = 0.0
+                n_drop += mod.p > 0
+                if not dropout:
+                    mod.p = 0.0
+        assert n_drop > 0
         ts = TrainStep(model, None, total_batch_size=B, imgsz=320)
         assert sorted(ts.dead) == sorted(m["dead_params"]) == sorted(dead_parameters(model))
-        step = GraphedTrainStep(ts, B, H, W, 16, cuda_device) if graphed else ts
-        losses = [float(step(*b)[0]) for b in batches]
         if graphed:
-            step.close()
+            step = GraphedTrainStep(ts, B, H, W, 16, cuda_device)
+            try:
+                losses = [float(step(*b)[0]) for b in batches]
+            finally:
+                step.close()
+        else:
+            ctr = torch.zeros(1, dtype=torch.int32, device=cuda_device)
+            _lib.check(_lib.lib().icaf_set_seed_offset(ctr.data_ptr()), "icaf_set_seed_offset")
+            losses = []
+            try:
+                for r, b in enumerate(batches, 1):
+                    A.manual_seed(S)
+                    ctr.fill_(r)
+                    losses.append(float(ts(*b)[0]))
+            finally:
+                torch.cuda.synchronize()
+                _lib.lib().icaf_set_seed_offset(None)
         torch.cuda.synchronize()
         runs.append((losses, {k: v.detach().float().cpu().clone() for k, v in model.state_dict().items()}, float(ts.scaler.get_scale())))
     (l0, s0, sc0), (l1, s1, sc1) = runs

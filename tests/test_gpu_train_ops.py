@@ -4,6 +4,7 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+import dropout_mask as DM
 from helpers import err, nhwc
 
 pytestmark = pytest.mark.gpu
@@ -117,11 +118,14 @@ def test_small_training_kernels(cuda_device):
     mr = m.float().requires_grad_(True)
     F.max_pool2d(mr, 5, 1, 2).backward(d1.float())
     assert err(ops.maxpool5_bwd(nhwc(m).to(cuda_device), nhwc(d1).to(cuda_device)).permute(0, 3, 1, 2), mr.grad) < 1e-3
-    # dropout: keeps ~ (1 - p), scales by 1 / (1 - p), same mask for the same seed
+    # dropout: keeps ~ (1 - p), scales by 1 / (1 - p), same mask for the same seed; bit for bit the restated mask and scale
     ones = torch.ones(1 << 16, dtype=torch.float16, device=cuda_device)
     a, b2, c2 = ops.eltwise(2, ones, p=0.1, seed=7), ops.eltwise(2, ones, p=0.1, seed=7), ops.eltwise(2, ones, p=0.1, seed=8)
     keep = float((a > 0).float().mean())
     assert torch.equal(a, b2) and not torch.equal(a, c2) and abs(keep - 0.9) < 0.01 and abs(float(a.max()) - 1 / 0.9) < 1e-3
+    for y, seed in ((a, 7), (c2, 8)):
+        want = DM.eltwise_dropout(ones, DM.eltwise_keep(ones.numel(), seed, 0, 0.1, cuda_device), 0.1)
+        assert torch.equal(y.view(torch.int16), want.view(torch.int16)), seed
 
 
 def _attn_ref(qkv_q, qkv_kv, N, C, h, mask=None, p=0.0):
@@ -179,6 +183,8 @@ def test_cross_attention_dropout(cuda_device):
     mask_i = (m_i.cpu().reshape(B, N, h, d).permute(0, 2, 1, 3) > 0).float()
     keep = float(torch.cat([mask_v, mask_i]).mean())
     assert abs(keep - (1 - p)) < 0.02 and not torch.equal(mask_v, mask_i)
+    want = DM.attn_keep_mask(seed, 0, B, h, N, p).view(2, B, h, N, N)
+    assert torch.equal(mask_v.bool(), want[0]) and torch.equal(mask_i.bool(), want[1])
     m2, _ = ops.cross_attention_train(pv.to(cuda_device), pi.to(cuda_device), B, N, n_pad, C, h, p, seed + 1)
     assert not torch.equal(m2, m_v)
     dov, doi = (torch.randn(B, n_pad, C, generator=g) * 0.1).half(), (torch.randn(B, n_pad, C, generator=g) * 0.1).half()
