@@ -90,6 +90,8 @@ SIGNATURES = {
     "icaf_nms": [_vp, _i, _i, _i, _f, _f, _i, C.c_uint64, _i, _vp, _vp, _vp, C.c_size_t, _vp],
     "icaf_nms_multi_label_workspace_bytes": [_i, _i, _i],
     "icaf_nms_multi_label": [_vp, _i, _i, _i, _f, _f, _i, C.c_uint64, _i, _vp, _vp, _vp, C.c_size_t, _vp],
+    "icaf_confluence_workspace_bytes": [_i, _i, _i],
+    "icaf_confluence": [_vp, _i, _i, _i, _i, _f, C.c_double, _vp, _vp, _i, _vp, _vp, C.c_size_t, _vp],
     "icaf_match_detections_workspace_bytes": [_i],
     "icaf_match_detections": [_vp, _vp, _i, _i, _vp, _i, _vp, _i, _i, _vp, _i, _i, _vp, _vp, _vp, C.c_size_t, _vp],
     "icaf_kaist_mr_workspace_bytes": [_i, _i, _i],
@@ -153,6 +155,7 @@ def lib() -> C.CDLL:
             fn.restype = {"icaf_last_error": C.c_char_p, "icaf_kernel_launches": C.c_longlong,
                           "icaf_nms_workspace_bytes": C.c_size_t, "icaf_loss_workspace_bytes": C.c_size_t,
                           "icaf_nms_multi_label_workspace_bytes": C.c_size_t,
+                          "icaf_confluence_workspace_bytes": C.c_size_t,
                           "icaf_match_detections_workspace_bytes": C.c_size_t,
                           "icaf_kaist_mr_workspace_bytes": C.c_size_t,
                           "icaf_conv2d_wgrad_workspace_bytes": C.c_size_t, "icaf_train_workspace_bytes": C.c_size_t,

@@ -13,7 +13,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libicaf_b200.so")
 SOURCES = ["api.cu", "conv_gemm.cu", "attn.cu", "image.cu", "pool.cu", "dmff.cu", "nms.cu", "loss.cu", "wgrad.cu", "train.cu",
-           "attn_bwd.cu", "augment.cu", "bottleneck.cu", "metrics.cu"]
+           "attn_bwd.cu", "augment.cu", "bottleneck.cu", "metrics.cu",
+           "confluence.cu"]
 HEADERS = ["ptx.cuh", "icaf_internal.cuh", "conv_common.cuh", "staging.cuh", os.path.join("..", "..", "include", "icaf_b200.h")]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "--use_fast_math=false"]

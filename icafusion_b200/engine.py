@@ -20,13 +20,18 @@ from .yolo_test import Model
 class GraphedDetector:
     def __init__(self, model: Model, batch: int, height: int, width: int, in_dtype: torch.dtype = torch.float16,
                  device: Optional[torch.device] = None, warmup: int = 2, nms: Optional[dict] = None,
-                 frame_hw: Optional[Tuple[int, int]] = None):
+                 frame_hw: Optional[Tuple[int, int]] = None, confluence: Optional[dict] = None):
         """`frame_hw`: (H0, W0) of the raw decoded BGR frames; when given, the device letterbox (utils/datasets.py:1404-1427 +
         the BGR->RGB / HWC->CHW of :238) is captured in front of the forward and ``infer_frames`` takes the raw uint8
         (B, H0, W0, 3) frames -- the whole detect_twostream.py:70-86 loop body as one graph.
         `nms`: keyword arguments of :func:`icafusion_b200.ops.nms` (e.g. ``dict(conf_thres=0.25, iou_thres=0.45)``); when
         given, the batched device NMS (utils/general.py:518-607) is captured behind the forward and ``infer_detections``
-        returns its fixed-capacity result -- the whole detect_twostream.py:84-86 step without a host round trip in between."""
+        returns its fixed-capacity result -- the whole detect_twostream.py:84-86 step without a host round trip in between.
+        `confluence`: keyword arguments of :func:`icafusion_b200.ops.confluence` (e.g. ``dict(conf_thres=0.1, p_thres=0.5)``),
+        the reference's alternative to NMS (utils/confluence.py), captured in its place; its count is the true number kept
+        and may exceed max_det."""
+        if nms is not None and confluence is not None:
+            raise ValueError("GraphedDetector: pass nms= or confluence=, not both")
         if model.training:
             raise ValueError("GraphedDetector needs model.eval()")
         self.model = model
@@ -66,6 +71,12 @@ class GraphedDetector:
                 need = ops.nms_workspace_bytes(*z0.shape, nms.get("multi_label", False))
                 self._nms_ws = torch.empty((need + 7) // 8, dtype=torch.int64, device=self.device)
                 self.stream.synchronize()
+            if confluence is not None:
+                z0 = self.model(self.rgb, self.ir)[0]
+                self._cf_ws = torch.empty((ops.confluence_workspace_bytes(*z0.shape) + 15) // 16, 2, dtype=torch.int64,
+                                          device=self.device)
+                self.det, self.count = ops.confluence(z0, workspace=self._cf_ws, **confluence)
+                self.stream.synchronize()
             self.graph = torch.cuda.CUDAGraph()
             n0 = ops.launch_count()
             with torch.cuda.graph(self.graph, stream=self.stream):
@@ -75,10 +86,12 @@ class GraphedDetector:
                 self.z, self.logits, self.xs = self.model(self.rgb, self.ir)
                 if nms is not None:
                     ops.nms(self.z, det=self.det, count=self.count, workspace=self._nms_ws, **nms)
+                if confluence is not None:
+                    ops.confluence(self.z, det=self.det, count=self.count, workspace=self._cf_ws, **confluence)
             self.launches_per_step = ops.launch_count() - n0
         self.stream.synchronize()
         self._z_host = torch.empty(self.z.shape, dtype=self.z.dtype, pin_memory=True)
-        if nms is not None:
+        if self.det is not None:
             self._det_host = torch.empty(self.det.shape, dtype=self.det.dtype, pin_memory=True)
             self._count_host = torch.empty(self.count.shape, dtype=self.count.dtype, pin_memory=True)
 
@@ -112,7 +125,7 @@ class GraphedDetector:
         """End-to-end step with the captured NMS: H2D, forward, NMS, D2H of the (B, max_det, 6) detections and their counts.
         Returns (det_host fp32, count_host int32), valid until the next call."""
         if self.det is None:
-            raise RuntimeError("GraphedDetector was built without nms=...")
+            raise RuntimeError("GraphedDetector was built without nms=... or confluence=...")
         self(rgb_host, ir_host)
         self._det_host.copy_(self.det, non_blocking=True)
         self._count_host.copy_(self.count, non_blocking=True)

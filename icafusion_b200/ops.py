@@ -642,6 +642,48 @@ def nms(z: torch.Tensor, conf_thres: float = 0.25, iou_thres: float = 0.45, agno
     return det, count
 
 
+def confluence_workspace_bytes(B: int, R: int, no: int) -> int:
+    """Device workspace :func:`confluence` needs for (B, R, no) predictions (no = 5 + the number of classes)."""
+    return int(_lib.lib().icaf_confluence_workspace_bytes(B, R, no))
+
+
+def confluence(z: torch.Tensor, conf_thres: float = 0.1, p_thres: float = 0.6, max_det: int = 300,
+               det: Optional[torch.Tensor] = None, count: Optional[torch.Tensor] = None,
+               workspace: Optional[torch.Tensor] = None, index: Optional[torch.Tensor] = None,
+               class_num: Optional[int] = None):
+    """Batched Confluence on the device (utils/confluence.py:50-193), the reference's alternative to NMS.  z: fp16 or fp32
+    (B, R, nc+5) decoded predictions, read in their own dtype.  Returns (det fp32 (B, max_det, 6) rows
+    [x1,y1,x2,y2,conf,cls] in ascending candidate order, count int32 (B,)): count is the true number kept, and rows past
+    max_det are not written when it is larger.  No host sync.  `workspace` must hold :func:`confluence_workspace_bytes`
+    bytes; `index` (int32 (B, max_det)), when given, receives the row of each written detection.
+    `class_num`: z is instead fp32 detection rows (B, R, 6) [x1,y1,x2,y2,conf,cls], what confluence() takes, clustered
+    per class 0 .. class_num-1 by their own cls and conf, without a threshold."""
+    rows = class_num is not None
+    if z.dim() != 3 or not on_device(z) or not z.is_contiguous() or \
+            (z.dtype != torch.float32 if rows else z.dtype not in (torch.float16, torch.float32)) or (rows and z.shape[2] != 6):
+        raise ValueError(f"confluence: expected a contiguous CUDA {'fp32 (B, R, 6)' if rows else 'fp16 or fp32 (B, R, nc+5)'} "
+                         f"tensor, got {z.dtype} {tuple(z.shape)}")
+    B, R = z.shape[:2]
+    no = int(class_num) + 5 if rows else z.shape[2]
+    if det is None:
+        det = torch.zeros(B, max_det, 6, dtype=torch.float32, device=z.device)
+    if count is None:
+        count = torch.zeros(B, dtype=torch.int32, device=z.device)
+    if workspace is None:
+        workspace = torch.empty((confluence_workspace_bytes(B, R, no) + 15) // 16, 2, dtype=torch.int64, device=z.device)
+    if det.dim() != 3 or (det.shape[0], det.shape[2]) != (B, 6) or det.dtype != torch.float32 or \
+            tuple(count.shape) != (B,) or count.dtype != torch.int32:
+        raise ValueError("confluence: det must be fp32 (B, max_det, 6) and count int32 (B,)")
+    if index is not None and (tuple(index.shape) != tuple(det.shape[:2]) or index.dtype != torch.int32):
+        raise ValueError("confluence: index must be int32 (B, max_det)")
+    dtype = 2 if rows else (0 if z.dtype == torch.float16 else 1)
+    _call("icaf_confluence", _lib.lib().icaf_confluence,
+          (_ptr(z), dtype, B, R, no, float(conf_thres), float(p_thres), _ptr(det), _ptr(index), det.shape[1], _ptr(count),
+           _ptr(workspace), C.c_size_t(workspace.numel() * workspace.element_size())),
+          {"bytes": float(z.numel() * z.element_size())})
+    return det, count
+
+
 def match_detections(det: torch.Tensor, count: torch.Tensor, targets: torch.Tensor, ratio_pad: torch.Tensor, height: int,
                      width: int, iouv: torch.Tensor, single_cls: bool = False, correct: Optional[torch.Tensor] = None,
                      native: Optional[torch.Tensor] = None, workspace: Optional[torch.Tensor] = None):

@@ -276,6 +276,30 @@ int icaf_nms_multi_label(const void* z, int B, int R, int no, float conf_thres, 
                          void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * Confluence on the decoded predictions, fully on the device: the reference's alternative to NMS
+ * (utils/confluence.py:50-193 confluence_process + confluence), clustering by normalised Manhattan distance.
+ * z: (B, R, no) decoded predictions, dtype 0 = fp16 or 1 = fp32 (read as they are: fp32 input is never rounded to fp16).
+ * Candidates: one per (row r, class j) with obj > conf_thres and cls_j * obj > conf_thres in fp32 (for nc == 1 this is the
+ * reference's best-class branch, otherwise its multi_label branch); boxes by xywh2xyxy in fp32.  Per class, in row order,
+ * in fp64 on the widened values: p_ab = sum over x1, x2, y1, y2 of |a' - b'| with each axis normalised by the min and
+ * max of its four coordinates (a degenerate axis gives NaN, which neither counts nor removes); the first box with the
+ * smallest min over p_ij < 2 of p_ij / conf_i (0 without such j) is kept, and it and every box with p < p_thres leave.
+ * det: fp32 (B, max_det, 6) rows [x1, y1, x2, y2, conf, cls] in ascending (row, class) order -- the reference's
+ * np.unique(keep) order; there is no max_det cut in the reference, so count: int32 (B) holds the TRUE number kept per
+ * image, and when it exceeds max_det the rows past max_det were not written (rows at or past the count are untouched).
+ * index: optional int32 (B, max_det), the row r of each written detection (NULL: not written).
+ * dtype 2: z holds fp32 detection rows (B, R, 6) [x1, y1, x2, y2, conf, cls], the input of confluence(): a row belongs to
+ * class j when its cls == j (j < no - 5), there is no threshold (conf_thres is ignored) and every conf must be >= 2.5e-4.
+ * conf_thres must be >= 2.5e-4: below 2e-4 the reference's scan, which starts at 10000, can find no box and raises.
+ * Up to 6144 candidates of one class are clustered in shared memory, more in the workspace (correct at any count, slower).
+ * workspace: icaf_confluence_workspace_bytes(B, R, no) bytes of device memory, 16-byte aligned (37 bytes per row and class
+ * plus 1); R * (no - 5) must fit in int, B <= 65535.  Returns 0 from the size query for a bad shape.
+ * ------------------------------------------------------------------------------------------- */
+size_t icaf_confluence_workspace_bytes(int B, int R, int no);
+int icaf_confluence(const void* z, int dtype, int B, int R, int no, float conf_thres, double p_thres, float* det, int* index,
+                    int max_det, int* count, void* workspace, size_t workspace_bytes, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * Validation: match one batch's NMS detections to its labels (test.py:196-227), one launch, no host round trip.
  * det / count: what icaf_nms / icaf_nms_multi_label write, fp32 (B, max_det, 6) and int32 (B).
  * targets: fp32 (T, 6) rows [image, cls, x, y, w, h] normalised to the (height, width) batch, in any order; rows whose image
