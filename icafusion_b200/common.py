@@ -87,7 +87,9 @@ class Conv(nn.Module):
         self.act = nn.SiLU() if act is True else (act if isinstance(act, nn.Module) else nn.Identity())
 
     # -- packed filter cache -------------------------------------------------------------------
-    def packed(self) -> PackedConv:
+    def packed(self, in_place: bool = False) -> PackedConv:
+        """The BN-folded filter in the kernel's layout, re-packed when a parameter or BN buffer changed.  `in_place`: copy a
+        re-pack into the cached tensors instead of replacing them (engine.refresh_packed_)."""
         conv = self.conv
         bn = getattr(self, "bn", None)
         key = _versions(conv.weight, conv.bias, *( (bn.weight, bn.bias, bn.running_mean, bn.running_var) if bn is not None else ()))
@@ -113,6 +115,8 @@ class Conv(nn.Module):
             pk = ops.pack_stem_weight(w, b, act)          # 6x6/s2/p2 over the image == 3x3/s1/p1 over its space-to-depth form
         else:
             pk = ops.pack_conv_weight(w, b, conv.stride[0], conv.padding[0], act)
+        if in_place and cache is not None:
+            pk = ops.copy_packed_(cache[1], pk)
         self.__dict__["_icaf_pack"] = (key, pk)
         return pk
 
@@ -211,11 +215,12 @@ class C3(nn.Module):
         self.cv3 = Conv(2 * c_, c2, 1)
         self.m = nn.Sequential(*[Bottleneck(c_, c_, shortcut, g, e=1.0) for _ in range(n)])
 
-    def packed_cv12(self) -> PackedConv:
+    def packed_cv12(self, in_place: bool = False) -> PackedConv:
         """cv1 and cv2 read the same input: one GEMM with the two filter banks stacked ([cv1 | cv2] output channels)."""
-        p1, p2 = self.cv1.packed(), self.cv2.packed()
+        p1, p2 = self.cv1.packed(in_place), self.cv2.packed(in_place)
+        keys = (self.cv1.__dict__["_icaf_pack"][0], self.cv2.__dict__["_icaf_pack"][0])    # in-place re-packs keep p1, p2
         cache = self.__dict__.get("_icaf_pack12")
-        if cache is not None and cache[0] is p1 and cache[1] is p2:
+        if cache is not None and cache[0] is p1 and cache[1] is p2 and cache[3] == keys:
             return cache[2]
         c_ = p1.cout
         w = torch.cat([p1.w[:c_], p2.w[:c_]], 0)
@@ -223,7 +228,9 @@ class C3(nn.Module):
         if rows != 2 * c_:
             w = torch.cat([w, w.new_zeros(rows - 2 * c_, w.shape[1])], 0)
         pk = PackedConv(w.contiguous(), torch.cat([p1.bias, p2.bias]).contiguous(), p1.cin, 2 * c_, 1, 1, 1, 0, p1.act)
-        self.__dict__["_icaf_pack12"] = (p1, p2, pk)
+        if in_place and cache is not None:
+            pk = ops.copy_packed_(cache[2], pk)
+        self.__dict__["_icaf_pack12"] = (p1, p2, pk, keys)
         return pk
 
     @staticmethod
@@ -400,7 +407,7 @@ class CrossAttention(nn.Module):
                 nn.init.constant_(m.bias, 0)
 
     # -- packed parameters ---------------------------------------------------------------------
-    def packed(self):
+    def packed(self, in_place: bool = False):
         live = [self.que_proj_vis, self.key_proj_vis, self.val_proj_vis, self.que_proj_ir, self.key_proj_ir, self.val_proj_ir,
                 self.out_proj_vis, self.out_proj_ir, self.LN1, self.LN2]
         key = _versions(*[p for m in live for p in (m.weight, m.bias)])
@@ -416,6 +423,8 @@ class CrossAttention(nn.Module):
             P[f"qkv_{mod}"] = ops.pack_linear_ln(torch.cat([q.weight, k.weight, v.weight], 0), torch.cat([q.bias, k.bias, v.bias], 0),
                                                  ln.weight, ln.bias, ln.eps)
             P[f"out_{mod}"] = ops.pack_linear(o.weight, o.bias)
+        if in_place and cache is not None:
+            P = ops.copy_packed_(cache[1], P)
         self.__dict__["_icaf_pack"] = (key, P)
         return P
 
@@ -484,7 +493,7 @@ class CrossTransformerBlock(nn.Module):
             setattr(self, f"coefficient{j}", LearnableCoefficient())
 
     # -- packed parameters ---------------------------------------------------------------------
-    def packed(self):
+    def packed(self, in_place: bool = False):
         live = [self.mlp_vis[0], self.mlp_vis[2], self.mlp_ir[0], self.mlp_ir[2], self.LN2]
         ts = [p for m in live for p in (m.weight, m.bias)] + [getattr(self, f"coefficient{j}").bias for j in range(1, 9)]
         key = _versions(*ts)
@@ -496,6 +505,8 @@ class CrossTransformerBlock(nn.Module):
             P[f"fc1_{mod}"] = ops.pack_linear_ln(mlp[0].weight, mlp[0].bias, self.LN2.weight, self.LN2.bias, self.LN2.eps, ACT_GELU)
             P[f"fc2_{mod}"] = ops.pack_linear(mlp[2].weight, mlp[2].bias)
         P["coef"] = torch.cat([getattr(self, f"coefficient{j}").bias.detach().float().reshape(1) for j in range(1, 9)])
+        if in_place and cache is not None:
+            P = ops.copy_packed_(cache[1], P)
         self.__dict__["_icaf_pack"] = (key, P)
         return P
 
@@ -557,7 +568,7 @@ class TransformerFusionBlock(nn.Module):
         self.concat = Concat(dimension=1)
         self.conv1x1_out = Conv(c1=d_model * 2, c2=d_model, k=1, s=1, p=0, g=1, act=True)
 
-    def _front(self):
+    def _front(self, in_place: bool = False):
         ts = (self.pos_emb_vis, self.pos_emb_ir, self.vis_coefficient.w1, self.vis_coefficient.w2,
               self.ir_coefficient.w1, self.ir_coefficient.w2)
         key = _versions(*ts)
@@ -567,6 +578,8 @@ class TransformerFusionBlock(nn.Module):
         pk = (self.pos_emb_vis.detach()[0].to(torch.float16).contiguous(),
               self.pos_emb_ir.detach()[0].to(torch.float16).contiguous(),
               torch.cat([t.detach().float().reshape(1) for t in ts[2:]]))
+        if in_place and cache is not None:
+            pk = ops.copy_packed_(cache[1], pk)
         self.__dict__["_icaf_pack"] = (key, pk)
         return pk
 

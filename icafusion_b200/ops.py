@@ -7,7 +7,7 @@ memory and the stream here -- every computation is a kernel from libicaf_b200.so
 from __future__ import annotations
 
 import ctypes as C
-from dataclasses import dataclass
+from dataclasses import dataclass, fields
 from typing import List, Optional, Sequence
 
 import torch
@@ -199,6 +199,34 @@ class PackedConv:
     is_weight: bool = True            # False when the "filter" operand is an activation (swap-AB linears)
     colsum: Optional[torch.Tensor] = None   # LN fold (pack_linear_ln): fp32 [w_rows] row sums of the gamma-folded fp16 filter
     ln_eps: float = 0.0
+
+
+def copy_packed_(old, new, what: str = "packed weights"):
+    """Copy a fresh pack `new` into the cached pack `old`, tensor by tensor, and return `old`.  Both are a PackedConv, a
+    tensor, or a dict / tuple / list of them.  No tensor is rebound, so every address a launch, a tensor map or a captured
+    CUDA graph holds stays valid.  Raises ValueError where a shape, dtype, stride, device or non-tensor field differs."""
+    if isinstance(old, PackedConv) and isinstance(new, PackedConv):
+        for f in fields(PackedConv):
+            a, b = getattr(old, f.name), getattr(new, f.name)
+            if torch.is_tensor(a) or torch.is_tensor(b):
+                copy_packed_(a, b, f"{what}.{f.name}")
+            elif a != b:
+                raise ValueError(f"{what}: {f.name} changed from {a!r} to {b!r}; the pack cannot be refreshed in place")
+    elif isinstance(old, dict) and isinstance(new, dict) and old.keys() == new.keys():
+        for k in old:
+            copy_packed_(old[k], new[k], f"{what}[{k!r}]")
+    elif isinstance(old, (tuple, list)) and type(old) is type(new) and len(old) == len(new):
+        for i, (a, b) in enumerate(zip(old, new)):
+            copy_packed_(a, b, f"{what}[{i}]")
+    elif torch.is_tensor(old) and torch.is_tensor(new):
+        if (old.shape, old.dtype, old.stride(), old.device) != (new.shape, new.dtype, new.stride(), new.device):
+            raise ValueError(f"{what}: {new.dtype} {tuple(new.shape)} strides {new.stride()} on {new.device} does not fit the "
+                             f"cached {old.dtype} {tuple(old.shape)} strides {old.stride()} on {old.device}")
+        if old.device.type != "meta" and old.data_ptr() != new.data_ptr():   # a bias may be the parameter itself
+            old.copy_(new)
+    elif old is not None or new is not None:
+        raise ValueError(f"{what}: {type(new).__name__} does not fit the cached {type(old).__name__}")
+    return old
 
 
 def pack_conv_weight(weight: torch.Tensor, bias: Optional[torch.Tensor], stride: int, pad: int, act: int,

@@ -166,10 +166,14 @@ def test(data,
          is_coco=False,
          opt=None,
          labels_list=None,
-         mr_annotations=None):
+         mr_annotations=None,
+         graphs=None):
     """reference: test.py:23-367, the path train.py takes (``model=`` an eval-mode CUDA Model, ``dataloader=`` batches of
     (img uint8 (B, 6, H, W), targets (T, 6), paths, shapes)).  The model is not cast: it runs in the precision it has.
-    mr_annotations: a KAIST annotation file or KaistAnnotations; image i of labels_list is the file's image id i."""
+    mr_annotations: a KAIST annotation file or KaistAnnotations; image i of labels_list is the file's image id i.
+    graphs: an :class:`~icafusion_b200.engine.ValidationGraphs` of ``model``, kept for the whole run: the batch loop then
+    replays CUDA graphs, with the filters refreshed in place from the model's current weights.  The results are the same;
+    ``t``'s inference time then includes the validation loss."""
     if model is None or dataloader is None:
         raise NotImplementedError("test: only the train.py path (model= and dataloader=) is built; the command-line path "
                                   "(weights=, attempt_load, a loader made from opt) is not")
@@ -182,6 +186,8 @@ def test(data,
     if plots:
         logger.warning("test: plots=True draws nothing here (no plots, no confusion matrix); the metrics are unaffected")
     device = next(model.parameters()).device
+    if graphs is not None:
+        graphs.check(model, device)
     if device.type != "cuda" and not (ops.dry_running() and device.type == "meta"):
         raise RuntimeError("icafusion_b200 runs on CUDA tensors only (no CPU fallback)")
     kaist = None
@@ -207,8 +213,23 @@ def test(data,
     names = {k: v for k, v in enumerate(model.names if hasattr(model, "names") else model.module.names)}
 
     loss = torch.zeros(4, device=device)
+    if graphs is not None:
+        loss = graphs.begin(iouv, (conf_thres, iou_thres, single_cls, compute_loss, save_txt or kaist is not None, kaist))
     batches, timers = [], []
     for img, targets, paths, shapes in dataloader:
+        entry = graphs.entry(img, targets.shape[0]) if graphs is not None else None
+        if entry is not None:
+            ev = [torch.cuda.Event(enable_timing=True) for _ in range(4)]
+            image = None
+            if kaist is not None:
+                if mr_rows is None:
+                    mr_rows, mr_span = graphs.kaist_buffers(kaist)
+                image = mr_positions(kaist, labels_list, paths, mr_seen)
+            det, count, correct, native = entry.run(img, targets, ratio_pad_rows(shapes), image, ev)
+            timers.append(ev)
+            batches.append((det, count, correct, native if save_txt else None, [Path(p) for p in paths],
+                            label_classes(targets, img.shape[0])))
+            continue
         img = img.to(device, non_blocking=True)
         targets_dev = targets.to(device, torch.float32, non_blocking=True).contiguous()
         nb, _, height, width = img.shape
@@ -229,7 +250,9 @@ def test(data,
             correct, _ = ops.match_detections(det, count, targets_dev, ratio_pad, height, width, iouv, single_cls,
                                               native=native)
             if kaist is not None:
-                if mr_rows is None:
+                if mr_rows is None and graphs is not None:      # the buffers the captured batches write
+                    mr_rows, mr_span = graphs.kaist_buffers(kaist)
+                elif mr_rows is None:
                     mr_rows = torch.empty(kaist.images * det.shape[1], 5, dtype=torch.float64, device=device)
                     mr_span = torch.zeros(kaist.images, 2, dtype=torch.int32, device=device)
                 image = mr_positions(kaist, labels_list, paths, mr_seen)
