@@ -62,6 +62,12 @@ class ValSample(C.Structure):
 
 KERNEL_TC = 0
 
+OPTIM_CHUNK, OPTIM_HYPER = 2048, 8        # ICAF_OPTIM_CHUNK, ICAF_OPTIM_HYPER
+
+
+class OptimTensor(C.Structure):
+    _fields_ = [(n, C.c_void_p) for n in ("p", "g", "m", "v", "step")] + [("numel", C.c_int64), ("chunk0", C.c_int64), ("reserved", C.c_int64)]
+
 _vp, _i, _i64, _f = C.c_void_p, C.c_int, C.c_int64, C.c_float
 # name -> argtypes; every symbol include/icaf_b200.h declares (tests check the .so exports them all)
 SIGNATURES = {
@@ -132,6 +138,12 @@ SIGNATURES = {
     "icaf_augment": [_vp, C.c_size_t, _i, _i, _i, _vp, _vp, _vp],
     "icaf_val_stage_params_bytes": [_i, _i],
     "icaf_val_stage": [_vp, C.c_size_t, _i, _i, _i, _i, _vp, _vp],
+    "icaf_optim_table_bytes": [_i],
+    "icaf_amp_unscale": [_vp, C.c_size_t, _i, _i64, _vp, _vp, _vp],
+    "icaf_sgd_step": [_vp, C.c_size_t, _i, _i64, _vp, _i, _i, _vp, _vp],
+    "icaf_adam_step": [_vp, C.c_size_t, _i, _i64, _vp, _i, _i, _vp, _i, _vp, _vp],
+    "icaf_amp_update_scale": [_vp, _vp, _vp, C.c_double, C.c_double, _i, _vp],
+    "icaf_ema_update": [_vp, C.c_size_t, _i, _i64, _vp, _vp],
 }
 
 _lib = None
@@ -160,7 +172,8 @@ def lib() -> C.CDLL:
                           "icaf_kaist_mr_workspace_bytes": C.c_size_t,
                           "icaf_conv2d_wgrad_workspace_bytes": C.c_size_t, "icaf_train_workspace_bytes": C.c_size_t,
                           "icaf_cross_attention_bwd_workspace_bytes": C.c_size_t,
-                          "icaf_augment_params_bytes": C.c_size_t, "icaf_val_stage_params_bytes": C.c_size_t}.get(name, C.c_int)
+                          "icaf_augment_params_bytes": C.c_size_t, "icaf_val_stage_params_bytes": C.c_size_t,
+                          "icaf_optim_table_bytes": C.c_size_t}.get(name, C.c_int)
         _lib = L
     return _lib
 

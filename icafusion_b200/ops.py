@@ -1078,3 +1078,78 @@ def maxpool5_bwd(x, dy):
     _call("icaf_maxpool5_bwd", _lib.lib().icaf_maxpool5_bwd, (_ptr(x), _ptr(dy), _ptr(dx), B, H, W, Cc, _ptr(ws), C.c_size_t(ws.numel() * 8)),
           {"bytes": 7.0 * x.numel()})
     return dx
+
+
+class OptimTable:
+    """A device table of icaf_optim_tensor entries (include/icaf_b200.h) for the optimiser-step kernels.  `rows` are tuples
+    (p, g, m, v, step) of dense fp32 tensors of one size (None where a kernel does not read the field); `ranges` names
+    consecutive row ranges (the parameter groups) that a launch may walk on their own.  The table holds the addresses of
+    these very tensors: rebuild it when one of them is reallocated."""
+
+    def __init__(self, rows, device, ranges=None):
+        from .datasets import ParamBlock
+        n = len(rows)
+        if n < 1:
+            raise ValueError("OptimTable: no tensors")
+        structs = (_lib.OptimTensor * n)()
+        self.chunk0, c = [], 0
+        for i, row in enumerate(rows):
+            p = row[0]
+            for t in row:
+                if t is None:
+                    continue
+                if t.dtype != torch.float32 or not t.is_contiguous() or not on_device(t) or (_DRY is None and t.device != p.device):
+                    raise ValueError(f"OptimTable: row {i}: every tensor must be dense fp32 on the device, got {t.dtype} "
+                                     f"{tuple(t.shape)} on {t.device}")
+                if t is not row[4] and t.numel() != p.numel():
+                    raise ValueError(f"OptimTable: row {i}: tensors of {t.numel()} and {p.numel()} elements")
+            if row[4] is not None and row[4].numel() != 1:
+                raise ValueError(f"OptimTable: row {i}: the step count must be one element")
+            structs[i] = _lib.OptimTensor(*[_addr(t) or 0 for t in row[:5]], p.numel(), c)
+            self.chunk0.append(c)
+            c += -(-p.numel() // _lib.OPTIM_CHUNK)
+        self.chunk0.append(c)
+        self.rows = list(rows)              # keeps the tensors the table points at alive
+        self.n = n
+        self.ranges = dict(ranges or {})
+        self.block = ParamBlock().upload(structs, [], int(_lib.lib().icaf_optim_table_bytes(n)), device)
+
+    def span(self, name=None):
+        """(table address, table bytes, tensors, chunks) of the named range, or of the whole table."""
+        lo, hi = self.ranges[name] if name is not None else (0, self.n)
+        entry = C.sizeof(_lib.OptimTensor)
+        addr = (_addr(self.block) or 0) + lo * entry
+        return C.c_void_p(addr), C.c_size_t(self.block.numel() - lo * entry), hi - lo, self.chunk0[hi] - self.chunk0[lo]
+
+
+def _optim_bytes(tab: OptimTable, name, tensors_per_row: int) -> float:
+    return 4.0 * tensors_per_row * sum(tab.rows[i][0].numel() for i in range(*(tab.ranges[name] if name is not None else (0, tab.n))))
+
+
+def amp_unscale(tab: OptimTable, scale: torch.Tensor, found_inf: torch.Tensor) -> None:
+    """GradScaler.unscale_ over the `g` tensors of the table; sets found_inf (fp32, one element) on a non-finite element."""
+    _call("icaf_amp_unscale", _lib.lib().icaf_amp_unscale, (*tab.span(), _ptr(scale), _ptr(found_inf)), {"bytes": _optim_bytes(tab, None, 2)})
+
+
+def sgd_step(tab: OptimTable, group: int, hyper: torch.Tensor, found_inf: torch.Tensor) -> None:
+    """Nesterov SGD over the table range `group` with the scalars of row `group` of hyper (float64 (groups, OPTIM_HYPER))."""
+    _call("icaf_sgd_step", _lib.lib().icaf_sgd_step, (*tab.span(group), _ptr(hyper), int(group), int(hyper.shape[0]), _ptr(found_inf)),
+          {"bytes": _optim_bytes(tab, group, 5)})
+
+
+def adam_step(tab: OptimTable, group: int, hyper: torch.Tensor, bias_corr: torch.Tensor, found_inf: torch.Tensor) -> None:
+    """Adam over the table range `group`; bias_corr is float64 (groups, steps, 2) of torch's (bc1, bc2_sqrt) per step."""
+    _call("icaf_adam_step", _lib.lib().icaf_adam_step,
+          (*tab.span(group), _ptr(hyper), int(group), int(hyper.shape[0]), _ptr(bias_corr), int(bias_corr.shape[1]), _ptr(found_inf)),
+          {"bytes": _optim_bytes(tab, group, 7)})
+
+
+def amp_update_scale(scale: torch.Tensor, growth_tracker: torch.Tensor, found_inf: torch.Tensor, growth_factor: float,
+                     backoff_factor: float, growth_interval: int) -> None:
+    _call("icaf_amp_update_scale", _lib.lib().icaf_amp_update_scale,
+          (_ptr(scale), _ptr(growth_tracker), _ptr(found_inf), float(growth_factor), float(backoff_factor), int(growth_interval)), {})
+
+
+def ema_update(tab: OptimTable, decay: torch.Tensor) -> None:
+    """ModelEMA.update over the table's (p = EMA entry, g = model entry) rows with d = decay[0] (device float64)."""
+    _call("icaf_ema_update", _lib.lib().icaf_ema_update, (*tab.span(), _ptr(decay)), {"bytes": _optim_bytes(tab, None, 3)})

@@ -186,13 +186,179 @@ class TrainStep:
         self.raw_model.zero_grad(set_to_none=True)
 
 
+def adam_bias_corrections(beta1: float, beta2: float, steps: int) -> np.ndarray:
+    """float64 (steps, 2): row s = (1 - beta1 ** s, (1 - beta2 ** s) ** 0.5), the Python expressions torch's Adam evaluates on
+    the host for a tensor at step s (_multi_tensor_adam, non-capturable branch).  Row 0 is never read."""
+    out = np.empty((steps, 2), dtype=np.float64)
+    for s in range(steps):
+        out[s, 0] = 1 - beta1 ** float(s)
+        out[s, 1] = (1 - beta2 ** float(s)) ** 0.5
+    return out
+
+
+class DeviceOptimizerStep:
+    """``scaler.step(optimizer); scaler.update(); ema.update(model)`` of train.py:347-352 as a fixed list of our kernels that
+    reads nothing back to the host, so it can be captured into a CUDA graph: unscale with the inf check into a device flag,
+    nesterov SGD or Adam over each parameter group (skipped on the device when the flag is set), the scale update (which
+    clears the flag) and the EMA update.  The kernels work on torch's own tensors -- parameters, ``.grad``, the optimiser's
+    state, GradScaler's ``_scale`` / ``_growth_tracker``, the EMA model's state -- so ``optimizer.state_dict()``,
+    ``scaler.state_dict()`` and ``ema.ema`` stay what the eager path would have made of them.
+
+    The tables hold the addresses of those tensors: every group parameter needs its ``.grad`` before construction, and none
+    of them may be reallocated afterwards.  Missing optimiser state is created as torch's first step would see it (a zero
+    momentum buffer gives buf = d; Adam's moments start at zero); Adam's ``step`` tensors move to the device.
+
+    Per-step scalars -- each group's lr, momentum / betas, weight decay and eps, and the EMA decay -- are read from
+    ``param_groups`` and ``ema.updates`` by :meth:`stage` and staged through a ring of pinned slots; each slot is reused only
+    once the copy out of it has completed (one CUDA event per slot).  GradScaler's growth factor, backoff factor and interval
+    are read at construction.
+
+    Adam's bias corrections come from a per-group table of rows 0 .. BIAS_STEPS - 1; when the number of stepping calls
+    reaches its size, :meth:`stage` reallocates it at twice the size and the launches must be captured again (a graph
+    capture synchronises the device: the one host wait of this path, once per doubling)."""
+
+    RING = 4
+    BIAS_STEPS = 65536          # rows of Adam's bias-correction table (train.py's 300 epochs of KAIST take ~42 000 steps);
+                                # it doubles when the step count reaches it
+
+    def __init__(self, optimizer, scaler, ema, model: nn.Module, device):
+        from . import ops
+        self.optimizer, self.scaler, self.ema = optimizer, scaler, ema
+        dev = torch.device(device)
+        self.adam = isinstance(optimizer, torch.optim.Adam)
+        if not self.adam and not isinstance(optimizer, torch.optim.SGD):
+            raise ValueError(f"DeviceOptimizerStep: SGD or Adam, got {type(optimizer).__name__}")
+        rows, ranges = [], {}
+        for gi, group in enumerate(optimizer.param_groups):
+            if group.get("maximize") or group.get("differentiable"):
+                raise ValueError("DeviceOptimizerStep: maximize / differentiable are not supported")
+            if self.adam and (group["amsgrad"] or group.get("decoupled_weight_decay")):
+                raise ValueError("DeviceOptimizerStep: Adam without amsgrad or decoupled weight decay only")
+            if not self.adam and (not group["nesterov"] or group["dampening"] != 0):
+                raise ValueError("DeviceOptimizerStep: SGD with nesterov=True and dampening=0 only (train.py:136)")
+            lo = len(rows)
+            for p in group["params"]:
+                if p.grad is None:
+                    raise ValueError("DeviceOptimizerStep: every group parameter needs its .grad (run a backward first)")
+                st = optimizer.state[p]
+                if self.adam:
+                    step = st.get("step")
+                    st["step"] = torch.zeros((), dtype=torch.float32, device=dev) if step is None else \
+                        torch.as_tensor(step, dtype=torch.float32).to(dev)
+                    for k in ("exp_avg", "exp_avg_sq"):
+                        if st.get(k) is None:
+                            st[k] = torch.zeros_like(p, memory_format=torch.preserve_format)
+                    rows.append((p, p.grad, st["exp_avg"], st["exp_avg_sq"], st["step"]))
+                else:
+                    if st.get("momentum_buffer") is None:
+                        st["momentum_buffer"] = torch.zeros_like(p, memory_format=torch.preserve_format)
+                    rows.append((p, p.grad, st["momentum_buffer"], None, None))
+            ranges[gi] = (lo, len(rows))
+        self.groups = [gi for gi, (lo, hi) in ranges.items() if hi > lo]
+        self.table = ops.OptimTable(rows, dev, ranges)
+        self.ema_table = None
+        if ema is not None:
+            msd = model.state_dict()
+            self.ema_table = ops.OptimTable([(v, msd[k], None, None, None) for k, v in ema.ema.state_dict().items()
+                                             if v.dtype.is_floating_point], dev)
+        self.scaled = scaler.is_enabled()
+        if self.scaled and scaler._scale is None:
+            raise ValueError("DeviceOptimizerStep: GradScaler has no scale tensor yet (call scaler.scale() once first)")
+        G = len(optimizer.param_groups)
+        self.found_inf = torch.zeros(1, dtype=torch.float32, device=dev)
+        self.scalars = torch.zeros(1 + G, _lib.OPTIM_HYPER, dtype=torch.float64, device=dev)   # row 0: EMA decay; 1 + g: group g
+        self.hyper = self.scalars[1:]
+        pinned = not ops.dry_running()
+        self.slots = torch.zeros(self.RING, 1 + G, _lib.OPTIM_HYPER, dtype=torch.float64, pin_memory=pinned)
+        self.slots_np = self.slots.numpy()
+        self.events = [None] * self.RING
+        self.slot = 0
+        self.device = dev
+        self.bias_corr = None
+        if self.adam:           # rows for every step the kernels can reach before the table next grows
+            self.max_step = 0 if ops.dry_running() or not rows else int(torch.stack([r[4] for r in rows]).max())
+            self._bias_corr_rows(self.BIAS_STEPS)
+
+    def _bias_corr_rows(self, steps: int) -> None:
+        from . import ops
+        self.betas = [tuple(map(float, g["betas"])) for g in self.optimizer.param_groups]
+        rows = {b: adam_bias_corrections(*b, steps) for b in set(self.betas)}
+        host = torch.from_numpy(np.stack([rows[b] for b in self.betas]))
+        host = host if ops.dry_running() else host.pin_memory()
+        if self.bias_corr is not None and self.bias_corr.shape[1] == steps:
+            self.bias_corr.copy_(host, non_blocking=True)       # same address: captured launches keep reading it
+        else:
+            self.bias_corr = host.to(self.device, non_blocking=True)
+
+    def enqueue(self) -> None:
+        """The step's launches on the current stream (what a CUDA graph captures)."""
+        from . import ops
+        sc = self.scaler
+        if self.scaled:
+            ops.amp_unscale(self.table, sc._scale, self.found_inf)
+        for gi in self.groups:
+            if self.adam:
+                ops.adam_step(self.table, gi, self.hyper, self.bias_corr, self.found_inf)
+            else:
+                ops.sgd_step(self.table, gi, self.hyper, self.found_inf)
+        if self.scaled:
+            ops.amp_update_scale(sc._scale, sc._growth_tracker, self.found_inf, sc._growth_factor, sc._backoff_factor,
+                                 sc._growth_interval)
+        if self.ema_table is not None:
+            ops.ema_update(self.ema_table, self.scalars[0])
+
+    def stage(self) -> bool:
+        """Host side of one step, before its launches run: copy this step's scalars to the device (ModelEMA's update count
+        advances here, as ``ema.update`` advances it).  Returns True when Adam's bias-correction table was reallocated to
+        cover more steps: launches enqueued (or captured) before then must be enqueued again."""
+        k = self.slot
+        if self.events[k] is None:
+            self.events[k] = torch.cuda.Event()
+        elif not self.events[k].query():             # the GPU is a whole ring behind: wait for this slot's last copy
+            self.events[k].synchronize()
+        s = self.slots_np[k]
+        for gi, g in enumerate(self.optimizer.param_groups):
+            row = s[1 + gi]
+            row[0], row[2] = g["lr"], g["weight_decay"]
+            if self.adam:
+                row[1], row[3] = g["betas"]
+                row[4] = g["eps"]
+            else:
+                row[1] = g["momentum"]
+        if self.ema is not None:
+            self.ema.updates += 1
+            s[0, 0] = self.ema.decay(self.ema.updates)
+        grew = False
+        if self.adam:
+            self.max_step += 1
+            betas = [tuple(map(float, g["betas"])) for g in self.optimizer.param_groups]
+            steps = self.bias_corr.shape[1]
+            if self.max_step >= steps or betas != self.betas:
+                grew = self.max_step >= steps
+                self._bias_corr_rows(2 * steps if grew else steps)
+        self.scalars.copy_(self.slots[k], non_blocking=True)
+        self.events[k].record()
+        self.slot = (k + 1) % self.RING
+        self.optimizer._opt_called = True            # what LRScheduler.step checks for "scheduler before optimizer"
+        return grew
+
+
 class GraphedTrainStep:
     """The same step with forward + loss + scaled backward (+ DDP's bucketed all-reduce) captured ONCE as a CUDA graph and
     replayed per batch: the ~3000 kernel launches of a yolov5l step cost the host more time than the GPU needs to run them.
     Static shapes: (B,3,H,W) uint8 batches and at most `max_targets` label rows (unused rows carry image index -1, which
-    build_targets rejects).  The optimiser step and GradScaler.update stay eager (train.py:348-350; GradScaler reads its
-    inf flag on the host).  Dropout masks: the kernels add a device-side step counter to their seeds (icaf_set_seed_offset),
+    build_targets rejects).  Dropout masks: the kernels add a device-side step counter to their seeds (icaf_set_seed_offset),
     incremented inside the graph, so every replay draws new masks.
+
+    The optimiser step (train.py:347-352: scaler.step, scaler.update, zero_grad, ema.update) is a third, small graph on the
+    same pool, replayed after the backward of every stepping call: :class:`DeviceOptimizerStep`'s unscale, SGD or Adam gated
+    on the device-side inf flag, scale update and EMA update.  A call reads nothing back and never calls
+    ``optimizer.step()``, so the host can prepare the next batch while the GPU trains.  (With Adam, the call that outgrows
+    the bias-correction table -- the 65 536th stepping call, then every doubling -- captures the step graph again, which
+    synchronises the device once.)  Each call stages the groups' current
+    lr / momentum (train.py's warm-up and LambdaLR write them between calls) and the EMA decay; ``optimizer.state_dict()``,
+    ``scaler.state_dict()`` and ``ema`` hold what the eager TrainStep would have after the same calls.  Under DDP every rank
+    steps on the same all-reduced gradients, so the ranks take the same skip decisions without an exchange.
 
     Gradient accumulation: the graph above (the "fresh" one) writes the gradients into the static ``.grad`` tensors.  The
     first call with ``optimizer_step=False`` captures a second, "accumulating" graph on the same inputs and memory pool while
@@ -223,6 +389,8 @@ class GraphedTrainStep:
         # the warm-up iterations are real steps on an all-zero batch: snapshot everything they touch and put it back afterwards
         saved = {k: v.detach().clone() for k, v in ts.raw_model.state_dict().items()}
         saved_scaler = ts.scaler.state_dict()
+        if ts.ema is not None:
+            saved_ema = ({k: v.detach().clone() for k, v in ts.ema.ema.state_dict().items()}, ts.ema.updates)
         cur = torch.cuda.current_stream(dev)
         side = torch.cuda.Stream(dev)
         side.wait_stream(cur)
@@ -239,12 +407,18 @@ class GraphedTrainStep:
                 for v in st.values():                # the gradient; Adam starts from step 0 and zero moments
                     if torch.is_tensor(v):
                         v.zero_()
+            if ts.ema is not None:
+                for k, v in ts.ema.ema.state_dict().items():
+                    v.copy_(saved_ema[0][k])
+                ts.ema.updates = saved_ema[1]
         if saved_scaler:
             ts.scaler.load_state_dict(saved_scaler)
         self.seed_ctr.zero_()
         ts.zero_grad()
         self.graph = torch.cuda.CUDAGraph()
         self.loss, self.items = self._capture(self.graph)
+        self.opt = DeviceOptimizerStep(ts.optimizer, ts.scaler, ts.ema, ts.raw_model, dev)    # on the graph's static .grad
+        self.step_graph = self._capture_step()
         self.acc_graph = None                            # the accumulating graph, captured on first use
         self.fresh = True                                # the next replay starts a new accumulation window
 
@@ -258,6 +432,12 @@ class GraphedTrainStep:
                 loss = loss * ts.world_size
             ts.scaler.scale(loss).backward()
         return loss, items
+
+    def _capture_step(self):
+        graph = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(graph, pool=self.graph.pool()):
+            self.opt.enqueue()
+        return graph
 
     def __call__(self, rgb: torch.Tensor, ir: torch.Tensor, targets: torch.Tensor, optimizer_step: bool = True):
         """As TrainStep.__call__; optimizer_step=False adds this batch's gradients to the static ``.grad`` tensors."""
@@ -279,11 +459,10 @@ class GraphedTrainStep:
             self.acc_graph.replay()
             loss, items = self.acc_loss, self.acc_items
         self.fresh = optimizer_step
-        if optimizer_step:
-            self.ts.scaler.step(self.ts.optimizer)        # gradients live in static buffers the next fresh replay overwrites
-            self.ts.scaler.update()
-            if self.ts.ema is not None:
-                self.ts.ema.update(self.ts.raw_model)
+        if optimizer_step:                               # the next fresh replay overwrites the static gradients (zero_grad)
+            if self.opt.stage():
+                self.step_graph = self._capture_step()
+            self.step_graph.replay()
         return loss.detach(), items
 
     def zero_grad(self) -> None:

@@ -532,6 +532,46 @@ size_t icaf_augment_params_bytes(int B, int s, int n_taps);
 /* params: device block laid out as above (16-byte aligned); rgb_out / ir_out: uint8 (B, 3, s, s) RGB planar. */
 int icaf_augment(const void* params, size_t params_bytes, int B, int s, int n_taps, void* rgb_out, void* ir_out, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * The optimiser step of train.py:347-352 on the device (csrc/optim.cu): GradScaler.unscale_ with the inf check, nesterov
+ * SGD or Adam skipped on the device when the check fired, GradScaler.update and ModelEMA.update -- bit-identical to torch's
+ * foreach implementations, with no read-back, so the step can be captured into a CUDA graph.  All tensors are dense fp32.
+ * ------------------------------------------------------------------------------------------- */
+#define ICAF_OPTIM_CHUNK 2048  /* elements per chunk of a tensor table                                               */
+#define ICAF_OPTIM_HYPER 8     /* doubles per parameter group in `hyper`: {lr, momentum | beta1, weight_decay, beta2,
+                                  eps, unused x 3}, read from the device at run time                                  */
+typedef struct {
+  void* p;         /* updated in place: the parameter (ema: the EMA model's entry)                                    */
+  void* g;         /* the gradient (ema: the model's entry); unscale updates it in place                             */
+  void* m;         /* SGD momentum_buffer / Adam exp_avg                                                              */
+  void* v;         /* Adam exp_avg_sq                                                                                 */
+  void* step;      /* Adam: the tensor's fp32 step count                                                             */
+  int64_t numel;
+  int64_t chunk0;  /* first chunk of this tensor: chunk0 of the previous entry + ceil(its numel / ICAF_OPTIM_CHUNK)    */
+  int64_t reserved;  /* 64-byte entries: every entry of a table starts a 16-byte aligned sub-table                  */
+} icaf_optim_tensor;
+
+/* Bytes of a device table of n_tensors entries (0 for n_tensors < 1).  A launch walks the n_tensors entries at `table`,
+ * which may start anywhere in a larger table, and the n_chunks chunks they cover. */
+size_t icaf_optim_table_bytes(int n_tensors);
+/* GradScaler.unscale_: g *= float(1.0 / double(*scale)) over every entry; *found_inf = 1 when any element is non-finite. */
+int icaf_amp_unscale(const void* table, size_t table_bytes, int n_tensors, int64_t n_chunks, const float* scale, float* found_inf,
+                     void* stream);
+/* torch.optim.SGD(nesterov=True, dampening=0) over one parameter group, skipped when *found_inf != 0:
+ * d = g + wd p (wd != 0); buf = buf m + d; d = d + m buf; p = p - lr d, with {lr, m, wd} = hyper[group]. */
+int icaf_sgd_step(const void* table, size_t table_bytes, int n_tensors, int64_t n_chunks, const double* hyper, int group, int n_groups,
+                  const float* found_inf, void* stream);
+/* torch.optim.Adam (amsgrad=False, L2 weight decay) over one parameter group, skipped when *found_inf != 0.  At each tensor's
+ * step s = *step + 1 it reads bias_corr[group][s] = {1 - beta1**s, (1 - beta2**s)**0.5} (doubles, rows 0 .. bc_steps - 1, as
+ * torch computes them on the host), then adds 1 to every step count. */
+int icaf_adam_step(const void* table, size_t table_bytes, int n_tensors, int64_t n_chunks, const double* hyper, int group, int n_groups,
+                   const double* bias_corr, int bc_steps, const float* found_inf, void* stream);
+/* torch._amp_update_scale_ on GradScaler's scale (fp32) and growth tracker (int32), then *found_inf = 0. */
+int icaf_amp_update_scale(float* scale, int* growth_tracker, float* found_inf, double growth_factor, double backoff_factor,
+                          int growth_interval, void* stream);
+/* ModelEMA.update with d = *decay (device double): p = p float(d), then p = p + float(1 - d) g. */
+int icaf_ema_update(const void* table, size_t table_bytes, int n_tensors, int64_t n_chunks, const double* decay, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
