@@ -65,6 +65,14 @@ KERNEL_TC = 0
 OPTIM_CHUNK, OPTIM_HYPER = 2048, 8        # ICAF_OPTIM_CHUNK, ICAF_OPTIM_HYPER
 
 
+class ValBatch(C.Structure):
+    _fields_ = [(n, C.c_void_p) for n in ("det", "count", "correct", "native")] + [("image0", C.c_int64)] + \
+               [(n, C.c_int) for n in ("B", "max_det", "local0")] + [("reserved", C.c_int * 3)]
+
+
+VAL_PACK_NATIVE, VAL_PACK_POS = 1, 2       # ICAF_VAL_PACK_NATIVE, ICAF_VAL_PACK_POS
+
+
 class OptimTensor(C.Structure):
     _fields_ = [(n, C.c_void_p) for n in ("p", "g", "m", "v", "step")] + [("numel", C.c_int64), ("chunk0", C.c_int64), ("reserved", C.c_int64)]
 
@@ -144,6 +152,11 @@ SIGNATURES = {
     "icaf_adam_step": [_vp, C.c_size_t, _i, _i64, _vp, _i, _i, _vp, _i, _vp, _vp],
     "icaf_amp_update_scale": [_vp, _vp, _vp, C.c_double, C.c_double, _i, _vp],
     "icaf_ema_update": [_vp, C.c_size_t, _i, _i64, _vp, _vp],
+    "icaf_val_pack_params_bytes": [_i, _i, _i],
+    "icaf_val_pack_bytes": [_i, _i, _i],
+    "icaf_val_pack": [_vp, C.c_size_t, _i, _i, _i, _i, _vp, C.c_size_t, _vp],
+    "icaf_val_merge_workspace_bytes": [_i],
+    "icaf_val_merge": [_vp, _i, _i64, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _vp, C.c_size_t, _vp],
 }
 
 _lib = None
@@ -173,7 +186,8 @@ def lib() -> C.CDLL:
                           "icaf_conv2d_wgrad_workspace_bytes": C.c_size_t, "icaf_train_workspace_bytes": C.c_size_t,
                           "icaf_cross_attention_bwd_workspace_bytes": C.c_size_t,
                           "icaf_augment_params_bytes": C.c_size_t, "icaf_val_stage_params_bytes": C.c_size_t,
-                          "icaf_optim_table_bytes": C.c_size_t}.get(name, C.c_int)
+                          "icaf_optim_table_bytes": C.c_size_t, "icaf_val_pack_params_bytes": C.c_size_t,
+                          "icaf_val_pack_bytes": C.c_size_t, "icaf_val_merge_workspace_bytes": C.c_size_t}.get(name, C.c_int)
         _lib = L
     return _lib
 

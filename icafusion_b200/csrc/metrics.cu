@@ -589,3 +589,307 @@ extern "C" int icaf_kaist_round_detections(const float* native, const float* det
   return launch_k("kaist_round_detections", kaist_round_kernel, dim3(blocks_for((long long)B * max_det, 256)), dim3(256), 0,
                   (cudaStream_t)stream, native, det, count, image, B, max_det, images, rows, span);
 }
+
+// ---------------------------------------------------------------------------------------------------------------------
+// Validation exchange buffers (icaf_val_pack / icaf_val_merge; layout in icaf_b200.h).
+namespace icaf {
+
+static_assert(sizeof(icaf_val_batch) == 64, "icaf_val_batch entries are 64 bytes");
+constexpr int kValScanThreads = 1024;
+constexpr int kValCopyThreads = 128;
+constexpr int kValHead = 4, kValImageWords = 4;
+
+__host__ __device__ inline int val_row_words(int flags) { return 3 + ((flags & ICAF_VAL_PACK_NATIVE) ? 4 : 0); }
+
+// Exclusive scan of one int per thread over the block; *total gets the block's sum.
+__device__ int val_block_scan(int v, int* s_warp, int* total) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  int inc = v;
+  for (int o = 1; o < 32; o <<= 1) {
+    const int u = __shfl_up_sync(0xffffffffu, inc, o);
+    if (lane >= o) inc += u;
+  }
+  if (lane == 31) s_warp[warp] = inc;
+  __syncthreads();
+  if (warp == 0) {
+    const int w = lane < (int)(blockDim.x >> 5) ? s_warp[lane] : 0;
+    int wi = w;
+    for (int o = 1; o < 32; o <<= 1) {
+      const int u = __shfl_up_sync(0xffffffffu, wi, o);
+      if (lane >= o) wi += u;
+    }
+    s_warp[lane] = wi - w;
+    if (lane == 31) *total = wi;
+  }
+  __syncthreads();
+  const int r = s_warp[warp] + inc - v;
+  __syncthreads();                                              // s_warp is reused by the next call
+  return r;
+}
+
+// The entry holding local image k: the last one whose local0 <= k.
+__device__ __forceinline__ const icaf_val_batch& val_entry(const icaf_val_batch* t, int n, int k) {
+  int lo = 0, hi = n - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (t[mid].local0 <= k) lo = mid; else hi = mid - 1;
+  }
+  return t[lo];
+}
+
+// One block: the image headers and the buffer header, rows placed by an exclusive scan over the clamped counts.
+__global__ void __launch_bounds__(kValScanThreads) val_pack_scan_kernel(const icaf_val_batch* t, int n_batches, const int* pos,
+                                                                       int n_images, int flags, int* out) {
+  pdl_launch_dependents();
+  pdl_wait();
+  __shared__ int s_warp[32];
+  __shared__ int s_total;
+  int carry = 0;
+  for (int base = 0; base < n_images; base += kValScanThreads) {
+    const int k = base + threadIdx.x;
+    int c = 0;
+    const icaf_val_batch* e = nullptr;
+    if (k < n_images) {
+      e = &val_entry(t, n_batches, k);
+      c = min(max(e->count[k - e->local0], 0), e->max_det);
+    }
+    const int first = carry + val_block_scan(c, s_warp, &s_total);
+    if (e) {
+      int* h = out + kValHead + kValImageWords * k;
+      h[0] = (int)(e->image0 + (k - e->local0));
+      h[1] = c;
+      h[2] = first;
+      h[3] = pos ? pos[k] : -1;
+    }
+    carry += s_total;
+  }
+  if (threadIdx.x == 0) {
+    const int rw = val_row_words(flags);
+    out[0] = n_images;
+    out[1] = carry;
+    out[2] = rw;
+    out[3] = kValHead + kValImageWords * n_images + carry * rw;
+  }
+}
+
+// One block per image (grid-stride): its rows, one thread per detection.
+__global__ void __launch_bounds__(kValCopyThreads) val_pack_rows_kernel(const icaf_val_batch* t, int n_batches, int n_images,
+                                                                       int niou, int flags, int* out) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const int rw = val_row_words(flags);
+  uint32_t* rows = reinterpret_cast<uint32_t*>(out + kValHead + kValImageWords * n_images);
+  for (int k = blockIdx.x; k < n_images; k += gridDim.x) {
+    const icaf_val_batch& e = val_entry(t, n_batches, k);
+    const int* h = out + kValHead + kValImageWords * k;
+    const int c = h[1], first = h[2];
+    const size_t b = (size_t)(k - e.local0);
+    for (int i = threadIdx.x; i < c; i += kValCopyThreads) {
+      const size_t s = b * e.max_det + i;
+      uint32_t* r = rows + (size_t)(first + i) * rw;
+      r[0] = __float_as_uint(e.det[s * 6 + 4]);
+      r[1] = __float_as_uint(e.det[s * 6 + 5]);
+      uint32_t bits = 0;
+      for (int j = 0; j < niou; ++j) bits |= (e.correct[s * niou + j] != 0 ? 1u : 0u) << j;
+      r[2] = bits;
+      if (flags & ICAF_VAL_PACK_NATIVE)
+        for (int j = 0; j < 4; ++j) r[3 + j] = __float_as_uint(e.native[s * 4 + j]);
+    }
+  }
+}
+
+// Workspace per global image: {claims, buffer, entry, unused}.
+__global__ void __launch_bounds__(256) val_merge_clear_kernel(int4* slot, int n_images, int* status) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const int k = blockIdx.x * 256 + threadIdx.x;
+  if (k < n_images) slot[k] = make_int4(0, -1, -1, 0);
+  if (k < 4) status[k] = 0;
+}
+
+// Every image header of every buffer claims its global image; malformed headers are counted in status[2].
+__global__ void __launch_bounds__(256) val_merge_claim_kernel(const int* bufs, long long buf_words, int n_images, int rw,
+                                                             int4* slot, int* status) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const int b = blockIdx.y;
+  const int* buf = bufs + (size_t)b * buf_words;
+  const int n = buf[0], nr = buf[1];
+  const bool ok = n >= 0 && nr >= 0 && buf[2] == rw && (long long)kValHead + (long long)kValImageWords * n + (long long)nr * rw == buf[3] &&
+                  buf[3] <= buf_words;
+  if (!ok) {
+    if (blockIdx.x == 0 && threadIdx.x == 0) atomicAdd(status + 2, 1);
+    return;
+  }
+  for (int e = blockIdx.x * 256 + threadIdx.x; e < n; e += gridDim.x * 256) {
+    const int* h = buf + kValHead + kValImageWords * e;
+    const int img = h[0];
+    if (img < 0 || img >= n_images || h[1] < 0 || h[2] < 0 || (long long)h[2] + h[1] > nr) {
+      atomicAdd(status + 2, 1);
+      continue;
+    }
+    atomicAdd(&slot[img].x, 1);
+    slot[img].y = b;                                             // only read when the image has exactly one claim
+    slot[img].z = e;
+  }
+}
+
+// One block: counts and offsets in global image order (exclusive scan); missing and duplicated images into the status.
+__global__ void __launch_bounds__(kValScanThreads) val_merge_scan_kernel(const int* bufs, long long buf_words, const int4* slot,
+                                                                        int n_images, int* counts, int* offsets, int* status) {
+  pdl_launch_dependents();
+  pdl_wait();
+  __shared__ int s_warp[32];
+  __shared__ int s_total;
+  int carry = 0, missing = 0, dup = 0;
+  for (int base = 0; base < n_images; base += kValScanThreads) {
+    const int k = base + threadIdx.x;
+    int c = 0;
+    if (k < n_images) {
+      const int4 s = slot[k];
+      missing += s.x == 0;
+      dup += s.x > 1;
+      if (s.x == 1) c = bufs[(size_t)s.y * buf_words + kValHead + kValImageWords * s.z + 1];
+      counts[k] = c;
+    }
+    const int off = carry + val_block_scan(c, s_warp, &s_total);
+    if (k < n_images) offsets[k] = off;
+    carry += s_total;
+  }
+  if (missing) atomicAdd(status, missing);
+  if (dup) atomicAdd(status + 1, dup);
+  if (threadIdx.x == 0) {
+    offsets[n_images] = carry;
+    status[3] = carry;
+  }
+}
+
+// One block per global image (grid-stride): its rows into the flat arrays, and the KAIST rows at its position.
+__global__ void __launch_bounds__(kValCopyThreads) val_merge_rows_kernel(const int* bufs, long long buf_words, const int4* slot,
+                                                                        int n_images, int n_rows, int niou, int flags,
+                                                                        const int* offsets, unsigned char* correct, float* conf,
+                                                                        float* pcls, float* native, double* mr_rows, int* mr_span,
+                                                                        int mr_images, int mr_max_det, int* status) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const int rw = val_row_words(flags);
+  for (int k = blockIdx.x; k < n_images; k += gridDim.x) {
+    const int4 s = slot[k];
+    if (s.x != 1) continue;
+    const int* buf = bufs + (size_t)s.y * buf_words;
+    const int* h = buf + kValHead + kValImageWords * s.z;
+    const int c = h[1], p = h[3];
+    const uint32_t* src = reinterpret_cast<const uint32_t*>(buf + kValHead + kValImageWords * buf[0]) + (size_t)h[2] * rw;
+    const int off = offsets[k];
+    const bool mr = mr_rows && p >= 0;
+    if (mr && threadIdx.x == 0) {
+      if (p < mr_images && c <= mr_max_det) {
+        mr_span[2 * p] = p * mr_max_det;
+        mr_span[2 * p + 1] = c;
+      } else {
+        atomicAdd(status + 2, 1);
+      }
+    }
+    for (int i = threadIdx.x; i < c; i += kValCopyThreads) {
+      const uint32_t* r = src + (size_t)i * rw;
+      const int o = off + i;
+      if (o < n_rows) {
+        conf[o] = __uint_as_float(r[0]);
+        pcls[o] = __uint_as_float(r[1]);
+        for (int j = 0; j < niou; ++j) correct[(size_t)o * niou + j] = (r[2] >> j) & 1u;
+        if (flags & ICAF_VAL_PACK_NATIVE)
+          for (int j = 0; j < 4; ++j) native[(size_t)o * 4 + j] = __uint_as_float(r[3 + j]);
+      }
+      if (mr && p < mr_images && c <= mr_max_det) {             // icaf_kaist_round_detections' arithmetic
+        const float x1 = __uint_as_float(r[3]), y1 = __uint_as_float(r[4]), x2 = __uint_as_float(r[5]),
+                    y2 = __uint_as_float(r[6]);
+        double* d = mr_rows + ((size_t)p * mr_max_det + i) * 5;
+        d[0] = round_g6(x1);
+        d[1] = round_g6(y1);
+        d[2] = round_g6(__fsub_rn(x2, x1));
+        d[3] = round_g6(__fsub_rn(y2, y1));
+        d[4] = round_g6(__uint_as_float(r[0]));
+      }
+    }
+  }
+}
+
+inline unsigned val_grid(int n) { return (unsigned)min(n, 8 * sm_count_cached()); }
+
+}  // namespace icaf
+
+static size_t align16(size_t x) { return (x + 15) & ~size_t(15); }
+
+extern "C" size_t icaf_val_pack_params_bytes(int n_batches, int n_images, int flags) {
+  if (n_batches < 1 || n_images < n_batches || (flags & ~(ICAF_VAL_PACK_NATIVE | ICAF_VAL_PACK_POS))) return 0;
+  return (size_t)n_batches * sizeof(icaf_val_batch) + ((flags & ICAF_VAL_PACK_POS) ? align16((size_t)n_images * 4) : 0);
+}
+
+extern "C" size_t icaf_val_pack_bytes(int n_images, int max_det, int flags) {
+  if (n_images < 0 || max_det < 1 || (flags & ~(ICAF_VAL_PACK_NATIVE | ICAF_VAL_PACK_POS))) return 0;
+  const long long words = kValHead + (long long)n_images * (kValImageWords + (long long)max_det * val_row_words(flags));
+  if (words > 0x7fffffffLL) return 0;                           // row indices and headers are int32
+  return (size_t)words * 4;
+}
+
+extern "C" int icaf_val_pack(const void* params, size_t params_bytes, int n_batches, int n_images, int niou, int flags, void* out,
+                             size_t out_bytes, void* stream) {
+  if (!params || !out) return set_error(ICAF_ERR_BAD_ARG, "val_pack: null params or out");
+  if (reinterpret_cast<uintptr_t>(params) & 15) return set_error(ICAF_ERR_BAD_ARG, "val_pack: params not 16-byte aligned");
+  if (reinterpret_cast<uintptr_t>(out) & 15) return set_error(ICAF_ERR_BAD_ARG, "val_pack: out not 16-byte aligned");
+  if (niou < 1 || niou > 32) return set_error(ICAF_ERR_BAD_ARG, "val_pack: niou outside [1, 32]");
+  const size_t need = icaf_val_pack_params_bytes(n_batches, n_images, flags);
+  if (!need || params_bytes != need)
+    return set_error(ICAF_ERR_BAD_ARG, "val_pack: the parameter block does not hold n_batches entries and n_images images "
+                                       "(icaf_val_pack_params_bytes)");
+  if (out_bytes < (size_t)(kValHead + kValImageWords * (long long)n_images) * 4)
+    return set_error(ICAF_ERR_BAD_ARG, "val_pack: out is shorter than the headers (size it with icaf_val_pack_bytes)");
+  const cudaStream_t st = (cudaStream_t)stream;
+  const icaf_val_batch* t = static_cast<const icaf_val_batch*>(params);
+  const int* pos = (flags & ICAF_VAL_PACK_POS) ? reinterpret_cast<const int*>(static_cast<const char*>(params) + n_batches * sizeof(icaf_val_batch)) : nullptr;
+  if (int rc = launch_k("val_pack_scan", val_pack_scan_kernel, dim3(1), dim3(kValScanThreads), 0, st, t, n_batches, pos, n_images,
+                        flags, static_cast<int*>(out)))
+    return rc;
+  return launch_k("val_pack_rows", val_pack_rows_kernel, dim3(val_grid(n_images)), dim3(kValCopyThreads), 0, st, t, n_batches,
+                  n_images, niou, flags, static_cast<int*>(out));
+}
+
+extern "C" size_t icaf_val_merge_workspace_bytes(int n_images) {
+  if (n_images < 1) return 0;
+  return (size_t)n_images * sizeof(int4);
+}
+
+extern "C" int icaf_val_merge(const void* bufs, int n_bufs, int64_t buf_words, int n_images, int n_rows, int niou, int flags,
+                              unsigned char* correct, float* conf, float* pcls, float* native, int* counts, int* offsets, int* status,
+                              double* mr_rows, int* mr_span, int mr_images, int mr_max_det, void* workspace, size_t workspace_bytes,
+                              void* stream) {
+  const bool with_native = flags & ICAF_VAL_PACK_NATIVE;
+  if (!bufs || !counts || !offsets || !status || !workspace || (n_rows > 0 && (!correct || !conf || !pcls || (with_native && !native))))
+    return set_error(ICAF_ERR_BAD_ARG, "val_merge: null pointer");
+  if (flags & ~(ICAF_VAL_PACK_NATIVE | ICAF_VAL_PACK_POS)) return set_error(ICAF_ERR_BAD_ARG, "val_merge: unknown flags");
+  if (!mr_rows != !mr_span) return set_error(ICAF_ERR_BAD_ARG, "val_merge: pass both mr_rows and mr_span, or neither");
+  if (mr_rows && (!with_native || mr_images < 1 || mr_max_det < 1 || (long long)mr_images * mr_max_det > 0x7fffffffLL))
+    return set_error(ICAF_ERR_BAD_ARG, "val_merge: the KAIST rows need native boxes and mr_images, mr_max_det >= 1");
+  if (n_bufs < 1 || n_bufs > 65535 || n_images < 1 || n_rows < 0 || niou < 1 || niou > 32 || buf_words < kValHead)
+    return set_error(ICAF_ERR_BAD_ARG, "val_merge: bad sizes (1 <= n_bufs <= 65535, n_images >= 1, n_rows >= 0, niou in [1, 32], "
+                                       "buf_words >= 4)");
+  if (reinterpret_cast<uintptr_t>(bufs) & 15) return set_error(ICAF_ERR_BAD_ARG, "val_merge: bufs not 16-byte aligned");
+  if (reinterpret_cast<uintptr_t>(workspace) & 15 || workspace_bytes < icaf_val_merge_workspace_bytes(n_images))
+    return set_error(ICAF_ERR_BAD_ARG, "val_merge: workspace not 16-byte aligned or shorter than icaf_val_merge_workspace_bytes");
+  const cudaStream_t st = (cudaStream_t)stream;
+  int4* slot = static_cast<int4*>(workspace);
+  const int* b = static_cast<const int*>(bufs);
+  const int rw = val_row_words(flags);
+  if (int rc = launch_k("val_merge_clear", val_merge_clear_kernel, dim3(blocks_for(max(n_images, 4), 256)), dim3(256), 0, st, slot,
+                        n_images, status))
+    return rc;
+  if (int rc = launch_k("val_merge_claim", val_merge_claim_kernel, dim3(blocks_for(n_images, 256), n_bufs), dim3(256), 0, st, b,
+                        (long long)buf_words, n_images, rw, slot, status))
+    return rc;
+  if (int rc = launch_k("val_merge_scan", val_merge_scan_kernel, dim3(1), dim3(kValScanThreads), 0, st, b, (long long)buf_words,
+                        (const int4*)slot, n_images, counts, offsets, status))
+    return rc;
+  return launch_k("val_merge_rows", val_merge_rows_kernel, dim3(val_grid(n_images)), dim3(kValCopyThreads), 0, st, b,
+                  (long long)buf_words, (const int4*)slot, n_images, n_rows, niou, flags, (const int*)offsets, correct, conf, pcls,
+                  native, mr_rows, mr_span, mr_images, mr_max_det, status);
+}

@@ -235,6 +235,20 @@ def refresh_packed_(model: Model) -> int:
     return n
 
 
+def broadcast_model_(model: Model, src: int = 0, group=None) -> None:
+    """Give every rank of `group` rank `src`'s weights, in place: every parameter and buffer of `model` (Detect's anchors
+    included) is broadcast into the tensor it already is, so the packed-filter caches and the CUDA graphs of a
+    :class:`ValidationGraphs` keep their addresses, and the next ``begin`` refreshes the packs.  For a sharded
+    ``test.test(..., group=)`` when only rank `src` holds the EMA model; ``TrainStep(..., ema=True)`` on every rank keeps
+    identical EMA weights without it."""
+    import torch.distributed as dist
+    with torch.no_grad():
+        for t in list(model.parameters()) + list(model.buffers()):
+            buf = t.detach().clone()
+            dist.broadcast(buf, src=src, group=group)
+            t.copy_(buf)                    # an in-place copy moves the tensor's version, which the packed caches are keyed on
+
+
 def decode_values(model: Model) -> tuple:
     """What the Detect decode launches take by value, as the next forward reads them: the anchors in pixels per level and
     the strides (one device to host copy)."""
@@ -273,6 +287,7 @@ class ValidationGraphs:
         self.entries = {}                 # (B, H, W, image dtype) -> _ShapeGraphs
         self.captures = 0                 # shapes captured so far, re-captures included
         self.settings = None
+        self.per_batch = False
         self.loss = self.iouv = None
         self._stream = None
         self._values = None               # what the captured decodes hold by value: Detect's anchors and strides
@@ -285,17 +300,18 @@ class ValidationGraphs:
         if device != self.device:
             raise ValueError(f"test: graphs= was built for the model on {self.device}, the model is now on {device}")
 
-    def begin(self, iouv: torch.Tensor, settings: tuple) -> torch.Tensor:
+    def begin(self, iouv: torch.Tensor, settings: tuple, per_batch: bool = False) -> torch.Tensor:
         """Start one test.test call: refresh the packed filters in place, drop the graphs whose by-value arguments or settings
-        changed, and zero the loss accumulator, which is returned."""
+        changed, and zero the loss accumulator, which is returned.  per_batch: the captured forward writes each batch's loss
+        items to the returned tensor instead of adding them (``run(..., loss_row=)`` then copies them out)."""
         refresh_packed_(self.model)
         values = decode_values(self.model)
         packs = self._packs()
-        if values != self._values or settings != self.settings or len(packs) != len(self._held) or \
-                any(a is not b for a, b in zip(packs, self._held)):
+        if values != self._values or settings != self.settings or per_batch != self.per_batch or \
+                len(packs) != len(self._held) or any(a is not b for a, b in zip(packs, self._held)):
             # an eager forward after a weight change re-packs into new tensors: the graphs' filters are then stale
             self.entries.clear()
-            self._values, self.settings = values, settings
+            self._values, self.settings, self.per_batch = values, settings, per_batch
         if self.loss is None:
             self.loss = torch.zeros(4, device=self.device)
             self.iouv = iouv.clone()
@@ -375,7 +391,11 @@ class _ShapeGraphs:
         compute_loss = self.owner.settings[3]
         out, _, train_out = self.owner.model(self.img[:, :3], self.img[:, 3:])
         if compute_loss:
-            self.owner.loss += compute_loss([x.float() for x in train_out], self.targets)[1][:4]
+            items = compute_loss([x.float() for x in train_out], self.targets)[1][:4]
+            if self.owner.per_batch:
+                self.owner.loss.copy_(items)
+            else:
+                self.owner.loss += items
         self.z = (out if out.dtype == torch.float16 else out.half()).contiguous()
 
     def _post(self):
@@ -388,9 +408,10 @@ class _ShapeGraphs:
             rows, span = self.owner._kaist[1], self.owner._kaist[2]
             ops.kaist_round_detections(self.native, self.det, self.count, self.image, rows, span)
 
-    def run(self, img, targets, ratio_pad, image, ev):
+    def run(self, img, targets, ratio_pad, image, ev, loss_row=None):
         """One batch: stage it into the static inputs, then replay (or, for the shape's first batch, run eagerly and capture).
-        ev: four CUDA events, recorded around the forward (+ loss) and around the NMS and matching.  Returns per-batch device
+        ev: four CUDA events, recorded around the forward (+ loss) and around the NMS and matching.  loss_row: with
+        ``begin(..., per_batch=True)``, a (4,) device tensor that receives this batch's loss items.  Returns per-batch device
         copies (det, count, correct, native); nothing waits for the device."""
         T = int(targets.shape[0])
         self.img.copy_(img, non_blocking=True)
@@ -405,6 +426,8 @@ class _ShapeGraphs:
                 self._forward()
             else:
                 self.fwd.replay()
+            if loss_row is not None:
+                loss_row.copy_(self.owner.loss)
             ev[1].record()
             ev[2].record()
             if self.fwd is None:

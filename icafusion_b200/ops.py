@@ -10,6 +10,7 @@ import ctypes as C
 from dataclasses import dataclass, fields
 from typing import List, Optional, Sequence
 
+import numpy as np
 import torch
 
 from . import _lib
@@ -1153,3 +1154,100 @@ def amp_update_scale(scale: torch.Tensor, growth_tracker: torch.Tensor, found_in
 def ema_update(tab: OptimTable, decay: torch.Tensor) -> None:
     """ModelEMA.update over the table's (p = EMA entry, g = model entry) rows with d = decay[0] (device float64)."""
     _call("icaf_ema_update", _lib.lib().icaf_ema_update, (*tab.span(), _ptr(decay)), {"bytes": _optim_bytes(tab, None, 3)})
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# Validation exchange buffers: a validation split over ranks packs its per-image results, the buffers cross ranks, and the
+# merge puts them back in the one-process image order (include/icaf_b200.h, icaf_val_pack / icaf_val_merge).
+def val_pack_bytes(n_images: int, max_det: int, native: bool) -> int:
+    """Bytes of the exchange buffer of n_images images of at most max_det rows (a pure function of its arguments)."""
+    return int(_lib.lib().icaf_val_pack_bytes(int(n_images), int(max_det), _lib.VAL_PACK_NATIVE if native else 0))
+
+
+def val_pack(batches, niou: int, native: bool = False, positions=None) -> torch.Tensor:
+    """Pack the per-image results of `batches` into one exchange buffer, in the given order.  batches: [(det fp32 (B, max_det,
+    6), count int32 (B,), correct uint8 / bool (B, max_det, niou), native fp32 (B, max_det, 4) or None, image0)], image0 the
+    global index of the batch's first image.  positions: the images' KAIST annotation positions (int32, one per image) or
+    None.  Returns the int32 device buffer (its header's word 3 is the number of words written); no host sync."""
+    if not batches:
+        raise ValueError("val_pack: no batches")
+    structs = (_lib.ValBatch * len(batches))()
+    n_images, max_det, device = 0, 1, batches[0][0].device
+    for k, (det, count, correct, nat, image0) in enumerate(batches):
+        if det.dim() != 3 or det.shape[2] != 6 or det.dtype != torch.float32 or not det.is_contiguous() or not on_device(det):
+            raise ValueError(f"val_pack: batch {k}: det must be contiguous CUDA fp32 (B, max_det, 6), got {det.dtype} {tuple(det.shape)}")
+        B, md = int(det.shape[0]), int(det.shape[1])
+        if tuple(count.shape) != (B,) or count.dtype != torch.int32 or not count.is_contiguous():
+            raise ValueError(f"val_pack: batch {k}: count must be int32 ({B},)")
+        if tuple(correct.shape) != (B, md, niou) or correct.dtype not in (torch.uint8, torch.bool) or not correct.is_contiguous():
+            raise ValueError(f"val_pack: batch {k}: correct must be contiguous uint8 / bool {(B, md, niou)}")
+        if native and (nat is None or tuple(nat.shape) != (B, md, 4) or nat.dtype != torch.float32 or not nat.is_contiguous()):
+            raise ValueError(f"val_pack: batch {k}: native must be contiguous fp32 {(B, md, 4)}")
+        for t in (count, correct) + ((nat,) if native else ()):
+            if t.device != det.device or (_DRY is None and t.device != device):
+                raise ValueError(f"val_pack: batch {k}: tensors on {t.device} and {det.device} (batch 0 on {device})")
+        structs[k] = _lib.ValBatch(_addr(det), _addr(count), _addr(correct), _addr(nat) if native else None, int(image0), B, md,
+                                   n_images)
+        n_images += B
+        max_det = max(max_det, md)
+    flags = (_lib.VAL_PACK_NATIVE if native else 0) | (_lib.VAL_PACK_POS if positions is not None else 0)
+    regions = ()
+    if positions is not None:
+        pos = np.ascontiguousarray(np.asarray(positions, dtype=np.int32).reshape(-1))
+        if pos.size != n_images:
+            raise ValueError(f"val_pack: {pos.size} positions for {n_images} images")
+        regions = (pos,)
+    from .datasets import ParamBlock
+    nbytes = int(_lib.lib().icaf_val_pack_params_bytes(len(batches), n_images, flags))
+    if nbytes == 0:
+        raise ValueError(f"val_pack: unsupported sizes ({len(batches)} batches, {n_images} images)")
+    params = ParamBlock().upload(structs, regions, nbytes, device)
+    out_bytes = val_pack_bytes(n_images, max_det, native)
+    if out_bytes == 0:
+        raise ValueError(f"val_pack: {n_images} images of {max_det} rows do not fit an int32-indexed buffer")
+    out = torch.empty(out_bytes // 4, dtype=torch.int32, device=device)
+    _call("icaf_val_pack", _lib.lib().icaf_val_pack,
+          (_ptr(params), C.c_size_t(nbytes), len(batches), n_images, int(niou), flags, _ptr(out), C.c_size_t(out_bytes)),
+          {"bytes": float(out_bytes)})
+    out._icaf_params = params                  # the block must outlive the launch
+    return out
+
+
+def val_merge(bufs: torch.Tensor, n_images: int, n_rows: int, niou: int, native: bool = False, mr=None) -> dict:
+    """Merge exchange buffers (int32 (n_bufs, words), one per row, as val_pack wrote them) into flat arrays in global image
+    order: correct uint8 (n_rows, niou), conf / pcls fp32 (n_rows,), native fp32 (n_rows, 4) or None, counts int32
+    (n_images,), offsets int32 (n_images + 1,) and status int32 (4,) (see :func:`val_merge_check`).  mr: (images, max_det)
+    to also write the icaf_kaist_round_detections rows / span of every image with a position ('mr_rows', 'mr_span').
+    No host sync."""
+    if bufs.dim() != 2 or bufs.dtype != torch.int32 or not bufs.is_contiguous() or not on_device(bufs):
+        raise ValueError(f"val_merge: bufs must be contiguous CUDA int32 (n_bufs, words), got {bufs.dtype} {tuple(bufs.shape)}")
+    if n_images < 1 or n_rows < 0:
+        raise ValueError(f"val_merge: {n_images} images, {n_rows} rows")
+    dev = bufs.device
+    out = dict(correct=torch.empty(n_rows, niou, dtype=torch.uint8, device=dev), conf=torch.empty(n_rows, dtype=torch.float32, device=dev),
+               pcls=torch.empty(n_rows, dtype=torch.float32, device=dev),
+               native=torch.empty(n_rows, 4, dtype=torch.float32, device=dev) if native else None,
+               counts=torch.empty(n_images, dtype=torch.int32, device=dev), offsets=torch.empty(n_images + 1, dtype=torch.int32, device=dev),
+               status=torch.empty(4, dtype=torch.int32, device=dev), mr_rows=None, mr_span=None)
+    mr_images = mr_max_det = 0
+    if mr is not None:
+        mr_images, mr_max_det = int(mr[0]), int(mr[1])
+        out["mr_rows"] = torch.empty(mr_images * mr_max_det, 5, dtype=torch.float64, device=dev)
+        out["mr_span"] = torch.zeros(mr_images, 2, dtype=torch.int32, device=dev)
+    need = int(_lib.lib().icaf_val_merge_workspace_bytes(int(n_images)))
+    ws = torch.empty(max(need // 16, 1), 4, dtype=torch.int32, device=dev)
+    flags = _lib.VAL_PACK_NATIVE if native else 0
+    _call("icaf_val_merge", _lib.lib().icaf_val_merge,
+          (_ptr(bufs), int(bufs.shape[0]), int(bufs.shape[1]), int(n_images), int(n_rows), int(niou), flags, _ptr(out["correct"]),
+           _ptr(out["conf"]), _ptr(out["pcls"]), _ptr(out["native"]), _ptr(out["counts"]), _ptr(out["offsets"]), _ptr(out["status"]),
+           _ptr(out["mr_rows"]), _ptr(out["mr_span"]), mr_images, mr_max_det, _ptr(ws), C.c_size_t(ws.numel() * 4)),
+          {"bytes": float(bufs.numel() * 4 + n_rows * (niou + 8 + (16 if native else 0)))})
+    return out
+
+
+def val_merge_check(status, n_rows: int) -> None:
+    """Refuse a merge whose status (host copy of val_merge's 'status') shows a missing, duplicated or malformed image."""
+    missing, dup, bad, rows = (int(v) for v in status)
+    if missing or dup or bad or rows != n_rows:
+        raise ValueError(f"val_merge: {missing} image(s) missing from every buffer, {dup} in more than one, {bad} malformed "
+                         f"entries, {rows} rows for {n_rows} expected")

@@ -167,13 +167,20 @@ def test(data,
          opt=None,
          labels_list=None,
          mr_annotations=None,
-         graphs=None):
+         graphs=None,
+         group=None):
     """reference: test.py:23-367, the path train.py takes (``model=`` an eval-mode CUDA Model, ``dataloader=`` batches of
     (img uint8 (B, 6, H, W), targets (T, 6), paths, shapes)).  The model is not cast: it runs in the precision it has.
     mr_annotations: a KAIST annotation file or KaistAnnotations; image i of labels_list is the file's image id i.
     graphs: an :class:`~icafusion_b200.engine.ValidationGraphs` of ``model``, kept for the whole run: the batch loop then
     replays CUDA graphs, with the filters refreshed in place from the model's current weights.  The results are the same;
-    ``t``'s inference time then includes the validation loss."""
+    ``t``'s inference time then includes the validation loss.
+    group: a torch.distributed process group of W > 1 ranks, every one calling test.test with the same arguments (each with
+    ``graphs=`` of its own model copy, if any): the batches are split over the ranks (see :func:`owned_batches`), their
+    per-image results are exchanged and merged on the device, and every rank returns exactly what one process returns,
+    except the times in ``t``, which sum every rank's batches.  A :class:`~icafusion_b200.valdata.ValBatches` loader
+    stages only the rank's own batches; any other iterable is iterated in full on every rank (each rank pays the loader's
+    cost of every batch) and the other ranks' batches are skipped."""
     if model is None or dataloader is None:
         raise NotImplementedError("test: only the train.py path (model= and dataloader=) is built; the command-line path "
                                   "(weights=, attempt_load, a loader made from opt) is not")
@@ -185,6 +192,9 @@ def test(data,
         raise NotImplementedError("test: augmented inference is not built")
     if plots:
         logger.warning("test: plots=True draws nothing here (no plots, no confusion matrix); the metrics are unaffected")
+    if group is not None and _world(group) > 1:
+        return _test_sharded(group, data, batch_size, imgsz, conf_thres, iou_thres, single_cls, verbose, model, dataloader,
+                             save_dir, save_txt, save_conf, compute_loss, labels_list, mr_annotations, graphs)
     device = next(model.parameters()).device
     if graphs is not None:
         graphs.check(model, device)
@@ -293,3 +303,222 @@ def test(data,
     results, maps = summarise(stats, nc, names, seen, verbose, mr_result)
     t = tuple(x / max(seen, 1) * 1e3 for x in (t0, t1, t0 + t1)) + (imgsz, imgsz, batch_size)
     return (*results, *(loss.cpu() / len(dataloader)).tolist()), maps, mr_result, t
+
+
+# ------------------------------------------------------------------------------------------------------------------------
+# Validation sharded over the ranks of a process group
+def _world(group) -> int:
+    import torch.distributed as dist
+    return dist.get_world_size(group)
+
+
+def owned_batches(n_batches: int, rank: int, world: int) -> range:
+    """The global batches rank `rank` of `world` runs: j = rank (mod world), which spreads the rect batch shapes evenly."""
+    if not 0 <= rank < world:
+        raise ValueError(f"test: rank {rank} outside a world of {world}")
+    return range(rank, n_batches, world)
+
+
+def _owned(dataloader, rank, world, total):
+    """(j, global index of the batch's first image, batch) of this rank's batches; total[0] gets the loader's image count."""
+    from .valdata import ValBatches
+    if isinstance(dataloader, ValBatches):
+        total[0] = len(dataloader.order)
+        yield from dataloader.shard(rank, world)
+        return
+    n = 0
+    for j, batch in enumerate(dataloader):
+        if j % world == rank:
+            yield j, n, batch
+        n += int(batch[0].shape[0])
+    total[0] = n
+
+
+def _gather_objects(obj, group) -> list:
+    import torch.distributed as dist
+    out = [None] * dist.get_world_size(group)
+    dist.all_gather_object(out, obj, group=group)
+    return out
+
+
+def _test_sharded(group, data, batch_size, imgsz, conf_thres, iou_thres, single_cls, verbose, model, dataloader, save_dir,
+                  save_txt, save_conf, compute_loss, labels_list, mr_annotations, graphs):
+    """test() over the ranks of `group`: each rank runs its own batches, packs their per-image results (icaf_val_pack), the
+    buffers are all-gathered, and rank 0 merges them in global image order (icaf_val_merge) and runs the one-process tail
+    on the same arrays, so every metric, the loss and the files are those of one process.  The result is broadcast."""
+    import torch.distributed as dist
+    from .engine import ValidationGraphs
+    rank, world = dist.get_rank(group), dist.get_world_size(group)
+    device = next(model.parameters()).device
+    problem = None
+    if graphs is not None:
+        try:
+            graphs.check(model, device)
+        except ValueError as e:
+            problem = str(e)
+    got = _gather_objects((len(dataloader), problem), group)      # before any launch: every rank refuses together
+    for _, p in got:
+        if p:
+            raise ValueError(p)
+    if len({n for n, _ in got}) != 1:
+        raise ValueError(f"test: the dataloader holds {[n for n, _ in got]} batches on ranks 0..{world - 1}; a sharded call "
+                         "needs the same loader on every rank")
+    if device.type != "cuda":
+        raise RuntimeError("icafusion_b200 runs on CUDA tensors only (no CPU fallback)")
+    kaist = None
+    if mr_annotations is not None:
+        from .kaist_eval import KaistAnnotations
+        if labels_list is None:
+            raise ValueError("test: mr_annotations= needs labels_list (a detection's image id is its label file's index)")
+        kaist = mr_annotations if isinstance(mr_annotations, KaistAnnotations) else KaistAnnotations(mr_annotations, device)
+        if kaist.device != device:
+            raise ValueError(f"test: mr_annotations are on {kaist.device}, the model on {device}")
+    labels_dir = None
+    if rank == 0:
+        save_dir = Path(save_dir)
+        (save_dir / "labels" if save_txt else save_dir).mkdir(parents=True, exist_ok=True)
+        labels_dir = increment_path(save_dir / "labels" / "pred", exist_ok=False, mkdir=True) if save_txt else None
+
+    model.eval()
+    if isinstance(data, str):
+        with open(data) as f:
+            data = yaml.safe_load(f)
+    nc = 1 if single_cls else int(data["nc"])
+    iouv = torch.linspace(0.5, 0.95, NIOU).to(device)
+    names = {k: v for k, v in enumerate(model.names if hasattr(model, "names") else model.module.names)}
+    need_native = save_txt or kaist is not None
+    max_det = ValidationGraphs.max_det
+
+    n_batches = len(dataloader)
+    own = owned_batches(n_batches, rank, world)
+    rows = torch.zeros(len(own), 4, device=device) if compute_loss else None       # loss items per batch this rank runs
+    if graphs is not None:
+        graphs.begin(iouv, (conf_thres, iou_thres, single_cls, compute_loss, need_native, kaist), per_batch=True)
+    batches, timers, images, positions, js = [], [], [], [], []
+    total, mr_seen, mr_rows = [0], set(), None
+    try:
+        for k, (j, image0, (img, targets, paths, shapes)) in enumerate(_owned(dataloader, rank, world, total)):
+            image = mr_positions(kaist, labels_list, paths, mr_seen) if kaist is not None else None
+            entry = graphs.entry(img, targets.shape[0]) if graphs is not None else None
+            ev = [torch.cuda.Event(enable_timing=True) for _ in range(4)]
+            nb = img.shape[0]
+            if entry is not None:
+                if kaist is not None and mr_rows is None:
+                    mr_rows = graphs.kaist_buffers(kaist)
+                det, count, correct, native = entry.run(img, targets, ratio_pad_rows(shapes), image, ev,
+                                                        loss_row=rows[k] if rows is not None else None)
+            else:
+                img = img.to(device, non_blocking=True)
+                targets_dev = targets.to(device, torch.float32, non_blocking=True).contiguous()
+                _, _, height, width = img.shape
+                with torch.no_grad():
+                    ev[0].record()
+                    out, _, train_out = model(img[:, :3], img[:, 3:])
+                    if compute_loss:
+                        rows[k].copy_(compute_loss([x.float() for x in train_out], targets_dev)[1][:4])
+                    ev[1].record()
+                    ev[2].record()
+                    z = out if out.dtype == torch.float16 else out.half()
+                    det, count = ops.nms(z.contiguous(), conf_thres, iou_thres, agnostic=single_cls, multi_label=True,
+                                         max_det=max_det)
+                    ev[3].record()
+                    ratio_pad = ratio_pad_rows(shapes).pin_memory().to(device, non_blocking=True)
+                    native = torch.empty(nb, det.shape[1], 4, dtype=torch.float32, device=device) if need_native else None
+                    correct, _ = ops.match_detections(det, count, targets_dev, ratio_pad, height, width, iouv, single_cls,
+                                                      native=native)
+            timers.append(ev)
+            batches.append((det, count, correct, native if need_native else None, image0))
+            tcls = label_classes(targets, nb)
+            images += [(image0 + si, Path(p).stem, tcls[si]) for si, p in enumerate(paths)]
+            if image is not None:
+                positions += image.tolist()
+            js.append(j)
+    except ValueError as e:                         # e.g. an image outside the KAIST annotations: refused on every rank
+        problem = str(e)
+    payload = None
+    if problem is None and batches:
+        payload = ops.val_pack(batches, NIOU, native=need_native, positions=positions if kaist is not None else None)
+    torch.cuda.synchronize()
+    head = payload[:4].cpu().tolist() if payload is not None else [0, 0, 3 + 4 * need_native, 4]
+    t0 = sum(e[0].elapsed_time(e[1]) for e in timers) / 1e3
+    t1 = sum(e[2].elapsed_time(e[3]) for e in timers) / 1e3
+    loss_rows = list(zip(js, rows.cpu().numpy())) if rows is not None else []
+    info = _gather_objects(dict(problem=problem, head=head, images=images, positions=positions, loss=loss_rows, t=(t0, t1),
+                                total=total[0]), group)
+    for i in info:
+        if i["problem"]:
+            raise ValueError(i["problem"])
+
+    width = max(i["head"][3] for i in info)
+    buf = torch.zeros(width, dtype=torch.int32, device=device)
+    if payload is not None:
+        buf[:head[3]].copy_(payload[:head[3]])
+    else:
+        buf[:4].copy_(torch.tensor(head, dtype=torch.int32))
+    gathered = [torch.empty_like(buf) for _ in range(world)]
+    dist.all_gather(gathered, buf, group=group)
+
+    result = None
+    if rank == 0:
+        try:
+            result = _sharded_tail(torch.stack(gathered), info, nc, names, single_cls, verbose, need_native, kaist, labels_list,
+                                   labels_dir, save_txt, save_conf, imgsz, batch_size, n_batches, max_det)
+        except ValueError as e:
+            result = e
+    box = [result]
+    dist.broadcast_object_list(box, src=dist.get_global_rank(group, 0) if group is not dist.group.WORLD else 0, group=group)
+    if isinstance(box[0], Exception):
+        raise box[0]
+    return box[0]
+
+
+def _sharded_tail(bufs, info, nc, names, single_cls, verbose, need_native, kaist, labels_list, labels_dir, save_txt, save_conf,
+                  imgsz, batch_size, n_batches, max_det):
+    """Rank 0's part of a sharded test(): merge the ranks' buffers and run the one-process tail on the merged arrays."""
+    n_images = info[0]["total"]
+    meta = {}
+    for i in info:
+        for g, stem, tc in i["images"]:
+            meta[g] = (stem, tc)
+    if kaist is not None:
+        pos = [p for i in info for p in i["positions"]]
+        if len(set(pos)) != len(pos):
+            dup = sorted({p for p in pos if pos.count(p) > 1})[0]
+            raise ValueError(f"test: an image at KAIST position {dup} is validated twice; the miss rate takes each image once")
+    n_rows = sum(i["head"][1] for i in info)
+    stats, seen, mr_result = [], 0, [0.0] * 10
+    if n_images:
+        m = ops.val_merge(bufs, n_images, n_rows, NIOU, native=need_native,
+                          mr=(kaist.images, max_det) if kaist is not None and meta else None)
+        mr_out = None
+        if m["mr_rows"] is not None:
+            from .kaist_eval import DAY_IMAGES
+            mr_out = ops.kaist_mr(kaist, m["mr_rows"], m["mr_span"], max_det, DAY_IMAGES)
+        status = m["status"].cpu().tolist()
+        ops.val_merge_check(status, n_rows)
+        counts, offsets = m["counts"].cpu().tolist(), m["offsets"].cpu().tolist()
+        correct, conf, pcls = m["correct"].cpu().numpy().astype(bool), m["conf"].cpu().numpy(), m["pcls"].cpu().numpy()
+        native = m["native"].cpu().numpy() if m["native"] is not None else None
+        for k in range(n_images):
+            n, o = counts[k], offsets[k]
+            stem, tc = meta[k]
+            seen += 1
+            if n == 0:
+                if tc:
+                    stats.append((np.zeros((0, NIOU), dtype=bool), np.zeros(0, np.float32), np.zeros(0, np.float32), tc))
+                continue
+            pc = np.zeros(n, np.float32) if single_cls else pcls[o:o + n]
+            if save_txt:
+                append_txt(labels_dir, stem, labels_list.index(stem + ".txt"), native[o:o + n], conf[o:o + n], save_conf)
+            stats.append((correct[o:o + n], conf[o:o + n], pc, tc))
+        if mr_out is not None:
+            mr_result = kaist_mr_result(mr_out[0].cpu().numpy(), mr_out[1].cpu().numpy())
+    if save_txt:
+        write_result_txt(labels_dir)
+    results, maps = summarise(stats, nc, names, seen, verbose, mr_result)
+    loss = np.zeros(4, np.float32)
+    for _, row in sorted(r for i in info for r in i["loss"]):    # the one-process call's fp32 adds, in batch order
+        loss = loss + row
+    t0, t1 = (sum(i["t"][0] for i in info), sum(i["t"][1] for i in info))
+    t = tuple(x / max(seen, 1) * 1e3 for x in (t0, t1, t0 + t1)) + (imgsz, imgsz, batch_size)
+    return (*results, *(torch.from_numpy(loss) / n_batches).tolist()), maps, mr_result, t

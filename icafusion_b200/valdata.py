@@ -301,6 +301,14 @@ class ValBatches:
         for j in range(len(self)):
             yield self.batch(j)
 
+    def shard(self, rank: int, world: int):
+        """The batches rank `rank` of `world` runs in a sharded ``test.test(..., group=)``: (j, index of the batch's first
+        image in the rect order, batch j) for every j = rank (mod world).  The other batches are neither decoded nor staged."""
+        if not 0 <= rank < world:
+            raise ValueError(f"val: rank {rank} outside a world of {world}")
+        for j in range(rank, len(self), world):
+            yield j, j * self.batch_size, self.batch(j)
+
     def reference(self, j: int, frames_host: Optional[Callable[[int], Frames]] = None):
         """Batch j through the numpy restatement: uint8 (B, 6, H, W) numpy images (targets, paths and shapes are batch()'s)."""
         ks = range(j * self.batch_size, min((j + 1) * self.batch_size, len(self.order)))

@@ -344,6 +344,52 @@ int icaf_kaist_round_detections(const float* native, const float* det, const int
                                 int images, double* rows, int* span, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * Per-image validation results in one compact, ordered buffer (csrc/metrics.cu), so that the batches of a validation split
+ * over ranks can be exchanged and put back in the one-process order.
+ *
+ * icaf_val_pack walks a parameter block of n_batches icaf_val_batch entries (in local image order: entry k covers local
+ * images local0 .. local0 + B - 1), followed, with ICAF_VAL_PACK_POS, by an int32 region of n_images KAIST annotation
+ * positions (16-byte aligned).  It writes the int32 words of one exchange buffer:
+ *   [0..3]                      {n_images, n_rows, row_words, total_words}
+ *   [4 + 4 k ..]                per image k: {global image index, kept count, first row, position (-1 without POS)}
+ *   [4 + 4 n_images + r * row_words ..]   row r: {conf, class (fp32 bits), correct (bit j = iouv[j]), x1, y1, x2, y2 (NATIVE)}
+ * The rows of an image follow its detections' order; the first rows come from an exclusive scan over the counts in local
+ * image order (no atomics).  Counts are clamped to [0, max_det].  No allocation, no host synchronisation.
+ *
+ * icaf_val_merge takes n_bufs such buffers, buffer b at word b * buf_words, and writes flat arrays in global image order:
+ * correct uint8 (n_rows, niou), conf / pcls fp32 (n_rows), native fp32 (n_rows, 4) (NATIVE), counts int32 (n_images),
+ * offsets int32 (n_images + 1).  With mr_rows / mr_span it also writes the icaf_kaist_round_detections layout of every image
+ * that has a position p < mr_images: rows at p * mr_max_det, span[p] = (p * mr_max_det, count); mr_span must be zeroed.
+ * status int32 [4] = {images missing from every buffer, images in more than one buffer, malformed entries (image or
+ * position out of range, inconsistent headers), rows written}: the merge is valid only when status == {0, 0, 0, n_rows}.
+ * ------------------------------------------------------------------------------------------- */
+#define ICAF_VAL_PACK_NATIVE 1   /* rows carry the native (scale_coords) box                                          */
+#define ICAF_VAL_PACK_POS 2      /* the parameter block holds the KAIST positions region; headers carry them          */
+typedef struct {
+  const float* det;              /* fp32 (B, max_det, 6): what icaf_nms writes                                         */
+  const int* count;              /* int32 (B)                                                                          */
+  const unsigned char* correct;  /* uint8 (B, max_det, niou): what icaf_match_detections writes                        */
+  const float* native;           /* fp32 (B, max_det, 4), or null without ICAF_VAL_PACK_NATIVE                         */
+  int64_t image0;                /* global image index of the batch's first image                                      */
+  int B, max_det;
+  int local0;                    /* the batch's first image in the buffer                                              */
+  int reserved[3];               /* 64-byte entries                                                                    */
+} icaf_val_batch;
+
+/* Bytes of the parameter block (0 for bad sizes). */
+size_t icaf_val_pack_params_bytes(int n_batches, int n_images, int flags);
+/* Bytes of the exchange buffer for n_images images of at most max_det rows (0 for bad sizes or overflow). */
+size_t icaf_val_pack_bytes(int n_images, int max_det, int flags);
+int icaf_val_pack(const void* params, size_t params_bytes, int n_batches, int n_images, int niou, int flags, void* out,
+                  size_t out_bytes, void* stream);
+/* Workspace of icaf_val_merge (0 for bad sizes). */
+size_t icaf_val_merge_workspace_bytes(int n_images);
+int icaf_val_merge(const void* bufs, int n_bufs, int64_t buf_words, int n_images, int n_rows, int niou, int flags,
+                   unsigned char* correct, float* conf, float* pcls, float* native, int* counts, int* offsets, int* status,
+                   double* mr_rows, int* mr_span, int mr_images, int mr_max_det, void* workspace, size_t workspace_bytes,
+                   void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * Detection loss, forward only (the validation loss test.py:132-133 accumulates; the training backward is not built):
  * utils/loss.py:325-463 ComputeLoss.__call__ + build_targets -- anchor-ratio matching with the four half-cell neighbour
  * offsets, CIoU box loss, objectness BCE against IoU-valued targets (largest IoU wins a contested cell), class BCE.
