@@ -82,6 +82,7 @@ SIGNATURES = {
     "icaf_version": [],
     "icaf_last_error": [],
     "icaf_sm_count": [],
+    "icaf_set_sm_count_target": [_i],
     "icaf_kernel_launches": [],
     "icaf_conv2d_fwd": [C.POINTER(ConvGeom), C.POINTER(ConvIO), _i, _vp],
     "icaf_conv2d_plan": [C.POINTER(ConvGeom), _i, _i, _i, C.POINTER(ConvPlan)],

@@ -30,7 +30,7 @@ int current_device() {
   if (cudaGetDevice(&dev) != cudaSuccess) return -1;
   return dev;
 }
-int sm_count_cached() {
+static int device_sm_count() {
   static int sms[kMaxDevices] = {0};
   const int dev = current_device();
   if (dev < 0 || dev >= kMaxDevices) return 148;
@@ -40,6 +40,15 @@ int sm_count_cached() {
     sms[dev] = n;
   }
   return sms[dev];
+}
+
+// icaf_set_sm_count_target: 0 = the device's own count, n > 0 = plan for min(n, device count) SMs
+static std::atomic<int> g_sm_target{0};
+
+int sm_count_cached() {
+  const int n = device_sm_count();
+  const int t = g_sm_target.load(std::memory_order_relaxed);
+  return t > 0 && t < n ? t : n;
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
@@ -127,6 +136,11 @@ extern "C" int icaf_sm_count(void) {
   if (cudaGetDevice(&dev) != cudaSuccess) return -1;
   if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) return -1;
   return sms;
+}
+extern "C" int icaf_set_sm_count_target(int n) {
+  if (n < 0) return icaf::set_error(ICAF_ERR_BAD_ARG, "set_sm_count_target: the target must be 0 (the device's count) or positive");
+  icaf::g_sm_target.store(n, std::memory_order_relaxed);
+  return ICAF_OK;
 }
 
 // Device-side offset added to every dropout seed (read by the kernels at run time): a captured CUDA graph of the training step

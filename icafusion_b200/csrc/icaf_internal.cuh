@@ -13,7 +13,8 @@ namespace icaf {
 int set_error(int code, const char* msg);
 int set_cuda_error(cudaError_t e, const char* where);
 const uint32_t* seed_offset_ptr();    // see icaf_set_seed_offset
-int sm_count_cached();   // SM count of the CURRENT device (cached per device ordinal)
+int sm_count_cached();   // SM count the planners size for: the CURRENT device's (cached per ordinal), or the lower
+                         // icaf_set_sm_count_target
 int current_device();    // cudaGetDevice; -1 on error
 bool pdl_enabled();        // programmatic dependent launch on every kernel (env ICAF_PDL, default on)
 

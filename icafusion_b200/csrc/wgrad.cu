@@ -7,8 +7,9 @@
 // stride, like in the forward kernels.  wgmma reads both operands transposed (MN-major descriptors).
 //   CTA work item = (128-wide n tile, <=128-wide c tile, filter tap, split): it walks its share of the 16 x 8 pixel tiles of
 //   the output map (one ring stage = dY box(es) + X box(es) of one tile, 8 MMAs of K = 16 pixels each), accumulates
-//   D[128 n][c tile] in registers and writes one fp32 partial; wgrad_reduce_kernel sums the splits in a fixed order into the
-//   (Cout, Cin, kh, kw) fp32 gradient (deterministic: no atomics).
+//   D[128 n][c tile] in registers (in chains of kWPromote tiles, added up in fp32) and writes one fp32 partial;
+//   wgrad_reduce_kernel sums the splits in a fixed order into the (Cout, Cin, kh, kw) fp32 gradient (deterministic: no
+//   atomics).
 // 288 threads: warps 0-7 two consumer warpgroups (n rows 0-63 / 64-127 of the tile), warp 8 TMA producer.
 // Also here: the fp32 -> fp16 filter packing and the zero-stuffing the training GEMMs consume, and the bias-gradient column sums.
 #include <cstring>
@@ -21,6 +22,7 @@ constexpr int kWStages = 3;
 constexpr int kWTile = 128 * 128;                  // one 64-channel block of a 128-pixel tile (128 rows x 128 B)
 constexpr int kWStageBytes = 4 * kWTile;           // dY: two 64-n blocks, X: two 64-c blocks
 constexpr int kWSmem = kWStages * kWStageBytes + 256 + 1024;
+constexpr int kWPromote = 16;                      // pixel tiles (128 MMAs of K = 16) per accumulator chain
 
 struct WgradParams {
   float* partial;          // [splits][n_pad][taps][c_pad] fp32
@@ -40,9 +42,12 @@ __device__ __forceinline__ void wgrad_consume(const WgradParams& P, uint32_t sme
   const int warp = threadIdx.x >> 5, g = warp >> 2, w = warp & 3, l = threadIdx.x & 31;
   const uint32_t x_row_bytes = uint32_t(P.c_blk) * 2u;      // 128 B, or 64 / 32 B for 32- / 16-channel maps
   const uint32_t x_blk_bytes = 128u * x_row_bytes;
-  float acc[CW / 2];
+  // The error of the tensor cores' fp32 accumulation grows with the length of one chain of MMAs: a CTA that walked all
+  // 10240 tiles of a 16 x 320 x 320 map in one chain (one split, as 8 SMs plan it) was 1.8e-3 of the gradient's maximum
+  // off.  So `acc` takes kWPromote tiles at a time and is added into `sum` with ordinary fp32 adds, whatever the split count.
+  float acc[CW / 2], sum[CW / 2];
 #pragma unroll
-  for (int i = 0; i < CW / 2; ++i) acc[i] = 0.f;
+  for (int i = 0; i < CW / 2; ++i) acc[i] = sum[i] = 0.f;
   int s = 0;
   uint32_t ph = 0;
   for (int mt = mt_begin; mt < mt_end; ++mt) {
@@ -59,13 +64,17 @@ __device__ __forceinline__ void wgrad_consume(const WgradParams& P, uint32_t sme
     wgmma_wait<0>();
     if (l == 0) mbar_arrive(empty_bar(s));
     if (++s == kWStages) { s = 0; ph ^= 1; }
+    if ((mt - mt_begin) % kWPromote == kWPromote - 1 || mt + 1 == mt_end) {
+#pragma unroll
+      for (int i = 0; i < CW / 2; ++i) { sum[i] += acc[i]; acc[i] = 0.f; }
+    }
   }
-  // ---- epilogue: acc[i] is n row 64g + 16w + l/4 + 8*((i>>1)&1), channel 8*(i>>2) + 2*(l&3) + (i&1) ----
+  // ---- epilogue: sum[i] is n row 64g + 16w + l/4 + 8*((i>>1)&1), channel 8*(i>>2) + 2*(l&3) + (i&1) ----
 #pragma unroll
   for (int i = 0; i < CW / 2; i += 2) {
     const int n = n0 + 64 * g + 16 * w + (l >> 2) + 8 * ((i >> 1) & 1);
     float* dst = P.partial + ((size_t(split) * P.n_pad + n) * P.taps + tap) * P.c_pad + c0 + 8 * (i >> 2) + 2 * (l & 3);
-    *reinterpret_cast<float2*>(dst) = make_float2(acc[i], acc[i + 1]);   // an empty split writes zeros
+    *reinterpret_cast<float2*>(dst) = make_float2(sum[i], sum[i + 1]);   // an empty split writes zeros
   }
 }
 

@@ -86,6 +86,29 @@ def dry_running() -> bool:
     return _DRY is not None
 
 
+_SM_TARGET = 0         # the library's icaf_set_sm_count_target, as last set through sm_count_target
+
+
+class sm_count_target:
+    """Context manager: every launch planned inside plans for min(n, SM count of the device) SMs (icaf_set_sm_count_target),
+    as it would on a part or MIG slice with that many SMs; n = 0 plans for the device's own count.  The previous target is
+    restored on exit.  Process-wide, and read when a call plans its launch: graphs captured earlier keep their plans."""
+
+    def __init__(self, n: int):
+        self.n = int(n)
+
+    def __enter__(self):
+        global _SM_TARGET
+        _lib.check(_lib.lib().icaf_set_sm_count_target(self.n), "icaf_set_sm_count_target")
+        self.prev, _SM_TARGET = _SM_TARGET, self.n
+        return self
+
+    def __exit__(self, *a):
+        global _SM_TARGET
+        _lib.check(_lib.lib().icaf_set_sm_count_target(self.prev), "icaf_set_sm_count_target")
+        _SM_TARGET = self.prev
+
+
 def on_device(t: torch.Tensor) -> bool:
     """True for CUDA tensors (and for anything while a dry run is recording: meta activations, CPU-resident filters)."""
     return t.is_cuda or _DRY is not None

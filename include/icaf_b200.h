@@ -54,8 +54,17 @@ const char* icaf_last_error(void);
 /* Kernels this library has enqueued so far in this process (monotonic; one C-ABI compute call may launch more than one
  * kernel, e.g. a convolution whose last wave is peeled off as a split-K tail).  bench.py reports its per-step delta. */
 long long icaf_kernel_launches(void);
-/* Number of SMs of the current device (grid sizing of callers' workspaces); <0 on error. */
+/* Number of SMs of the current device (grid sizing of callers' workspaces); <0 on error.  Not affected by the target below. */
 int icaf_sm_count(void);
+/* SM-count target of the planners (as cublasSetSmCountTarget), process-wide: n > 0 makes every launch plan for
+ * min(n, SM count of the device) SMs -- conv tile width, split-K and persistent CTA count, the weight-gradient splits
+ * (and so icaf_conv2d_wgrad_workspace_bytes), the fused Bottleneck's CTAs and the grid-stride walkers' grids -- as on a
+ * part or MIG slice with that many SMs; n = 0 restores the device's count; n < 0 is ICAF_ERR_BAD_ARG.
+ *   - The target is read when a call plans its launch: CUDA graphs captured earlier keep the plans they captured, and a
+ *     workspace sized under one target must be sized again under another.
+ *   - Lowering the count never makes a launch need more co-resident CTAs than the full count does: persistent grids are
+ *     at most the target in size, and split-K clusters are scheduled by the hardware as a unit. */
+int icaf_set_sm_count_target(int n);
 
 /* ---------------------------------------------------------------------------------------------
  * Implicit-GEMM convolution / linear layer on the Hopper tensor cores (wgmma).
@@ -95,8 +104,9 @@ int icaf_conv2d_fwd(const icaf_conv_geom* g, const icaf_conv_io* io, int n_io, v
 
 /* The dispatcher's decision for one layer geometry, computed on the HOST only (no device, no stream, no pointers):
  * which kernel family runs it, with which tile shapes, grid and shared memory.  icaf_conv2d_fwd launches exactly the
- * plan this returns for (geometry, n_io, SM count of the current device); the same invariant checks run in both, so a
- * GPU-less test can walk every layer of a model through the dispatcher (tests/test_abi_cpu.py).
+ * plan this returns for (geometry, n_io, SM count of the current device or its lower icaf_set_sm_count_target); the same
+ * invariant checks run in both, so a GPU-less test can walk every layer of a model through the dispatcher
+ * (tests/test_abi_cpu.py).
  * pair_mode: accepted for ABI stability and ignored (sm_90a has no CTA-pair MMA). */
 #define ICAF_KERNEL_TC 0      /* wgmma implicit GEMM, 128 x BN tiles (conv_gemm.cu): one tile per CTA with split-K
                                  clusters, or, for BN = 128 grids of more than one wave, `ctas` persistent CTAs       */

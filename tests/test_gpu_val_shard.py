@@ -25,12 +25,22 @@ def _to_dev(batches, dev):
 
 @pytest.mark.parametrize("native", [False, True])
 def test_pack_and_merge_equal_the_host_loop(cuda_device, native):
-    """Ragged B = 1 / 4 batches with images of 0 and 300 rows, packed per rank for W = 3 (and W = 8: ranks without a batch),
-    merged on the device: every flat array equals the host loop's slices; the packed words equal the numpy layout."""
+    """Ragged B = 1 / 4 batches with images of 0 and 300 rows, packed per rank for W = 1, 3 and 8 (ranks without a batch),
+    merged on the device: every flat array equals the host loop's slices; the packed words equal the numpy layout.  At the
+    device's SM count the row kernels give each image its own block; planned for one SM their grids are 8 blocks, so that
+    the merge of the 15 images and the pack of W = 1 walk two images per block."""
     from icafusion_b200 import ops
     batches, n = ragged_batches(7 + native, [1, 4, 4, 2, 1, 3], native=native)
+    assert n > 8
     want = host_loop(batches)
-    for world in (3, 8):
+    for target in (0, 1):
+        with ops.sm_count_target(target):
+            _pack_and_merge(cuda_device, batches, n, want, native)
+
+
+def _pack_and_merge(cuda_device, batches, n, want, native):
+    from icafusion_b200 import ops
+    for world in (1, 3, 8):
         bufs = []
         for part_h, part_d in zip(shard(batches, world), shard(_to_dev(batches, cuda_device), world)):
             if not part_d:
