@@ -1,6 +1,8 @@
 // Detection loss, forward (utils/loss.py:325-463 ComputeLoss.__call__ + build_targets): target assignment, CIoU box loss,
-// objectness BCE against IoU-valued targets, class BCE -- three launches, no host round trip, deterministic (no floating
-// point atomics: objectness targets meet in an integer atomicMax, every sum is reduced in a fixed order).
+// objectness BCE against IoU-valued targets, class BCE -- three launches, no host round trip -- and its backward in two.
+// Deterministic, forward and backward: no floating point atomics.  Objectness targets meet in an integer atomicMax; every
+// sum is reduced in a fixed order, including the backward's sum over the candidates that meet in one cell (ascending
+// candidate index, see loss_obj_bwd_kernel).
 // Both BCE terms are optionally wrapped in the focal loss of utils/loss.py:37-64 (hyp fl_gamma > 0, loss.py:341-344): the
 // candidate and objectness kernels, forward and backward, take it as a template argument, so the plain BCE path compiles to
 // the code it has without it.
@@ -32,7 +34,9 @@ struct LossParams {
   const float* targets;                 // (nt, 6): image, class, x, y, w, h (normalised)
   int* cand_count;                      // [nl] matched candidates per level (written by finalize, read by the backward)
   const float* gout;                    // backward: d / d(out[0]) (device scalar)
-  float* dacc;                          // backward: fp32 gradient accumulator, all levels, [cells][no]
+  int* cell_head;                       // backward: per cell of all levels, first candidate of its list (-1: none)
+  int* cand_next;                       // backward: [nl][nt][na][5] next candidate in the same cell's list (-1: end)
+  float* cand_grad;                     // backward: [nl][nt][na][5][no] each candidate's box and class gradient
   void* dp[kLossMaxLevels];             // backward: fp16 / fp32 gradient of p, same memory layout as p
   float* tobj;                          // all levels, (B, na, ny, nx) each
   float* cand_box; float* cand_cls; int* cand_valid;     // [nl][nt][na][5]
@@ -132,7 +136,7 @@ __device__ __forceinline__ T ciou_t(const T& px, const T& py, const T& pw, const
 // One (level, target, anchor, offset) candidate of build_targets (loss.py:405-463).
 struct Cand {
   int lvl, a, c, gi, gj;
-  long long cell;        // index in (B, na, ny, nx) order (tobj, dacc)
+  long long cell;        // index in (B, na, ny, nx) order (tobj, cell_head)
   long long pb;          // element offset of the cell's `no` values in p / dp
   float tx, ty, gw, gh, aw, ah;
 };
@@ -200,8 +204,9 @@ __global__ void loss_candidates_kernel(const LossParams P) {
   atomicMax(reinterpret_cast<int*>(P.tobj + P.cell_off[K.lvl] + K.cell), __float_as_int(score));
 }
 
-// Backward, 1 of 2: box and class gradients of every matched candidate, accumulated in fp32 per (cell, channel) -- several
-// candidates can meet in one cell.  (fp32 atomics: the sum order is not fixed; the result is rounded to the dtype of p.)
+// Backward, 1 of 2: box and class gradients of every matched candidate, written to the candidate's own row of cand_grad,
+// and the candidate pushed onto its cell's list (several candidates can meet in one cell).  The integer atomicExch leaves
+// the list in the order the pushes land; loss_obj_bwd_kernel sorts it before it sums.
 template <bool kFocal>
 __global__ void loss_candidates_bwd_kernel(const LossParams P) {
   pdl_launch_dependents();
@@ -222,20 +227,24 @@ __global__ void loss_candidates_bwd_kernel(const LossParams P) {
   px.d[0] = 2.f * s[0] * (1.f - s[0]); py.d[1] = 2.f * s[1] * (1.f - s[1]);
   pw.d[2] = 8.f * s[2] * K.aw * s[2] * (1.f - s[2]); ph.d[3] = 8.f * s[3] * K.ah * s[3] * (1.f - s[3]);
   const Dual4 ciou = ciou_t<Dual4>(px, py, pw, ph, K.tx, K.ty, K.gw, K.gh);
-  float* acc = P.dacc + (P.cell_off[K.lvl] + K.cell) * P.no;
+  float* row = P.cand_grad + idx * P.no;
   const float kb = -g * P.box / float(n);                                           // d(1 - ciou).mean()
 #pragma unroll
-  for (int i = 0; i < 4; ++i) atomicAdd(acc + i, kb * ciou.d[i]);
+  for (int i = 0; i < 4; ++i) row[i] = kb * ciou.d[i];
   if (P.no - 5 > 1) {
     const float kc = g * P.cls / (float(n) * float(P.no - 5));
     for (int j = 0; j < P.no - 5; ++j) {
       const float x = loss_ld(pl, P.p_fp32, K.pb + 5 + j), y = (j == K.c) ? P.cp : P.cn;
-      atomicAdd(acc + 5 + j, kc * bce_elem_grad<kFocal>(x, y, P.cls_pw, P.fl_gamma));
+      row[5 + j] = kc * bce_elem_grad<kFocal>(x, y, P.cls_pw, P.fl_gamma);
     }
   }
+  P.cand_next[idx] = atomicExch(P.cell_head + P.cell_off[K.lvl] + K.cell, int(idx));
 }
 
-// Backward, 2 of 2: objectness gradient of every cell, plus the accumulated candidate gradients, written as dp.
+// Backward, 2 of 2: objectness gradient of every cell, plus the gradients of the candidates in the cell, written as dp.  The
+// one thread that owns a cell first relinks the cell's list by ascending candidate index (insertion sort: a list holds the
+// few candidates that meet in one cell), then sums each channel over the list in that order from 0 -- the same sum
+// whatever order the pushes landed in.
 template <bool kFocal>
 __global__ void __launch_bounds__(256) loss_obj_bwd_kernel(const LossParams P) {
   pdl_launch_dependents();
@@ -250,11 +259,24 @@ __global__ void __launch_bounds__(256) loss_obj_bwd_kernel(const LossParams P) {
     const int gj = int(t % ny); t /= ny;
     const int a = int(t % P.na), b = int(t / P.na);
     const long long pb = cell_offset(P, lvl, b, a, gj, gi);
-    const float* acc = P.dacc + (P.cell_off[lvl] + c) * P.no;
+    int head = -1;
+    for (int i = P.cell_head[P.cell_off[lvl] + c]; i >= 0;) {
+      const int nxt = P.cand_next[i];
+      if (head < 0 || i < head) {
+        P.cand_next[i] = head; head = i;
+      } else {
+        int q = head;
+        while (P.cand_next[q] >= 0 && P.cand_next[q] < i) q = P.cand_next[q];
+        P.cand_next[i] = P.cand_next[q]; P.cand_next[q] = i;
+      }
+      i = nxt;
+    }
     const float x = loss_ld(P.p[lvl], P.p_fp32, pb + 4), y = P.tobj[P.cell_off[lvl] + c];
     for (int j = 0; j < P.no; ++j) {
-      float v = acc[j];
+      float v = 0.f;
       if (j == 4) v += g * bce_elem_grad<kFocal>(x, y, P.obj_pw, P.fl_gamma);
+      else if (j < 4 || P.no - 5 > 1)
+        for (int i = head; i >= 0; i = P.cand_next[i]) v += P.cand_grad[(long long)i * P.no + j];
       if (P.p_fp32) reinterpret_cast<float*>(P.dp[lvl])[pb + j] = v;
       else reinterpret_cast<__half*>(P.dp[lvl])[pb + j] = __float2half(v);
     }
@@ -343,8 +365,8 @@ extern "C" size_t icaf_loss_workspace_bytes(int B, int na, int nt, const int* ny
   size_t cells = 0;
   for (int i = 0; i < nl; ++i) cells += (size_t)B * na * ny[i] * nx[i];
   const size_t cand = (size_t)nl * (nt > 0 ? nt : 1) * na * 5;
-  return align256(cells * 4) + 3 * align256(cand * 4) + align256((size_t)nl * kLossObjBlocks * 4) + align256(kLossMaxLevels * 4) +
-         align256(cells * no_bwd * 4);
+  const size_t fwd = align256(cells * 4) + 3 * align256(cand * 4) + align256((size_t)nl * kLossObjBlocks * 4) + align256(kLossMaxLevels * 4);
+  return no_bwd ? fwd + align256(cells * 4) + align256(cand * 4) + align256(cand * no_bwd * 4) : fwd;
 }
 
 // Argument checks and workspace partition shared by the forward and the backward entry.
@@ -354,6 +376,8 @@ static int loss_setup(const char* what, const void* const* p, int p_fp32, int p_
   if (!p || !ny || !nx || !anchors_host || !hyp || !workspace) return set_error(ICAF_ERR_BAD_ARG, "compute_loss: null pointer");
   if (nl < 1 || nl > kLossMaxLevels || B < 1 || na < 1 || na > 8 || no < 6 || nt < 0 || (nt > 0 && !targets))
     return set_error(ICAF_ERR_BAD_ARG, "compute_loss: bad shape (nl <= 5, na <= 8)");
+  if (bwd && (long long)nl * nt * na * 5 > 0x7fffffffLL)
+    return set_error(ICAF_ERR_BAD_ARG, "compute_loss_bwd: more than 2^31 - 1 candidates (nl * nt * na * 5)");
   if (p_ld != 0 && p_ld < na * no) return set_error(ICAF_ERR_BAD_ARG, "compute_loss: p_ld is 0 ((B,na,ny,nx,no) contiguous) or the pixel pitch of the (B,ny,nx,na*no) head map");
   if (workspace_bytes < icaf_loss_workspace_bytes(B, na, nt, ny, nx, nl, bwd ? no : 0) || (reinterpret_cast<uintptr_t>(workspace) & 255))
     return set_error(ICAF_ERR_BAD_ARG, "compute_loss: workspace too small (icaf_loss_workspace_bytes) or not 256-byte aligned");
@@ -380,7 +404,11 @@ static int loss_setup(const char* what, const void* const* p, int p_fp32, int p_
   P.cand_valid = (int*)w; w += align256(cand * 4);
   P.obj_part = (float*)w; w += align256((size_t)nl * kLossObjBlocks * 4);
   P.cand_count = (int*)w; w += align256(kLossMaxLevels * 4);
-  P.dacc = (float*)w;
+  if (bwd) {
+    P.cell_head = (int*)w; w += align256(cells * 4);
+    P.cand_next = (int*)w; w += align256(cand * 4);
+    P.cand_grad = (float*)w;
+  }
   return ICAF_OK;
 }
 
@@ -423,7 +451,7 @@ extern "C" int icaf_compute_loss_bwd(const void* const* p, int p_fp32, int p_ld,
   P.gout = grad_out;
   const bool focal = P.fl_gamma > 0.f;
   cudaStream_t st = (cudaStream_t)stream;
-  cudaError_t e = cudaMemsetAsync(P.dacc, 0, cells * no * 4, st);
+  cudaError_t e = cudaMemsetAsync(P.cell_head, 0xff, cells * 4, st);                // every cell's list empty (-1)
   if (e != cudaSuccess) return set_cuda_error(e, "compute_loss_bwd: cudaMemsetAsync");
   if (nt > 0) {
     const long long total = (long long)nl * nt * na * 5;

@@ -430,7 +430,8 @@ int icaf_compute_loss_fwd(const void* const* p, int p_fp32, int p_ld, const int*
  * Same arguments as the forward call that filled `workspace` (sized with no_bwd = no); grad_out: device fp32 scalar (the
  * GradScaler factor arrives here).  The CIoU derivative is the forward expression evaluated on forward-mode duals; the
  * objectness target and CIoU's alpha are constants, as in the reference (loss.py:372, general.py:444).  Candidate gradients
- * meeting in one cell are summed with fp32 atomics (sum order not fixed), then rounded once. */
+ * meeting in one cell are summed in fp32 by ascending candidate index (level, target, anchor, offset), then rounded once:
+ * bit-reproducible, no floating-point atomics. */
 int icaf_compute_loss_bwd(const void* const* p, int p_fp32, int p_ld, const int* ny, const int* nx, int nl, int B, int na, int no,
                           const float* targets, int nt, const float* anchors_host, const icaf_loss_hyp* hyp, const float* grad_out,
                           void* const* dp, void* workspace, size_t workspace_bytes, void* stream);

@@ -1039,15 +1039,17 @@ def _loss_case(crit, R: Operands, views, bufs, p_ld, tg, anchors, hyp, gr, tag) 
     out, out2 = R.nan(5, dtype=torch.float32), R.nan(5, dtype=torch.float32)
     ws = crit._launch(ps, p_ld, tg, out=out)
     crit._launch(ps, p_ld, tg, out=out2)
-    dbufs, dps = [], []
+    dbufs, dps, dps2 = [], [], []
     for v in views:
         _, _, ny, nx, _ = v.shape
         d = R.nan(B + 2, ny, nx, p_ld)                        # images 0 and B + 1: NaN neighbours the backward must not touch
         d[1:B + 1, ..., na * no:] = 0                         # pad channels zeroed, as _LossFn.backward allocates them
         dbufs.append(d)
         dps.append(d[1:B + 1].as_strided(v.shape, v.stride()))
+        dps2.append(R.nan(B, ny, nx, p_ld).as_strided(v.shape, v.stride()))
     gout = torch.full((1,), LOSS_GRAD_OUT, dtype=torch.float32, device=R.dev)
     crit._launch(ps, p_ld, tg, ws=ws, grad_out=gout, dps=dps)
+    crit._launch(ps, p_ld, tg, ws=ws, grad_out=gout, dps=dps2)   # same workspace: the backward leaves it reusable
     if R.meta:
         return []
 
@@ -1065,6 +1067,7 @@ def _loss_case(crit, R: Operands, views, bufs, p_ld, tg, anchors, hyp, gr, tag) 
         scale = lambda lvl=lvl: float(ref()[1][lvl].abs().max())                              # noqa: E731
         checks.append(Check(f"{tag}: dp[{lvl}]", lambda dp=dp, s=scale: dp.double().cpu() / s(),
                             lambda lvl=lvl, s=scale: ref()[1][lvl] / s(), 1.0, "close", (2e-5, 2.0 ** -11)))
+        checks.append(Check(f"{tag}: dp[{lvl}] repeat", dps2[lvl], dp, 0.0, "exact"))
         if p_ld > na * no:
             checks.append(Check(f"{tag}: dp[{lvl}] pad channels", lambda d=d: d[1:B + 1, ..., na * no:],
                                 lambda d=d: torch.zeros_like(d[1:B + 1, ..., na * no:]), 0.0, "exact"))
