@@ -76,10 +76,9 @@ def models(yolo, seed=1234):
         _save(name, meta, z16=z.numpy().astype(np.float16), **{"fp:" + k: fingerprint(v.numpy(), k) for k, v in outs.items()})
 
 
-def train_step(yolo):
-    """gen_golden_train.main on yolov5n_Transfusion_FLIR."""
+def train_step(yolo, c=TRAIN_CASE):
+    """gen_golden_train.main on the case `c` (yolov5n_Transfusion_FLIR by default)."""
     from utils.loss import ComputeLoss
-    c = TRAIN_CASE
     model = yolo.Model(_yaml(c["size"], c["dataset"]), ch=3)
     assert model.yaml["nc"] == c["nc"]
     shapes = {k: tuple(v.shape) for k, v in model.state_dict().items()}

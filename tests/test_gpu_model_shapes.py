@@ -4,12 +4,12 @@ batch.  tests/test_model_shapes_cpu.py pins the oracle used here to the same gol
 import pytest
 import torch
 
+import train_grads
 from conftest import load_golden
 from helpers import err, load_synth
 from oracle import icaf_oracle as O
 from oracle import synth
 from test_gpu_model import TOL_MODEL
-from test_gpu_train_model import check_training_step
 
 pytestmark = pytest.mark.gpu
 
@@ -42,4 +42,4 @@ def test_model_matches_reference_golden_at_544x672(cuda_device, name, fused):
 
 
 def test_training_step_yolov5s_640(cuda_device):
-    check_training_step(cuda_device, "train_yolov5s_640")
+    train_grads.run_case(cuda_device, "train_yolov5s_640")

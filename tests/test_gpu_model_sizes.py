@@ -3,22 +3,20 @@ the head-dim-8 backward), both detectors against the reference's goldens (oracle
 through the CUDA graph, and one yolov5n training step."""
 import math
 
-import numpy as np
 import pytest
 import torch
 
 import dropout_mask as DM
+import train_grads
 from conftest import load_golden
 from helpers import err, load_synth
 from oracle import icaf_oracle as O
 from oracle import synth
-from oracle.gen_golden_train import fingerprint
 from test_gpu_attn import TOL, _oracle
 from test_gpu_train_ops import _attn_ref
 
 pytestmark = pytest.mark.gpu
 TOL_MODEL = 3e-3          # as tests/test_gpu_model.py
-LOSS_SCALE = 256.0        # as tests/test_gpu_train_model.py
 PADDED = [8, 24, 48, 96]  # DMFF head dims of yolov5n P3 and yolov5m P3 / P4 / P5 (C / 8 heads)
 
 
@@ -194,67 +192,5 @@ def test_yolov5m_b16_through_graph(cuda_device):
 
 def test_training_step_yolov5n_320(cuda_device):
     """One yolov5n training step (P3 attention at head dim 8) against fp32 autograd through the oracle and the reference's own
-    step (tests/golden/train_yolov5n_flir_320.npz), with the yardsticks of test_training_step_yolov5s_320."""
-    from icafusion_b200 import Model
-    from icafusion_b200.cfg import load_cfg
-    from icafusion_b200.loss import ComputeLoss
-    m, d = load_golden("train_yolov5n_flir_320")
-    name = f"yolov5{m['size']}_Transfusion_FLIR"
-    cfg = load_cfg(name)
-    rgb, ir = synth.synth_images(m["B"], m["H"], m["W"], m["seed"])
-    t = torch.from_numpy(d["targets"])
-    model = Model(name)
-    load_synth(model, m["seed"])
-    model = model.to(cuda_device).train()
-    for mod in model.modules():
-        if isinstance(mod, torch.nn.Dropout):
-            mod.p = 0.0
-    model.hyp, model.gr = dict(m["hyp"]), m["gr"]
-    pred = model(rgb.to(cuda_device), ir.to(cuda_device))
-    loss, items = ComputeLoss(model)(pred, t.to(cuda_device))
-    (loss * LOSS_SCALE).sum().backward()
-    torch.cuda.synchronize()
-    sd = synth.synth_state_dict(synth.model_param_shapes(cfg), m["seed"])
-    rl, ri, rg, rp, _ = O.train_step(sd, cfg, rgb, ir, t, m["hyp"], m["gr"])
-    _, _, ag, ap, _ = O.train_step(sd, cfg, rgb, ir, t, m["hyp"], m["gr"], autocast_device=cuda_device, loss_scale=LOSS_SCALE)
-    got = torch.cat([loss.detach(), items]).cpu().numpy()
-    want = np.concatenate([rl.numpy().reshape(1), ri.numpy()])
-    print(f"\n[yolov5n train step] loss device {got}  oracle {want}  reference {d['out']}")
-    assert np.allclose(got, want, rtol=3e-3, atol=1e-4) and np.allclose(got, d["out"], rtol=3e-3, atol=1e-4)
-    for i in range(3):
-        e = float((pred[i].detach().float().cpu() - rp[i]).abs().max() / rp[i].abs().max())
-        ea = float((ap[i].detach().float().cpu() - rp[i]).abs().max() / rp[i].abs().max())
-        print(f"[yolov5n train step] Detect map {i}: {e:.2e}   (fp16-autocast oracle: {ea:.2e})")
-        assert e < max(1.5 * ea, 5e-3)
-    params = dict(model.named_parameters())
-    live = [k for k, p in params.items() if p.grad is not None]
-    assert sorted(live) == sorted(m["params"]) == sorted(rg)
-    num = den = num_a = 0.0
-    for k in live:
-        g = params[k].grad.detach().float().cpu() / LOSS_SCALE
-        assert torch.isfinite(g).all(), k
-        num += float(((g - rg[k]) ** 2).sum())
-        num_a += float(((ag[k].float().cpu() - rg[k]) ** 2).sum())
-        den += float((rg[k] ** 2).sum())
-    rel_l2, rel_l2_amp = (num / den) ** 0.5, (num_a / den) ** 0.5
-    print(f"[yolov5n train step] all {len(live)} gradients: relative L2 error {rel_l2:.2e} (fp16-autocast oracle: {rel_l2_amp:.2e})")
-    assert rel_l2 < max(1.5 * rel_l2_amp, 2e-3), (rel_l2, rel_l2_amp)
-    # per-tensor gradient norms against the reference's: the floor for the mathematically-zero gradients (key-projection biases,
-    # last MLP biases) is 1 % of the median norm -- the 1e-3 of the yolov5s test at its scale; yolov5n's gradients are ~4x larger.
-    # The one-element parameters (LearnableCoefficient / LearnableWeights) are one cancelling sum over a whole fp16 tensor each
-    # (see _module_case in test_gpu_train_model.py): both fp16 regimes land up to ~100 % off on some of them, so they are held
-    # by the all-gradient relative L2 above only.
-    floor = 1e-2 * float(np.median([d["g:" + k][0] for k in live]))
-    nrm = lambda g, k: float(fingerprint(g.detach().float().cpu().numpy(), k)[0])      # noqa: E731
-    dev = lambda g, k: abs(nrm(g, k) - d["g:" + k][0]) / max(d["g:" + k][0], floor)     # noqa: E731
-    rel = sorted(((dev(params[k].grad / LOSS_SCALE, k), k) for k in live), reverse=True)
-    tensors = [(e, k) for e, k in rel if params[k].numel() > 1]
-    worst = tensors[0][0]
-    worst_a = max(dev(ag[k], k) for k in live if params[k].numel() > 1)
-    print(f"[yolov5n train step] gradient norms vs the reference's fp32 backward (floor {floor:.1e}): worst tensor {worst:.2e} "
-          f"(fp16-autocast oracle: {worst_a:.2e}); worst: " + ", ".join(f"{k} {e:.2e}" for e, k in rel[:5]))
-    assert worst < max(1.5 * worst_a, 2e-2)
-    state = model.state_dict()
-    for k in m["bn_probes"]:
-        assert np.allclose(state[k + ".running_mean"].cpu().numpy(), d["rm:" + k], rtol=5e-3, atol=2e-4), k
-        assert np.allclose(state[k + ".running_var"].cpu().numpy(), d["rv:" + k], rtol=5e-3, atol=2e-4), k
+    step (tests/golden/train_yolov5n_flir_320.npz), one gradient tensor at a time (tests/train_grads.py)."""
+    train_grads.run_case(cuda_device, "train_yolov5n_flir_320")

@@ -4,93 +4,20 @@ import numpy as np
 import pytest
 import torch
 
+import train_grads
 from conftest import load_golden
 from helpers import load_synth
 from oracle import icaf_oracle as O
 from oracle import synth
-from oracle.gen_golden_train import fingerprint, synth_targets
+from oracle.gen_golden_train import synth_targets
 
 pytestmark = pytest.mark.gpu
 
-LOSS_SCALE = 256.0        # static stand-in for train.py:343's GradScaler: keeps the fp16 activation gradients above underflow
-
-
-def _step(cuda_device, m, d):
-    from icafusion_b200 import Model
-    from icafusion_b200.cfg import load_cfg
-    from icafusion_b200.loss import ComputeLoss
-    cfg = load_cfg(f"yolov5{m['size']}_Transfusion_kaist")
-    rgb, ir = synth.synth_images(m["B"], m["H"], m["W"], m["seed"])
-    t = synth_targets(m["nt"], m["B"], m["seed"])
-    model = Model(f"yolov5{m['size']}_Transfusion_kaist")
-    load_synth(model, m["seed"])
-    model = model.to(cuda_device).train()
-    for mod in model.modules():
-        if isinstance(mod, torch.nn.Dropout):
-            mod.p = 0.0                                   # the golden / oracle graph is dropout free
-    model.hyp, model.gr = dict(m["hyp"]), m["gr"]
-    pred = model(rgb.to(cuda_device), ir.to(cuda_device))
-    loss, items = ComputeLoss(model)(pred, torch.from_numpy(t).to(cuda_device))
-    (loss * LOSS_SCALE).sum().backward()
-    torch.cuda.synchronize()
-    sd = synth.synth_state_dict(synth.model_param_shapes(cfg), m["seed"])
-    ref = O.train_step(sd, cfg, rgb, ir, torch.from_numpy(t), m["hyp"], m["gr"])
-    # the reference's own regime -- fp16 autocast + loss scale (train.py:334-344) -- as the yardstick for the fp16 noise floor
-    amp = O.train_step(sd, cfg, rgb, ir, torch.from_numpy(t), m["hyp"], m["gr"], autocast_device=cuda_device, loss_scale=LOSS_SCALE)
-    return model, pred, loss, items, ref, amp
-
 
 def test_training_step_yolov5s_320(cuda_device):
-    check_training_step(cuda_device, "train_yolov5s_320")
-
-
-def check_training_step(cuda_device, name):
-    """One step of the golden's case against fp32 autograd through the oracle and the reference's own step, each bar taken
-    relative to the reference's fp16-autocast regime."""
-    m, d = load_golden(name)
-    model, pred, loss, items, (rl, ri, rg, rp, rstate), (_, _, ag, ap, _) = _step(cuda_device, m, d)
-    got = torch.cat([loss.detach(), items]).cpu().numpy()
-    want = np.concatenate([rl.numpy().reshape(1), ri.numpy()])
-    print(f"\n[train step] loss device {got}  oracle {want}  reference {d['out']}")
-    assert np.allclose(got, want, rtol=3e-3, atol=1e-4) and np.allclose(got, d["out"], rtol=3e-3, atol=1e-4)
-    for i in range(3):
-        e = float((pred[i].detach().float().cpu() - rp[i]).abs().max() / rp[i].abs().max())
-        ea = float((ap[i].detach().float().cpu() - rp[i]).abs().max() / rp[i].abs().max())
-        print(f"[train step] Detect map {i}: {e:.2e}   (fp16-autocast oracle: {ea:.2e})")
-        # fp16 activations through ~60 batch-statistics BatchNorms: the bar is the reference regime's own distance from fp32
-        assert e < max(1.5 * ea, 5e-3)
-    params = dict(model.named_parameters())
-    live = [k for k, p in params.items() if p.grad is not None]
-    assert sorted(live) == sorted(m["params"]) == sorted(rg)        # the reference's 30 dead parameters stay without gradient
-    num = den = num_a = 0.0
-    rows = []
-    for k in live:
-        g = params[k].grad.detach().float().cpu() / LOSS_SCALE
-        r = rg[k]
-        assert torch.isfinite(g).all(), k
-        num += float(((g - r) ** 2).sum())
-        num_a += float(((ag[k].float().cpu() - r) ** 2).sum())
-        den += float((r ** 2).sum())
-        # per tensor: error against the tensor's own largest gradient, floored for the mathematically-zero ones
-        rows.append((float((g - r).abs().max() / max(float(r.abs().max()), 1e-4)), float(((g - r).norm() / max(float(r.norm()), 1e-4))), k))
-    rows.sort(reverse=True)
-    rel_l2, rel_l2_amp = (num / den) ** 0.5, (num_a / den) ** 0.5
-    print(f"[train step] all {len(live)} gradients: relative L2 error {rel_l2:.2e} (fp16-autocast oracle: {rel_l2_amp:.2e}); worst tensors (max-norm, l2):")
-    for e, e2, k in rows[:8]:
-        print(f"    {e:.2e} {e2:.2e} {k}")
-    med = sorted(r[0] for r in rows)[len(rows) // 2]
-    print(f"[train step] median per-tensor max-norm error {med:.2e}")
-    assert rel_l2 < max(1.5 * rel_l2_amp, 2e-3), (rel_l2, rel_l2_amp)
-    # the REAL reference's gradients, through the stored fingerprints (norm of each gradient tensor); same yardstick
-    nrm = lambda g, k: float(fingerprint(g.detach().float().cpu().numpy(), k)[0])      # noqa: E731
-    worst = max(abs(nrm(params[k].grad / LOSS_SCALE, k) - d["g:" + k][0]) / max(d["g:" + k][0], 1e-3) for k in live)
-    worst_a = max(abs(nrm(ag[k], k) - d["g:" + k][0]) / max(d["g:" + k][0], 1e-3) for k in live)
-    print(f"[train step] gradient norms vs the reference's own fp32 backward: worst relative difference {worst:.2e} (fp16-autocast oracle: {worst_a:.2e})")
-    assert worst < max(1.5 * worst_a, 2e-2)
-    state = model.state_dict()
-    for k in m["bn_probes"]:
-        assert np.allclose(state[k + ".running_mean"].cpu().numpy(), d["rm:" + k], rtol=5e-3, atol=2e-4), k
-        assert np.allclose(state[k + ".running_var"].cpu().numpy(), d["rv:" + k], rtol=5e-3, atol=2e-4), k
+    """One step against fp32 autograd through the oracle and the reference's own step, one gradient tensor at a time, at loss
+    scales 2^8 and 2^16 (tests/train_grads.py)."""
+    train_grads.run_case(cuda_device, "train_yolov5s_320")
 
 
 def _module_case(cuda_device, mod, pre, fwd_ref, fwd_dev, inputs, tol, l2=False):

@@ -66,23 +66,42 @@ def test_model_oracle_matches_reference(name):
 
 
 def test_training_step_oracle_matches_reference_yolov5n():
+    check_training_step_oracle("train_yolov5n_flir_320")
+
+
+def test_training_step_oracle_matches_reference_yolov5l():
+    """yolov5l (head dim 128 in the attention backward, up to nine Bottlenecks per C3; oracle/gen_golden_train_l.py): the
+    oracle the GPU training-step test holds the device to."""
+    # one-element gradients: one cancelling fp32 sum each over a 109 M-parameter model's token streams; the oracle run in
+    # float64 lands 2 % from both fp32 steps on model.20.crosstransformer.0.coefficient7.bias, so summation order alone
+    # moves them past 2e-4 (1.6e-3 measured)
+    m, _ = check_training_step_oracle("train_yolov5l_320", scalar_tol=3e-3)
+    assert len(m["params"]) == 633
+
+
+def check_training_step_oracle(name, scalar_tol=2e-4):
+    """The fp32 oracle's step against the reference's: loss, every gradient's fingerprint, the Detect maps, the BN probes."""
     from oracle.gen_golden_train import fingerprint
-    m, d = load_golden("train_yolov5n_flir_320")
-    cfg = load_cfg(f"yolov5{m['size']}_Transfusion_FLIR")
+    m, d = load_golden(name)
+    cfg = load_cfg(f"yolov5{m['size']}_Transfusion_{m['dataset']}")
     sd = synth.synth_state_dict(synth.model_param_shapes(cfg), m["seed"])
     rgb, ir = synth.synth_images(m["B"], m["H"], m["W"], m["seed"])
     loss, items, grads, pred, state = O.train_step(sd, cfg, rgb, ir, torch.from_numpy(d["targets"]), m["hyp"], m["gr"])
     got = np.concatenate([loss.numpy().reshape(1), items.numpy()])
     assert np.allclose(got, d["out"], rtol=1e-4, atol=1e-6), (got, d["out"])
     assert sorted(grads) == sorted(m["params"]) and len(m["dead_params"]) == 30
-    worst = max(float(np.abs(fingerprint(grads[k].numpy(), k) - d["g:" + k]).max() / max(d["g:" + k][0], 1e-3)) for k in m["params"])
+    dev = {k: float(np.abs(fingerprint(grads[k].numpy(), k) - d["g:" + k]).max() / max(d["g:" + k][0], 1e-3)) for k in m["params"]}
+    worst = max(e for k, e in dev.items() if grads[k].numel() > 1)
     assert worst < 2e-4, worst
+    worst = max(e for k, e in dev.items() if grads[k].numel() == 1)
+    assert worst < scalar_tol, worst
     for i in range(3):
         want = d[f"pred{i}"]
         assert np.abs(fingerprint(pred[i].numpy(), f"pred{i}") - want).max() < 1e-4 * want[0]
     for k in m["bn_probes"]:
         assert np.allclose(state[k + ".running_mean"].numpy(), d["rm:" + k], rtol=1e-4, atol=1e-6)
         assert np.allclose(state[k + ".running_var"].numpy(), d["rv:" + k], rtol=1e-4, atol=1e-6)
+    return m, d
 
 
 def _plan_all(records):
