@@ -142,6 +142,15 @@ SIGNATURES = {
     "icaf_cross_attention_bwd_workspace_bytes": [_i, _i, _i],
     "icaf_cross_attention_bwd": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _f, C.c_uint32, _vp, C.c_size_t, _vp],
     "icaf_axpby": [_vp, _vp, _vp, _vp, _vp, _i64, _vp],
+    "icaf_dmff_pool_tokens_f32": [_vp, _vp, _i64, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp],
+    "icaf_dmff_pool_tokens_bwd_f32": [_vp, _vp, _i64, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp, C.c_size_t, _vp],
+    "icaf_dmff_upsample_cat_f32": [_vp, _vp, _i, _vp, _vp, _i64, _vp, _i64, _i, _i, _i, _i, _i, _i, _vp],
+    "icaf_dmff_upsample_cat_bwd_f32": [_vp, _i64, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp],
+    "icaf_layernorm_f32": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _i, _f, _vp],
+    "icaf_layernorm_bwd_f32": [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _i, _f, _f, _i, _vp, C.c_size_t, _vp],
+    "icaf_axpby_f32": [_vp, _vp, _vp, _vp, _vp, _i, _i64, _vp],
+    "icaf_dot_f32": [_vp, _vp, _i, _i64, _i, _vp, _f, _i, _vp, C.c_size_t, _vp],
+    "icaf_colsum_f32": [_vp, _i64, _i, _vp, _f, _i, _vp, C.c_size_t, _vp],
     "icaf_detect_decode": [_vp, _i64, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _f, C.POINTER(C.c_float), _vp],
     "icaf_augment_params_bytes": [_i, _i, _i],
     "icaf_augment": [_vp, C.c_size_t, _i, _i, _i, _vp, _vp, _vp],

@@ -7,7 +7,10 @@ pool.cu, dmff.cu, attn_bwd.cu).  torch provides the graph walk, the gradient acc
 and the ``.grad`` buffers -- so the reference's optimiser, GradScaler, EMA and DDP (train.py:120-235) work unchanged.
 
 Activations and activation gradients are fp16 NHWC (the reference trains under autocast, train.py:334); parameters stay
-fp32 masters and are re-packed to the kernels' fp16 layout each step; parameter gradients are fp32.
+fp32 masters and are re-packed to the kernels' fp16 layout each step; parameter gradients are fp32.  A TransformerFusionBlock
+whose ``stream_dtype`` is torch.float32 keeps its token streams and their gradients in fp32, from the pooling to the
+upsample-and-add, where the reference's autocast makes them fp32 (an fp32 one-element parameter times an fp16 tensor promotes);
+GEMM operands, attention and branch outputs stay fp16.  The nodes on the stream take their precision from the tensors they get.
 
 Reference semantics reproduced here (training mode): BatchNorm with batch statistics and running-stat update
 (common.py:56), dropout on attention probabilities, projection and MLP outputs (common.py:677-685, 716-721), nearest
@@ -197,9 +200,13 @@ class LinearFn(Function):
 
 
 class LayerNormFn(Function):
+    """fp16 output for either input: over an fp32 token stream it is autocast's fp32 LayerNorm followed by the fp16 cast at the
+    Linear it feeds, and the backward adds an fp32 dx into the stream's gradient."""
+
     @staticmethod
     def forward(ctx, x, gamma, beta, eps: float):
-        y = ops.layernorm(x.contiguous(), _f32(gamma), _f32(beta), eps=eps)
+        ln = ops.layernorm_f32 if x.dtype == torch.float32 else ops.layernorm
+        y = ln(x.contiguous(), _f32(gamma), _f32(beta), eps=eps)
         ctx.save_for_backward(x, gamma)
         ctx.eps = eps
         return y
@@ -209,7 +216,8 @@ class LayerNormFn(Function):
         x, gamma = ctx.saved_tensors
         dg = torch.empty(gamma.shape, dtype=torch.float32, device=x.device)
         db = torch.empty_like(dg)
-        dx = ops.layernorm_bwd(x, dy, _f32(gamma), ctx.eps, dg, db)
+        bwd = ops.layernorm_bwd_f32 if x.dtype == torch.float32 else ops.layernorm_bwd
+        dx = bwd(x.contiguous(), dy, _f32(gamma), ctx.eps, dg, db)
         return dx, dg, db, None
 
 
@@ -242,17 +250,24 @@ def dropout(x: torch.Tensor, p: float) -> torch.Tensor:
 
 
 class CoefPairFn(Function):
-    """c_a * x + c_b * o with two LearnableCoefficient scalars (common.py:747-750)."""
+    """c_a * x + c_b * o with two LearnableCoefficient scalars (common.py:747-750).  With an fp32 stream x (and the fp16 branch
+    output o) the result and dx are fp32 and do is fp16, each the reference's autocast value bit for bit."""
 
     @staticmethod
     def forward(ctx, x, o, ca, cb):
         ctx.save_for_backward(x, o, ca, cb)
+        if x.dtype == torch.float32:
+            return ops.axpby_f32(x, _f32(ca), o, _f32(cb))
         return ops.axpby(x, _f32(ca), o, _f32(cb))
 
     @staticmethod
     def backward(ctx, dy):
         x, o, ca, cb = ctx.saved_tensors
         dy = dy.contiguous()
+        if x.dtype == torch.float32:
+            dx = ops.axpby_f32(dy, _f32(ca)) if ctx.needs_input_grad[0] else None
+            do = ops.axpby_f32(dy, _f32(cb), out_dtype=o.dtype) if ctx.needs_input_grad[1] else None
+            return dx, do, ops.dot_f32(dy, x).to(ca.dtype), ops.dot_f32(dy, o).to(cb.dtype)
         dx = ops.axpby(dy, _f32(ca)) if ctx.needs_input_grad[0] else None
         do = ops.axpby(dy, _f32(cb)) if ctx.needs_input_grad[1] else None
         return dx, do, ops.dot(dy, x).to(ca.dtype), ops.dot(dy, o).to(cb.dtype)
@@ -290,49 +305,63 @@ class CrossAttentionFn(Function):
 
 
 class PoolTokensFn(Function):
-    """avg / max adaptive pooling mixed by LearnableWeights + positional embedding (common.py:817-823)."""
+    """avg / max adaptive pooling mixed by LearnableWeights + positional embedding (common.py:817-823).  f32: fp32 tokens with
+    the fp32 pos_emb, and fp32 token gradients in the backward (the reference's autocast regime); else fp16 tokens."""
 
     @staticmethod
-    def forward(ctx, rgb, ir, pos_v, pos_i, w1v, w2v, w1i, w2i, nh: int, nw: int):
+    def forward(ctx, rgb, ir, pos_v, pos_i, w1v, w2v, w1i, w2i, nh: int, nw: int, f32: bool = False):
         mix = torch.cat([_f32(t).reshape(1) for t in (w1v, w2v, w1i, w2i)])
-        tv, ti = ops.dmff_pool_tokens(rgb, ir, pos_v.detach()[0].to(torch.float16).contiguous(), pos_i.detach()[0].to(torch.float16).contiguous(),
-                                      mix, nh, nw)
+        if f32:
+            tv, ti = ops.dmff_pool_tokens_f32(rgb, ir, _f32(pos_v[0]), _f32(pos_i[0]), mix, nh, nw)
+        else:
+            tv, ti = ops.dmff_pool_tokens(rgb, ir, pos_v.detach()[0].to(torch.float16).contiguous(),
+                                          pos_i.detach()[0].to(torch.float16).contiguous(), mix, nh, nw)
         ctx.save_for_backward(rgb, ir, mix)
-        ctx.cfg = (nh, nw, pos_v.dtype, w1v.dtype)
+        ctx.cfg = (nh, nw, pos_v.dtype, w1v.dtype, f32)
         return tv, ti
 
     @staticmethod
     def backward(ctx, dtv, dti):
         rgb, ir, mix = ctx.saved_tensors
-        nh, nw, pdt, wdt = ctx.cfg
+        nh, nw, pdt, wdt, f32 = ctx.cfg
         dtv, dti = dtv.contiguous(), dti.contiguous()
         B, n_pad, C = dtv.shape
         N = nh * nw
-        dx_v, dx_i = ops.dmff_pool_tokens_bwd(rgb, ir, dtv, dti, mix, nh, nw)
-        # positional embeddings: sum over the batch; mixing weights: <dtok, avg-pooled> and <dtok, max-pooled>
-        dpos = [ops.colsum(t.view(B, n_pad * C))[:N * C].view(1, N, C).to(pdt) for t in (dtv, dti)]
+        pool_bwd, colsum, dot = (ops.dmff_pool_tokens_bwd_f32, ops.colsum_f32, ops.dot_f32) if f32 else \
+            (ops.dmff_pool_tokens_bwd, ops.colsum, ops.dot)
+        dx_v, dx_i = pool_bwd(rgb, ir, dtv, dti, mix, nh, nw)
+        # positional embeddings: sum over the batch; mixing weights: <dtok, avg-pooled> and <dtok, max-pooled>, the pooled
+        # tokens fp16 in both regimes (torch's fp16 pooling returns fp16)
+        dpos = [colsum(t.view(B, n_pad * C))[:N * C].view(1, N, C).to(pdt) for t in (dtv, dti)]
         zero = torch.zeros(N, C, dtype=torch.float16, device=rgb.device)
         dev = rgb.device
         even = (torch.arange(4, device=dev) % 2 == 0).float()          # (1, 0, 1, 0), built on the device (graph-capture safe)
         avg = ops.dmff_pool_tokens(rgb, ir, zero, zero, even, nh, nw)
         mx = ops.dmff_pool_tokens(rgb, ir, zero, zero, 1.0 - even, nh, nw)
-        dw = [ops.dot(dtv, avg[0]), ops.dot(dtv, mx[0]), ops.dot(dti, avg[1]), ops.dot(dti, mx[1])]
+        dw = [dot(dtv, avg[0]), dot(dtv, mx[0]), dot(dti, avg[1]), dot(dti, mx[1])]
         return (dx_v if ctx.needs_input_grad[0] else None, dx_i if ctx.needs_input_grad[1] else None, dpos[0], dpos[1],
-                dw[0].to(wdt), dw[1].to(wdt), dw[2].to(wdt), dw[3].to(wdt), None, None)
+                dw[0].to(wdt), dw[1].to(wdt), dw[2].to(wdt), dw[3].to(wdt), None, None, None)
 
 
 class UpsampleCatFn(Function):
-    """tokens -> (nh,nw) map -> nearest resample to (H,W), + residual, concat over channels (common.py:827-840, training)."""
+    """tokens -> (nh,nw) map -> nearest resample to (H,W), + residual, concat over channels (common.py:827-840, training).
+    fp32 tokens: each sum is formed in fp32 and rounded once to the fp16 concat, and the token gradients are fp32."""
 
     @staticmethod
     def forward(ctx, tok_v, tok_i, rgb, ir, nh: int, nw: int):
-        ctx.cfg = (nh, nw, tok_v.shape[1], rgb.shape[3])
+        f32 = tok_v.dtype == torch.float32
+        ctx.cfg = (nh, nw, tok_v.shape[1], rgb.shape[3], f32)
+        if f32:
+            return ops.dmff_upsample_cat_f32(tok_v, tok_i, rgb, ir, nh, nw)
         return ops.dmff_upsample_cat(tok_v, tok_i, rgb, ir, nh, nw, mode=1)
 
     @staticmethod
     def backward(ctx, dcat):
-        nh, nw, n_pad, C = ctx.cfg
-        dt_v, dt_i = ops.dmff_upsample_cat_bwd(dcat, nh, nw, n_pad, mode=1)
+        nh, nw, n_pad, C, f32 = ctx.cfg
+        if f32:
+            dt_v, dt_i = ops.dmff_upsample_cat_bwd_f32(dcat, nh, nw, n_pad)
+        else:
+            dt_v, dt_i = ops.dmff_upsample_cat_bwd(dcat, nh, nw, n_pad, mode=1)
         return dt_v, dt_i, dcat[..., :C], dcat[..., C:], None, None
 
 
@@ -456,7 +485,8 @@ def _mlp(mlp: nn.Sequential, x, training: bool):
 
 
 def cross_transformer_block(m, r2, i2, B: int, N: int, n_pad: int):
-    """common.py:737-759"""
+    """common.py:737-759.  r2 / i2 carry the stream's precision (fp16, or fp32): the LayerNorms and coefficient pairs follow it,
+    and with loops > 1 the stream they return is fed back in the same precision."""
     c = [getattr(m, f"coefficient{j}").bias for j in range(1, 9)]
     for _ in range(m.loops):
         o_r, o_i = cross_attention(m.crossatt, r2, i2, B, N, n_pad)
@@ -468,20 +498,29 @@ def cross_transformer_block(m, r2, i2, B: int, N: int, n_pad: int):
 
 
 def fusion_block(m, rgb, ir):
-    """TransformerFusionBlock.forward in training mode (common.py:807-841)."""
+    """TransformerFusionBlock.forward in training mode (common.py:807-841), its token streams in ``m.stream_dtype``."""
+    f32 = stream_is_f32(m)
     B, H, W, C = rgb.shape
     nh, nw = m.avgpool.out_size(H, W)
     N = nh * nw
     if N != m.pos_emb_vis.shape[1]:
         raise ValueError(f"TransformerFusionBlock: {nh}x{nw} tokens but pos_emb has {m.pos_emb_vis.shape[1]} rows")
     tv, ti = PoolTokensFn.apply(rgb, ir, m.pos_emb_vis, m.pos_emb_ir, m.vis_coefficient.w1, m.vis_coefficient.w2,
-                                m.ir_coefficient.w1, m.ir_coefficient.w2, nh, nw)
+                                m.ir_coefficient.w1, m.ir_coefficient.w2, nh, nw, f32)
     n_pad = tv.shape[1]
     r2, i2 = tv.view(B * n_pad, C), ti.view(B * n_pad, C)
     for blk in m.crosstransformer:
         r2, i2 = cross_transformer_block(blk, r2, i2, B, N, n_pad)
     cat = UpsampleCatFn.apply(r2.view(B, n_pad, C), i2.view(B, n_pad, C), rgb, ir, nh, nw)
     return conv_bn_act(m.conv1x1_out, cat)
+
+
+def stream_is_f32(m) -> bool:
+    """True when the TransformerFusionBlock `m` trains with fp32 token streams (``stream_dtype``: torch.float16 or float32)."""
+    dt = getattr(m, "stream_dtype", torch.float16)
+    if dt not in (torch.float16, torch.float32):
+        raise ValueError(f"TransformerFusionBlock.stream_dtype: torch.float16 or torch.float32, got {dt}")
+    return dt == torch.float32
 
 
 def detect(m, xs: Sequence[torch.Tensor]) -> List[torch.Tensor]:

@@ -546,7 +546,14 @@ class CrossTransformerBlock(nn.Module):
 
 
 class TransformerFusionBlock(nn.Module):
-    """The DMFF block (reference: models/common.py:762-865)."""
+    """The DMFF block (reference: models/common.py:762-865).
+
+    ``stream_dtype`` (training only; not part of the state_dict): torch.float16 keeps the token streams and their gradients in
+    fp16; torch.float32 keeps them in fp32 from the pooling to the upsample-and-add, the precision the reference's autocast
+    gives them (an fp32 LearnableWeights / LearnableCoefficient parameter times an fp16 tensor promotes to fp32), with fp16
+    GEMM operands.  TrainStep(dmff_fp32=True) sets it on every block; eval() ignores it."""
+
+    stream_dtype = torch.float16
 
     def __init__(self, d_model, vert_anchors=16, horz_anchors=16, h=8, block_exp=4, n_layer=1, embd_pdrop=0.1,
                  attn_pdrop=0.1, resid_pdrop=0.1):

@@ -353,6 +353,15 @@ __device__ __forceinline__ void ld8f(const float* __restrict__ p, float (&v)[8])
   const float4 a = __ldg(reinterpret_cast<const float4*>(p)), b = __ldg(reinterpret_cast<const float4*>(p) + 1);
   v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
 }
+// 8 consecutive values of an fp16 or an fp32 tensor as fp32 (load), and back (store, rounded to nearest for fp16): the kernels
+// that serve both DMFF token-stream precisions are templates over the stream's element type
+__device__ __forceinline__ void ld8(const __half* p, float (&v)[8]) { unpack8(ldg16(p), v); }
+__device__ __forceinline__ void ld8(const float* p, float (&v)[8]) { ld8f(p, v); }
+__device__ __forceinline__ void st8(__half* p, const float (&v)[8]) { *reinterpret_cast<uint4*>(p) = pack8(v); }
+__device__ __forceinline__ void st8(float* p, const float (&v)[8]) {
+  reinterpret_cast<float4*>(p)[0] = make_float4(v[0], v[1], v[2], v[3]);
+  reinterpret_cast<float4*>(p)[1] = make_float4(v[4], v[5], v[6], v[7]);
+}
 
 // Coordinates of 16-byte vector i of a (B, H, W, 8 * C8) NHWC map: channel chunk c of pixel p = (b * H + y) * W + x
 struct Nhwc8 { int c; long long p; int x, y, b; };
@@ -370,17 +379,18 @@ __device__ __forceinline__ uint2 pack_argmax8(const uint32_t (&arg)[8]) {
 }
 __device__ __forceinline__ uint32_t argmax_code(const uint2& cd, int e) { return ((e < 4 ? cd.x : cd.y) >> (8 * (e & 3))) & 0xffu; }
 
-// LayerNorm statistics of row `row` of a (rows, C <= 2048) fp16 matrix, one warp per row (the forward and the backward share
-// them): lane l caches the row's 16-byte chunks l, l + 32, ... in v[0..7]; every lane gets the mean and 1 / sqrt(var + eps),
-// the variance taken in a second pass over the registers.
-__device__ __forceinline__ void ln_row_moments(const __half* x, long long row, int C, float eps, float (&v)[8][8], float& mean, float& rstd) {
+// LayerNorm statistics of row `row` of a (rows, C <= 2048) fp16 or fp32 matrix, one warp per row (the forward and the backward
+// share them): lane l caches the row's 8-channel chunks l, l + 32, ... in v[0..7]; every lane gets the mean and
+// 1 / sqrt(var + eps), the variance taken in a second pass over the registers.
+template <typename T>
+__device__ __forceinline__ void ln_row_moments(const T* x, long long row, int C, float eps, float (&v)[8][8], float& mean, float& rstd) {
   const int lane = threadIdx.x & 31, nch = C >> 3;
   float s = 0.f;
 #pragma unroll
   for (int j = 0; j < 8; ++j) {
     const int ch = lane + 32 * j;
     if (ch < nch) {
-      unpack8(ldg16(x + row * C + ch * 8), v[j]);
+      ld8(x + row * C + ch * 8, v[j]);
 #pragma unroll
       for (int e = 0; e < 8; ++e) s += v[j][e];
     }

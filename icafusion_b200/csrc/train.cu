@@ -15,8 +15,9 @@ __device__ __forceinline__ float sigmoidf_(float z) { return __fdividef(1.f, 1.f
 // per-channel partial sums over row chunks: out[chunk][which][c], which = 0 / 1.
 // MODE 0: (x, x^2)  [BatchNorm statistics]      MODE 1: (dz, dz * xhat) with dz = dy * silu'(x*a + b)  [BN + SiLU backward]
 // MODE 2: (dy, dy * xhat_row) with per-ROW (mean, rstd)  [LayerNorm gamma / beta gradients]   MODE 3: (x * y, 0)  [dot products]
-template <int MODE>
-__global__ void __launch_bounds__(256) chan_partial_kernel(const __half* __restrict__ x, const __half* __restrict__ dy, const float* __restrict__ a,
+// TX / TY: element types of x / dy (fp16; x fp32 and dy fp16 or fp32 for an fp32 DMFF token stream)
+template <int MODE, typename TX = __half, typename TY = __half>
+__global__ void __launch_bounds__(256) chan_partial_kernel(const TX* __restrict__ x, const TY* __restrict__ dy, const float* __restrict__ a,
                                                            const float* __restrict__ b, const float* __restrict__ mean, const float* __restrict__ invstd,
                                                            float* __restrict__ out, long long rows, int C, int act, int chunks) {
   pdl_launch_dependents();
@@ -49,14 +50,14 @@ __global__ void __launch_bounds__(256) chan_partial_kernel(const __half* __restr
       const long long rb = r + rpp;
       const bool two = rb < r1;
       float xv[2][8], dv[2][8];
-      const uint4 xa = ldg16(x + r * C + cg * 8);
-      const uint4 xb = two ? ldg16(x + rb * C + cg * 8) : make_uint4(0, 0, 0, 0);
-      uint4 da = make_uint4(0, 0, 0, 0), db = make_uint4(0, 0, 0, 0);
+#pragma unroll
+      for (int e = 0; e < 8; ++e) xv[1][e] = dv[0][e] = dv[1][e] = 0.f;
+      ld8(x + r * C + cg * 8, xv[0]);
+      if (two) ld8(x + rb * C + cg * 8, xv[1]);
       if (MODE != 0) {
-        da = ldg16(dy + r * C + cg * 8);
-        if (two) db = ldg16(dy + rb * C + cg * 8);
+        ld8(dy + r * C + cg * 8, dv[0]);
+        if (two) ld8(dy + rb * C + cg * 8, dv[1]);
       }
-      unpack8(xa, xv[0]); unpack8(xb, xv[1]); unpack8(da, dv[0]); unpack8(db, dv[1]);
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         if (h == 1 && !two) break;
@@ -249,8 +250,10 @@ __global__ void eltwise_kernel(const __half* __restrict__ x, const __half* __res
   reinterpret_cast<uint4*>(y)[i] = pack8(xv);
 }
 
-// LayerNorm backward, dx part (one warp per row, C <= 2048): dx = rstd * (g - mean(g) - xhat * mean(g * xhat)), g = dy * gamma
-__global__ void ln_bwd_kernel(const __half* __restrict__ x, const __half* __restrict__ dy, const float* __restrict__ gamma, __half* __restrict__ dx,
+// LayerNorm backward, dx part (one warp per row, C <= 2048): dx = rstd * (g - mean(g) - xhat * mean(g * xhat)), g = dy * gamma.
+// T: element type of x and dx (fp32 for an fp32 DMFF token stream, whose LayerNorm output is the fp16 GEMM operand: dy is fp16)
+template <typename T>
+__global__ void ln_bwd_kernel(const T* __restrict__ x, const __half* __restrict__ dy, const float* __restrict__ gamma, T* __restrict__ dx,
                               float* __restrict__ row_mean, float* __restrict__ row_rstd, long long rows, int C, float eps) {
   pdl_launch_dependents();
   pdl_wait();
@@ -283,7 +286,7 @@ __global__ void ln_bwd_kernel(const __half* __restrict__ x, const __half* __rest
       float o[8];
 #pragma unroll
       for (int e = 0; e < 8; ++e) o[e] = rstd * (gv[j][e] - sg - xv[j][e] * sgx);
-      *reinterpret_cast<uint4*>(dx + row * C + ch * 8) = pack8(o);
+      st8(dx + row * C + ch * 8, o);
     }
   }
   if (lane == 0) { row_mean[row] = mean; row_rstd[row] = rstd; }
@@ -413,26 +416,42 @@ extern "C" int icaf_eltwise(int mode, const void* x, const void* dy, void* y, in
                   seed_offset_ptr());
 }
 
+// LayerNorm backward launches: dx (and the row statistics), then dgamma / dbeta as a two-stage channel reduction
+template <typename T>
+static int layernorm_bwd_launch(const T* x, const __half* dy, const float* gamma, T* dx, float* dgamma, float* dbeta, int64_t rows, int C, float eps,
+                                float grad_scale, int accumulate, float* workspace, cudaStream_t st) {
+  constexpr bool f32 = sizeof(T) == 4;
+  float* rmean = workspace + ws_floats(C);
+  float* rrstd = rmean + rows;
+  if (int rc = launch_k(f32 ? "layernorm_bwd_f32(dx)" : "layernorm_bwd(dx)", ln_bwd_kernel<T>, dim3(blocks_for(rows, 4)), dim3(128), 0, st, x, dy,
+                        gamma, dx, rmean, rrstd, (long long)rows, C, eps)) return rc;
+  if (dgamma || dbeta) {
+    const int chunks = pick_chunks(rows, C);
+    if (int rc = launch_k(f32 ? "layernorm_bwd_f32(partial)" : "layernorm_bwd(partial)", chan_partial_kernel<2, T, __half>,
+                          dim3(blocks_for(C / 8, 32), chunks), dim3(256), 0, st, x, dy, (const float*)nullptr, (const float*)nullptr,
+                          (const float*)rmean, (const float*)rrstd, workspace, (long long)rows, C, 0, chunks)) return rc;
+    if (int rc = launch_k(f32 ? "layernorm_bwd_f32(param grads)" : "layernorm_bwd(param grads)", chan_final_kernel<false>, dim3(blocks_for(C, 32)),
+                          dim3(32, kFinLanes), 0, st, (const float*)workspace, dbeta, dgamma, C, grad_scale, accumulate, chunks, (float*)nullptr,
+                          (float*)nullptr, (const float*)nullptr, (const float*)nullptr, (const float*)nullptr, (const float*)nullptr, 0.f,
+                          (float*)nullptr, (const float*)nullptr, (float*)nullptr, 0.f)) return rc;
+  }
+  return ICAF_OK;
+}
+
 extern "C" int icaf_layernorm_bwd(const void* x, const void* dy, const float* gamma, void* dx, float* dgamma, float* dbeta, int64_t rows, int C, float eps,
                                   float grad_scale, int accumulate, float* workspace, size_t workspace_bytes, void* stream) {
   if (!x || !dy || !gamma || !dx || !workspace || rows < 1 || C % 8 || C > 2048) return set_error(ICAF_ERR_BAD_ARG, "layernorm_bwd: bad argument (C % 8, C <= 2048)");
   if (workspace_bytes < icaf_train_workspace_bytes(C) + 2 * size_t(rows) * sizeof(float)) return set_error(ICAF_ERR_BAD_ARG, "layernorm_bwd: workspace too small (icaf_train_workspace_bytes + 2 rows floats)");
-  cudaStream_t st = (cudaStream_t)stream;
-  float* rmean = workspace + ws_floats(C);
-  float* rrstd = rmean + rows;
-  if (int rc = launch_k("layernorm_bwd(dx)", ln_bwd_kernel, dim3(blocks_for(rows, 4)), dim3(128), 0, st, (const __half*)x, (const __half*)dy, gamma,
-                        (__half*)dx, rmean, rrstd, (long long)rows, C, eps)) return rc;
-  if (dgamma || dbeta) {
-    const int chunks = pick_chunks(rows, C);
-    if (int rc = launch_k("layernorm_bwd(partial)", chan_partial_kernel<2>, dim3(blocks_for(C / 8, 32), chunks), dim3(256), 0, st, (const __half*)x,
-                          (const __half*)dy, (const float*)nullptr, (const float*)nullptr, (const float*)rmean, (const float*)rrstd, workspace,
-                          (long long)rows, C, 0, chunks)) return rc;
-    if (int rc = launch_k("layernorm_bwd(param grads)", chan_final_kernel<false>, dim3(blocks_for(C, 32)), dim3(32, kFinLanes), 0, st,
-                          (const float*)workspace, dbeta, dgamma, C, grad_scale, accumulate, chunks, (float*)nullptr, (float*)nullptr,
-                          (const float*)nullptr, (const float*)nullptr, (const float*)nullptr, (const float*)nullptr, 0.f, (float*)nullptr,
-                          (const float*)nullptr, (float*)nullptr, 0.f)) return rc;
-  }
-  return ICAF_OK;
+  return layernorm_bwd_launch((const __half*)x, (const __half*)dy, gamma, (__half*)dx, dgamma, dbeta, rows, C, eps, grad_scale, accumulate, workspace,
+                              (cudaStream_t)stream);
+}
+
+// fp32 token stream: x and dx fp32, dy fp16 (the data gradient of the GEMM the LayerNorm output feeds)
+extern "C" int icaf_layernorm_bwd_f32(const float* x, const void* dy, const float* gamma, float* dx, float* dgamma, float* dbeta, int64_t rows, int C,
+                                      float eps, float grad_scale, int accumulate, float* workspace, size_t workspace_bytes, void* stream) {
+  if (!x || !dy || !gamma || !dx || !workspace || rows < 1 || C % 8 || C > 2048) return set_error(ICAF_ERR_BAD_ARG, "layernorm_bwd_f32: bad argument (C % 8, C <= 2048)");
+  if (workspace_bytes < icaf_train_workspace_bytes(C) + 2 * size_t(rows) * sizeof(float)) return set_error(ICAF_ERR_BAD_ARG, "layernorm_bwd_f32: workspace too small (icaf_train_workspace_bytes + 2 rows floats)");
+  return layernorm_bwd_launch(x, (const __half*)dy, gamma, dx, dgamma, dbeta, rows, C, eps, grad_scale, accumulate, workspace, (cudaStream_t)stream);
 }
 
 // out[0] = (accumulate ? out[0] : 0) + scale * <x, y> over (rows, C) fp16 matrices (gradients of the scalar gains)
@@ -446,4 +465,23 @@ extern "C" int icaf_dot(const void* x, const void* y, int64_t rows, int C, float
                         (const __half*)y, (const float*)nullptr, (const float*)nullptr, (const float*)nullptr, (const float*)nullptr, workspace,
                         (long long)rows, C, 0, chunks)) return rc;
   return launch_k("dot", scalar_final_kernel, dim3(1), dim3(1024), 0, st, (const float*)workspace, out, C, scale, accumulate, chunks);
+}
+
+// out[0] = (accumulate ? out[0] : 0) + scale * <x, y> with x an fp32 (rows, C) matrix and y fp16 (y_f16) or fp32: the gradients of
+// the scalar gains along an fp32 DMFF token stream, in the fixed order of icaf_dot
+extern "C" int icaf_dot_f32(const float* x, const void* y, int y_f16, int64_t rows, int C, float* out, float scale, int accumulate, float* workspace,
+                            size_t workspace_bytes, void* stream) {
+  if (!x || !y || !out || !workspace || rows < 1 || C < 8 || C % 8) return set_error(ICAF_ERR_BAD_ARG, "dot_f32: bad argument");
+  if (workspace_bytes < icaf_train_workspace_bytes(C)) return set_error(ICAF_ERR_BAD_ARG, "dot_f32: workspace too small");
+  cudaStream_t st = (cudaStream_t)stream;
+  const int chunks = pick_chunks(rows, C, 64);
+  const dim3 grid(blocks_for(C / 8, 32), chunks);
+  const int rc = y_f16 ? launch_k("dot_f32(partial)", chan_partial_kernel<3, float, __half>, grid, dim3(256), 0, st, x, (const __half*)y,
+                                  (const float*)nullptr, (const float*)nullptr, (const float*)nullptr, (const float*)nullptr, workspace,
+                                  (long long)rows, C, 0, chunks)
+                       : launch_k("dot_f32(partial)", chan_partial_kernel<3, float, float>, grid, dim3(256), 0, st, x, (const float*)y,
+                                  (const float*)nullptr, (const float*)nullptr, (const float*)nullptr, (const float*)nullptr, workspace,
+                                  (long long)rows, C, 0, chunks);
+  if (rc) return rc;
+  return launch_k("dot_f32", scalar_final_kernel, dim3(1), dim3(1024), 0, st, (const float*)workspace, out, C, scale, accumulate, chunks);
 }

@@ -214,8 +214,12 @@ __global__ void zero_stuff2_kernel(const __half* __restrict__ x, __half* __restr
   *reinterpret_cast<uint4*>(y + i * 8) = v;
 }
 
-// column sums of a (rows, C) fp16 matrix in fp32 (bias gradients): fixed chunks per block, fixed-order second stage
-__global__ void colsum_partial_kernel(const __half* __restrict__ x, float* __restrict__ part, long long rows, int C, int chunks) {
+// column sums of a (rows, C) fp16 (or fp32) matrix in fp32 (bias gradients; positional-embedding gradients of an fp32 DMFF token
+// stream): fixed chunks per block, fixed-order second stage
+__device__ __forceinline__ float to_f32(__half v) { return __half2float(v); }
+__device__ __forceinline__ float to_f32(float v) { return v; }
+template <typename T>
+__global__ void colsum_partial_kernel(const T* __restrict__ x, float* __restrict__ part, long long rows, int C, int chunks) {
   pdl_launch_dependents();
   pdl_wait();
   const int c = blockIdx.x * blockDim.x + threadIdx.x;
@@ -223,7 +227,7 @@ __global__ void colsum_partial_kernel(const __half* __restrict__ x, float* __res
   const long long per = (rows + chunks - 1) / chunks;
   const long long r0 = blockIdx.y * per, r1 = min(r0 + per, rows);
   float s = 0.f;
-  for (long long r = r0; r < r1; ++r) s += __half2float(x[r * C + c]);
+  for (long long r = r0; r < r1; ++r) s += to_f32(x[r * C + c]);
   part[size_t(blockIdx.y) * C + c] = s;
 }
 __global__ void colsum_final_kernel(const float* __restrict__ part, float* __restrict__ out, int C, int chunks, float scale, int accumulate) {
@@ -370,9 +374,21 @@ extern "C" int icaf_colsum(const void* x, int64_t rows, int C, float* out, float
   if (!x || !out || !workspace || rows < 1 || C < 1) return set_error(ICAF_ERR_BAD_ARG, "colsum: bad argument");
   if (workspace_bytes < size_t(kChunks) * C * sizeof(float)) return set_error(ICAF_ERR_BAD_ARG, "colsum: workspace needs 64 * C floats");
   cudaStream_t st = (cudaStream_t)stream;
-  if (int rc = launch_k("colsum(partial)", colsum_partial_kernel, dim3(blocks_for(C, 128), kChunks), dim3(128), 0, st, (const __half*)x, workspace,
+  if (int rc = launch_k("colsum(partial)", colsum_partial_kernel<__half>, dim3(blocks_for(C, 128), kChunks), dim3(128), 0, st, (const __half*)x, workspace,
                         (long long)rows, C, kChunks)) return rc;
   return launch_k("colsum", colsum_final_kernel, dim3(blocks_for(C, 128)), dim3(128), 0, st, (const float*)workspace, out, C, kChunks, scale,
+                  accumulate);
+}
+
+extern "C" int icaf_colsum_f32(const float* x, int64_t rows, int C, float* out, float scale, int accumulate, float* workspace, size_t workspace_bytes,
+                               void* stream) {
+  constexpr int kChunks = 64;
+  if (!x || !out || !workspace || rows < 1 || C < 1) return set_error(ICAF_ERR_BAD_ARG, "colsum_f32: bad argument");
+  if (workspace_bytes < size_t(kChunks) * C * sizeof(float)) return set_error(ICAF_ERR_BAD_ARG, "colsum_f32: workspace needs 64 * C floats");
+  cudaStream_t st = (cudaStream_t)stream;
+  if (int rc = launch_k("colsum_f32(partial)", colsum_partial_kernel<float>, dim3(blocks_for(C, 128), kChunks), dim3(128), 0, st, x, workspace,
+                        (long long)rows, C, kChunks)) return rc;
+  return launch_k("colsum_f32", colsum_final_kernel, dim3(blocks_for(C, 128)), dim3(128), 0, st, (const float*)workspace, out, C, kChunks, scale,
                   accumulate);
 }
 

@@ -652,6 +652,178 @@ def axpby(x: torch.Tensor, a: torch.Tensor, y: Optional[torch.Tensor] = None, b:
     return out
 
 
+# ------------------------------------------------------------------------------------------------
+# fp32 DMFF token streams (training with TransformerFusionBlock.stream_dtype = float32): the reference's autocast makes its token
+# streams fp32 from the pooling to the upsample-and-add.  Tokens and token gradients are fp32 here; maps, map gradients and
+# GEMM operands stay fp16.  Every wrapper checks each operand's dtype: the C ABI takes untyped pointers.
+def _need(t: torch.Tensor, dtype, what: str, shape=None) -> torch.Tensor:
+    if not torch.is_tensor(t) or t.dtype != dtype or not on_device(t):
+        raise ValueError(f"{what}: expected a CUDA {dtype} tensor, got "
+                         f"{(t.dtype, t.device) if torch.is_tensor(t) else type(t).__name__}")
+    if shape is not None and tuple(t.shape) != tuple(shape):
+        raise ValueError(f"{what}: expected shape {tuple(shape)}, got {tuple(t.shape)}")
+    return t
+
+
+def _need_contig(t: torch.Tensor, dtype, what: str, shape=None) -> torch.Tensor:
+    _need(t, dtype, what, shape)
+    if not t.is_contiguous():
+        raise ValueError(f"{what}: must be contiguous")
+    return t
+
+
+def dmff_pool_tokens_f32(x_vis, x_ir, pos_vis, pos_ir, mix, nh: int, nw: int):
+    """dmff_pool_tokens over an fp32 stream: fp16 maps, fp32 (N, C) position embeddings -> fp32 (B, Npad, C) tokens."""
+    B, H, W, Cc = x_vis.shape
+    ld = _check_view(x_vis, "dmff x_vis")
+    if tuple(x_ir.shape) != tuple(x_vis.shape) or _check_view(x_ir, "dmff x_ir") != ld:
+        raise ValueError("dmff_pool_tokens_f32: the two feature maps must share shape and pitch")
+    for t, w in ((pos_vis, "pos_vis"), (pos_ir, "pos_ir")):
+        _need_contig(t, torch.float32, f"dmff_pool_tokens_f32 {w}", (nh * nw, Cc))
+    _need_contig(mix, torch.float32, "dmff_pool_tokens_f32 mix", (4,))
+    n_pad = round_up(nh * nw, 8)
+    tv = torch.empty(B, n_pad, Cc, dtype=torch.float32, device=x_vis.device)
+    ti = torch.empty_like(tv)
+    _call("icaf_dmff_pool_tokens_f32", _lib.lib().icaf_dmff_pool_tokens_f32,
+          (_ptr(x_vis), _ptr(x_ir), ld, _ptr(pos_vis), _ptr(pos_ir), _ptr(mix), _ptr(tv), _ptr(ti), B, H, W, Cc, nh, nw, n_pad),
+          {"bytes": 4.0 * x_vis.numel() + 8.0 * tv.numel() + 8.0 * pos_vis.numel()})
+    return tv, ti
+
+
+def dmff_pool_tokens_bwd_f32(x_vis, x_ir, dtok_vis, dtok_ir, mix, nh: int, nw: int):
+    """Gradients of dmff_pool_tokens_f32 w.r.t. the two fp16 NHWC maps, from fp32 token gradients."""
+    B, H, W, Cc = x_vis.shape
+    ld = _check_view(x_vis, "dmff x_vis")
+    if tuple(x_ir.shape) != tuple(x_vis.shape) or _check_view(x_ir, "dmff x_ir") != ld:
+        raise ValueError("dmff_pool_tokens_bwd_f32: the two feature maps must share shape and pitch")
+    n_pad = dtok_vis.shape[1]
+    for t, w in ((dtok_vis, "dtok_vis"), (dtok_ir, "dtok_ir")):
+        _need_contig(t, torch.float32, f"dmff_pool_tokens_bwd_f32 {w}", (B, n_pad, Cc))
+    _need_contig(mix, torch.float32, "dmff_pool_tokens_bwd_f32 mix", (4,))
+    dx_v = torch.empty(B, H, W, Cc, dtype=torch.float16, device=x_vis.device)
+    dx_i = torch.empty_like(dx_v)
+    ws = torch.empty((2 * B * nh * nw * Cc + 7) // 8, dtype=torch.int64, device=x_vis.device)
+    _call("icaf_dmff_pool_tokens_bwd_f32", _lib.lib().icaf_dmff_pool_tokens_bwd_f32,
+          (_ptr(x_vis), _ptr(x_ir), ld, _ptr(dtok_vis), _ptr(dtok_ir), _ptr(mix), _ptr(dx_v), _ptr(dx_i), B, H, W, Cc, nh, nw, n_pad, _ptr(ws),
+           C.c_size_t(ws.numel() * 8)),
+          {"bytes": 2.0 * 2 * 2 * x_vis.numel() + 4.0 * 2 * dtok_vis.numel()})
+    return dx_v, dx_i
+
+
+def dmff_upsample_cat_f32(tok_vis, tok_ir, x_vis, x_ir, nh: int, nw: int) -> torch.Tensor:
+    """The training-mode (nearest) tail over fp32 tokens: fp16 (B, H, W, 2C) = [up(tok_vis) + x_vis | up(tok_ir) + x_ir], each sum
+    formed in fp32 and rounded once."""
+    B, H, W, Cc = x_vis.shape
+    ld = _check_view(x_vis, "dmff x_vis")
+    if tuple(x_ir.shape) != tuple(x_vis.shape) or _check_view(x_ir, "dmff x_ir") != ld:
+        raise ValueError("dmff_upsample_cat_f32: the two feature maps must share shape and pitch")
+    n_pad = tok_vis.shape[1]
+    if n_pad < nh * nw:
+        raise ValueError(f"dmff_upsample_cat_f32: {n_pad} token rows for a {nh}x{nw} grid")
+    for t, w in ((tok_vis, "tok_vis"), (tok_ir, "tok_ir")):
+        _need_contig(t, torch.float32, f"dmff_upsample_cat_f32 {w}", (B, n_pad, Cc))
+    out = torch.empty(B, H, W, 2 * Cc, dtype=torch.float16, device=x_vis.device)
+    _call("icaf_dmff_upsample_cat_f32", _lib.lib().icaf_dmff_upsample_cat_f32,
+          (_ptr(tok_vis), _ptr(tok_ir), n_pad, _ptr(x_vis), _ptr(x_ir), ld, _ptr(out), 2 * Cc, B, H, W, Cc, nh, nw),
+          {"bytes": 2.0 * (2 * x_vis.numel() + out.numel()) + 4.0 * 2 * tok_vis.numel()})
+    return out
+
+
+def dmff_upsample_cat_bwd_f32(dcat: torch.Tensor, nh: int, nw: int, n_pad: int):
+    """fp32 token-stream gradients of dmff_upsample_cat_f32; dcat: fp16 (B,H,W,2C) NHWC view."""
+    B, H, W, C2 = dcat.shape
+    Cc = C2 // 2
+    ld = _check_view(dcat, "dmff dcat")
+    dt_v = torch.empty(B, n_pad, Cc, dtype=torch.float32, device=dcat.device)
+    dt_i = torch.empty_like(dt_v)
+    _call("icaf_dmff_upsample_cat_bwd_f32", _lib.lib().icaf_dmff_upsample_cat_bwd_f32,
+          (_ptr(dcat), ld, _ptr(dt_v), _ptr(dt_i), B, H, W, Cc, nh, nw, n_pad), {"bytes": 2.0 * dcat.numel() + 8.0 * dt_v.numel()})
+    return dt_v, dt_i
+
+
+def layernorm_f32(x: torch.Tensor, g: torch.Tensor, b: torch.Tensor, eps: float = 1e-5) -> torch.Tensor:
+    """LayerNorm over the last dim of an fp32 contiguous (.., C) tensor -> fp16 (the fp32 LayerNorm, rounded once)."""
+    _need_contig(x, torch.float32, "layernorm_f32 x")
+    Cc = x.shape[-1]
+    for t, w in ((g, "gamma"), (b, "beta")):
+        _need_contig(t, torch.float32, f"layernorm_f32 {w}", (Cc,))
+    y = torch.empty(x.shape, dtype=torch.float16, device=x.device)
+    _call("icaf_layernorm_f32", _lib.lib().icaf_layernorm_f32,
+          (_ptr(x), _ptr(None), _ptr(g), _ptr(b), _ptr(None), _ptr(None), _ptr(y), _ptr(None), x.numel() // Cc, Cc, float(eps)),
+          {"bytes": 6.0 * x.numel()})
+    return y
+
+
+def layernorm_bwd_f32(x, dy, gamma, eps: float, dgamma=None, dbeta=None, grad_scale: float = 1.0, accumulate: bool = False):
+    """LayerNorm backward with fp32 x, fp16 dy -> fp32 dx; dgamma / dbeta (fp32 [C]) when given."""
+    _need_contig(x, torch.float32, "layernorm_bwd_f32 x")
+    Cc = x.shape[-1]
+    rows = x.numel() // Cc
+    dy = _need(dy, torch.float16, "layernorm_bwd_f32 dy", x.shape).contiguous()
+    _need_contig(gamma, torch.float32, "layernorm_bwd_f32 gamma", (Cc,))
+    for t, w in ((dgamma, "dgamma"), (dbeta, "dbeta")):
+        if t is not None:
+            _need_contig(t, torch.float32, f"layernorm_bwd_f32 {w}", (Cc,))
+    dx = torch.empty_like(x)
+    ws = _train_ws(Cc, 2 * rows, x.device)
+    _call("icaf_layernorm_bwd_f32", _lib.lib().icaf_layernorm_bwd_f32,
+          (_ptr(x), _ptr(dy), _ptr(gamma), _ptr(dx), _ptr(dgamma), _ptr(dbeta), rows, Cc, float(eps), float(grad_scale), int(accumulate), _ptr(ws),
+           C.c_size_t(ws.numel() * 4)), {"bytes": 14.0 * x.numel()})
+    return dx
+
+
+def axpby_f32(x: torch.Tensor, a: torch.Tensor, y: Optional[torch.Tensor] = None, b: Optional[torch.Tensor] = None,
+              out_dtype=torch.float32) -> torch.Tensor:
+    """out = a*x (+ b*y) with x fp32, y fp16: torch's fp32 `a * x + b * y` bit for bit (a coefficient pair of an fp32 token
+    stream, common.py:747-750); out fp32, or fp16 (the backward's gradient of an fp16 branch output)."""
+    x = _need(x, torch.float32, "axpby_f32 x").contiguous()
+    if out_dtype not in (torch.float32, torch.float16):
+        raise ValueError(f"axpby_f32: output dtype float32 or float16, got {out_dtype}")
+    n = x.numel()
+    if n % 8:
+        raise ValueError("axpby_f32: element count must be a multiple of 8")
+    _need(a, torch.float32, "axpby_f32 a", (1,))
+    if y is not None:
+        y = _need(y, torch.float16, "axpby_f32 y", x.shape).contiguous()
+        _need(b, torch.float32, "axpby_f32 b", (1,))
+    out = torch.empty(x.shape, dtype=out_dtype, device=x.device)
+    _call("icaf_axpby_f32", _lib.lib().icaf_axpby_f32, (_ptr(x), _ptr(y), _ptr(a), _ptr(b), _ptr(out), int(out_dtype == torch.float16), n),
+          {"bytes": n * (4.0 + out.element_size() + (2.0 if y is not None else 0.0))})
+    return out
+
+
+def dot_f32(x: torch.Tensor, y: torch.Tensor, out: Optional[torch.Tensor] = None, scale: float = 1.0):
+    """<x, y> (fp32, one element) with x fp32 and y fp16 or fp32 of x's shape; accumulates into `out` when given."""
+    x = _need(x, torch.float32, "dot_f32 x").contiguous()
+    if not torch.is_tensor(y) or y.dtype not in (torch.float16, torch.float32):
+        raise ValueError("dot_f32: y must be an fp16 or fp32 tensor")
+    y = _need(y, y.dtype, "dot_f32 y", x.shape).contiguous()
+    Cc = x.shape[-1]
+    acc = out is not None
+    if out is None:
+        out = torch.empty(1, dtype=torch.float32, device=x.device)
+    _need(out, torch.float32, "dot_f32 out", (1,))
+    ws = _train_ws(Cc, 0, x.device)
+    _call("icaf_dot_f32", _lib.lib().icaf_dot_f32, (_ptr(x), _ptr(y), int(y.dtype == torch.float16), x.numel() // Cc, Cc, _ptr(out), float(scale),
+                                                   int(acc), _ptr(ws), C.c_size_t(ws.numel() * 4)),
+          {"bytes": (4.0 + y.element_size()) * x.numel()})
+    return out
+
+
+def colsum_f32(x: torch.Tensor, scale: float = 1.0, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """Column sums (fp32) of a dense fp32 (rows, C) matrix; accumulates into `out` when given."""
+    _need_contig(x, torch.float32, "colsum_f32 x")
+    rows, Cc = x.shape
+    acc = out is not None
+    if out is None:
+        out = torch.empty(Cc, dtype=torch.float32, device=x.device)
+    _need(out, torch.float32, "colsum_f32 out", (Cc,))
+    ws = torch.empty(64 * Cc, dtype=torch.float32, device=x.device)
+    _call("icaf_colsum_f32", _lib.lib().icaf_colsum_f32, (_ptr(x), rows, Cc, _ptr(out), float(scale), int(acc), _ptr(ws), C.c_size_t(ws.numel() * 4)),
+          {"bytes": 4.0 * x.numel()})
+    return out
+
+
 def nms_workspace_bytes(B: int, R: int, no: int, multi_label: bool = False) -> int:
     """Device workspace :func:`nms` needs for a (B, R, no) prediction tensor (multi_label only counts when nc = no - 5 > 1)."""
     if multi_label and no - 5 > 1:

@@ -23,7 +23,7 @@ import torch
 import torch.nn as nn
 
 from . import _lib
-from .common import CrossTransformerBlock
+from .common import CrossTransformerBlock, TransformerFusionBlock
 from .loss import ComputeLoss
 
 HYP_SCRATCH = dict(lr0=0.01, momentum=0.937, weight_decay=0.0005, box=0.05, cls=0.5, cls_pw=1.0, obj=1.0, obj_pw=1.0, anchor_t=4.0,
@@ -65,6 +65,13 @@ def param_groups(model: nn.Module):
     # (like the reference, parameters that are neither .weight nor .bias -- pos_emb, LearnableWeights.w1/w2 -- join no group;
     #  LearnableCoefficient.bias lands in the bias group)
     return pg0, pg1, pg2
+
+
+def set_dmff_stream_dtype(model: nn.Module, fp32: bool) -> None:
+    """Train every DMFF block of `model` with fp32 token streams (fp32) or fp16 ones: TransformerFusionBlock.stream_dtype."""
+    for m in model.modules():
+        if isinstance(m, TransformerFusionBlock):
+            m.stream_dtype = torch.float32 if fp32 else torch.float16
 
 
 class ModelEMA:
@@ -117,12 +124,19 @@ class TrainStep:
 
     sync_bn (train.py --sync-bn): with world_size > 1, every BatchNorm2d is converted to nn.SyncBatchNorm after the optimiser
     groups are built and before the DDP wrap (train.py:195-198), so BatchNorm normalises over the batch of all ranks.  At
-    world size 1 the model is left as it is.  A model the caller converted beforehand trains synchronised as well."""
+    world size 1 the model is left as it is.  A model the caller converted beforehand trains synchronised as well.
+
+    dmff_fp32: True gives every TransformerFusionBlock fp32 token streams and stream gradients (stream_dtype): the dtype
+    each DMFF node has in the reference's autocast step, with fp16 GEMM operands.  False gives them fp16 streams; None (the
+    default) keeps each block's stream_dtype as it is (fp16 unless the caller set it).  The precision of the whole step's
+    one-element DMFF gradients is measured, per model, in DESIGN.md section 4.6."""
 
     def __init__(self, model: nn.Module, hyp: Optional[Dict[str, float]] = None, total_batch_size: int = 64, world_size: int = 1,
                  local_rank: Optional[int] = None, imgsz: int = 640, amp_scale: bool = True, ema: bool = False, sync_bn: bool = False,
-                 adam: bool = False):
+                 adam: bool = False, dmff_fp32: Optional[bool] = None):
         hyp = dict(HYP_SCRATCH if hyp is None else hyp)
+        if dmff_fp32 is not None:
+            set_dmff_stream_dtype(model, dmff_fp32)
         det = model.model[-1]
         nl, nc = det.nl, det.nc
         nbs = 64
@@ -367,10 +381,15 @@ class GraphedTrainStep:
     every call never captures it.
 
     DDP (world_size > 1): construct the TrainStep inside ``torch.cuda.stream(side)`` and set TORCH_NCCL_ASYNC_ERROR_HANDLING=0
-    before init_process_group, as torch's CUDA-graph notes require; 11 eager iterations run before the capture."""
+    before init_process_group, as torch's CUDA-graph notes require; 11 eager iterations run before the capture.
 
-    def __init__(self, ts: TrainStep, B: int, H: int, W: int, max_targets: int, device, warmup: Optional[int] = None):
+    dmff_fp32: as TrainStep's, set on the model before the capture; None keeps what the TrainStep set."""
+
+    def __init__(self, ts: TrainStep, B: int, H: int, W: int, max_targets: int, device, warmup: Optional[int] = None,
+                 dmff_fp32: Optional[bool] = None):
         from .autograd import sync_group
+        if dmff_fp32 is not None:
+            set_dmff_stream_dtype(ts.raw_model, dmff_fp32)
         for m in ts.raw_model.modules():           # SyncBatchNorm exchanges are captured like DDP's all-reduces: over NCCL only
             g = sync_group(m)
             if g is not None and torch.distributed.get_backend(g) != "nccl":

@@ -551,6 +551,43 @@ int icaf_cross_attention_bwd(const void* qkv_vis, const void* qkv_ir, const void
 int icaf_axpby(const void* x, const void* y, const float* a, const float* b, void* out, int64_t n, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * fp32 DMFF token streams (training).  Under the reference's autocast a one-element fp32 parameter (LearnableWeights,
+ * LearnableCoefficient) times an fp16 tensor promotes to fp32, so its token streams are fp32 from the pooling to the
+ * upsample-and-add, and so are their gradients; GEMM operands are fp16 (autocast's cast at every Linear).  These entry points
+ * are the fp32-stream forms of the calls above: tokens and token gradients fp32, maps, map gradients, LayerNorm outputs and
+ * branch outputs fp16.  Every reduction keeps the fixed order of its fp16 form (deterministic, no atomics). */
+/* icaf_dmff_pool_tokens with fp32 pos_emb and fp32 tokens: tok = fp32(w1 * fp16(avg)) + fp32(w2 * max) + pos, each step
+ * rounded (no FMA contraction), pad rows 0.  No row statistics. */
+int icaf_dmff_pool_tokens_f32(const void* x_vis, const void* x_ir, int64_t x_ld, const float* pos_vis, const float* pos_ir, const float* mix,
+                              float* tok_vis, float* tok_ir, int B, int H, int W, int C, int nh, int nw, int n_pad, void* stream);
+/* icaf_dmff_pool_tokens_bwd with fp32 token gradients; the map gradients are fp16, accumulated in fp32 and rounded once. */
+int icaf_dmff_pool_tokens_bwd_f32(const void* x_vis, const void* x_ir, int64_t x_ld, const float* dtok_vis, const float* dtok_ir, const float* mix,
+                                  void* dx_vis, void* dx_ir, int B, int H, int W, int C, int nh, int nw, int n_pad, void* workspace,
+                                  size_t workspace_bytes, void* stream);   /* workspace: 2*B*nh*nw*C bytes, 8-byte aligned */
+/* icaf_dmff_upsample_cat in its training mode (nearest) over fp32 tokens: token + map added in fp32, rounded once to the fp16
+ * concat buffer. */
+int icaf_dmff_upsample_cat_f32(const float* tok_vis, const float* tok_ir, int n_pad, const void* x_vis, const void* x_ir, int64_t x_ld,
+                               void* y, int64_t y_ld, int B, int H, int W, int C, int nh, int nw, void* stream);
+/* icaf_dmff_upsample_cat_bwd (nearest) with fp32 token gradients. */
+int icaf_dmff_upsample_cat_bwd_f32(const void* dcat, int64_t d_ld, float* dtok_vis, float* dtok_ir, int B, int H, int W, int C, int nh, int nw,
+                                   int n_pad, void* stream);
+/* icaf_layernorm over fp32 tokens; y fp16 (the fp32 LayerNorm rounded once, as the Linear after it casts it). */
+int icaf_layernorm_f32(const float* x0, const float* x1, const float* g0, const float* b0, const float* g1, const float* b1, void* y0, void* y1,
+                       int64_t rows, int C, float eps, void* stream);
+/* icaf_layernorm_bwd with fp32 x and dx and fp16 dy.  workspace: icaf_train_workspace_bytes(C) + 2 rows floats. */
+int icaf_layernorm_bwd_f32(const float* x, const void* dy, const float* gamma, float* dx, float* dgamma, float* dbeta, int64_t rows, int C,
+                           float eps, float grad_scale, int accumulate, float* workspace, size_t workspace_bytes, void* stream);
+/* out = a[0] * x (+ b[0] * y) with x fp32, y fp16 (or NULL), n % 8 == 0: two rounded products and a rounded sum, torch's fp32
+ * `a * x + b * y` bit for bit.  out is fp16 (rounded once) when out_f16, else fp32. */
+int icaf_axpby_f32(const float* x, const void* y, const float* a, const float* b, void* out, int out_f16, int64_t n, void* stream);
+/* icaf_dot with x fp32 and y fp16 (y_f16) or fp32. */
+int icaf_dot_f32(const float* x, const void* y, int y_f16, int64_t rows, int C, float* out, float scale, int accumulate, float* workspace,
+                 size_t workspace_bytes, void* stream);
+/* icaf_colsum of a dense fp32 (rows, C) matrix; workspace: 64 * C floats. */
+int icaf_colsum_f32(const float* x, int64_t rows, int C, float* out, float scale, int accumulate, float* workspace, size_t workspace_bytes,
+                    void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * Training augmentation of RGB/IR pairs: LoadMultiModalImagesAndLabels.__getitem__ (utils/datasets.py:948-1024) with
  * augment=True -- mosaic (load_mosaic_RGB_IR :1208-1309, resize of load_image_rgb_ir :1097-1125), affine warp
  * (random_perspective_rgb_ir :1535-1630, perspective = 0), HSV jitter (augment_hsv :1129-1141), flipud / fliplr and
